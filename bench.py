@@ -1,5 +1,5 @@
-"""Benchmark of the SC-SfMLearner training hot path (BASELINE.json metric: train-step frames/sec at
-256x832 ResNet-18 on 1/2/4/8 B200; warp-loss HBM GB/s).
+"""Benchmark of the SC-SfMLearner training hot path (train-step frames/sec at 256x832 ResNet-18 on 1/2/4/8 H100;
+warp-loss HBM GB/s).
 
     python bench.py --gpus N --steps K --warmup W [--config kitti_r18|kitti_r50|nyu_r18]     # our arm (torchrun launches N>1)
     python bench.py --impl reference --gpus N --steps K --warmup W                           # the reference's own CPU path
@@ -8,11 +8,17 @@ A "step" is one complete optimisation step (train.py:254-282): 1 + n_ref DispRes
 forward/backward calls, fused photometric/geometry/smoothness losses, gradient all-reduce (N>1), Adam, on a synthetic
 batch (weak scaling: the per-GPU batch is fixed).  One JSON line is printed by rank 0.
 
+Every timed step is the FIRST optimisation step from the same seeded initial state (parameters, Adam moments, BatchNorm
+running statistics are restored between steps, outside the timed events): the work per step is that of any training step,
+and its results are a function of the seeded inputs alone.  Chaining the steps instead would make them a training
+trajectory, along which the rounding-level run-to-run differences of the fp32 atomic reductions (gradient scatters,
+split-K weight gradients) grow to O(1) within a few Adam steps.
+
   config kitti_r18 (default, BASELINE configs 2/3): DispResNet18+PoseResNet18, 256x832, 2 refs, 4 frames per GPU
   config kitti_r50 (BASELINE config 4):             DispResNet50+PoseResNet50, 256x832, 2 refs, 2 frames per GPU
   config nyu_r18   (BASELINE config 5):             DispResNet18+PoseResNet18, 256x320, 1 ref,  8 frames per GPU
 
-`value` is measured in the convolution mode --conv-mode (default tf32x3: the tcgen05 split-accumulate mode that meets
+`value` is measured in the convolution mode --conv-mode (default tf32x3: the wgmma split-accumulate mode that meets
 the 1e-4 parity contract, tests/test_train_step_gpu.py::test_full_size_benchmarked_step_vs_oracle); the single-product
 TF32 figure (cuDNN's default arithmetic) is reported beside it as `tf32`.  Extras in the line: `warp_loss` (CUDA-event
 timed loss kernels as HBM GB/s, metric half 2), `gpu_reference` (the unmodified reference step through stock PyTorch/cuDNN
@@ -57,7 +63,8 @@ def load_peaks():
         d = json.load(open(path))
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"], "tflops_sustained": d["bf16_tflops_sustained"],
                 "source": "MEASURED_PEAKS.json (of measured)"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "B200_PROFILING.md fallback"}
+    # NVIDIA H100 SXM data sheet (700 W part): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -155,7 +162,7 @@ def run_ref_driver(device, config, steps, warmup, threads=0, budget_s=0.0, extra
 
 
 def cpu_oracle_port(cfg, steps, budget_s):
-    """Fallback CPU baseline when baseline/_ref is absent: the oracle port of the step (oracle/step.py)."""
+    """Fallback CPU baseline when oracle/_ref is absent: the oracle port of the step (oracle/step.py)."""
     import time
     from oracle import geometry as OGEO
     from oracle import nets as N
@@ -187,7 +194,7 @@ def cpu_baseline(config, cfg, steps, warmup, budget_s):
     r = run_ref_driver("cpu", config, steps, warmup, threads=cores, budget_s=budget_s)
     if "unavailable" in r:
         base = cpu_oracle_port(cfg, steps, budget_s)
-        base["note"] = "baseline/_ref unavailable (%s): oracle port timed instead" % r["unavailable"]
+        base["note"] = "oracle/_ref unavailable (%s): oracle port timed instead" % r["unavailable"]
         return base
     return {"value": r["frames_per_s"], "unit": "frames/s", "cores": r["threads"], "kind": "reference",
             "sample": "%d timed step(s) (after %d warm-up) of the UNMODIFIED reference train.train() (train.py:235-299, autograd anomaly "
@@ -237,10 +244,10 @@ def input_pipeline_extra(cfg, dev, peaks, iters=20):
            "e2e_frames_per_s": round(B / (ms_e2e * 1e-3), 1), "e2e_ms_per_batch": round(ms_e2e, 4), "h2d_bytes_per_batch": int(frames.size),
            "how": "%d batches of %d samples x %d frames %dx%d; device: CUDA events around the whole call (host draws + 2 small uploads + 2 kernels), "
                   "frames resident; e2e: uint8 frames from pinned host memory, synchronised per batch; algorithmic 15 B/pixel" % (iters, B, n_img, H, W)}
-    ref_dir = os.path.join(ROOT, "baseline", "_ref")
+    ref_dir = os.environ.get("SCSFM_REFERENCE_DIR") or os.path.join(ROOT, "oracle", "_ref")
     try:
         sys.path.insert(0, ref_dir)
-        import custom_transforms as T       # the reference's (baseline/_ref: unmodified copy made by __graft_entry__.install_reference)
+        import custom_transforms as T       # the original project's (oracle/_ref/ or $SCSFM_REFERENCE_DIR)
         chain = T.Compose([T.RandomHorizontalFlip(), T.RandomScaleCrop(), T.ArrayToTensor(), T.Normalize(mean=[0.45] * 3, std=[0.225] * 3)])
         nthreads = torch.get_num_threads()
         torch.set_num_threads(1)
@@ -264,6 +271,24 @@ def input_pipeline_extra(cfg, dev, peaks, iters=20):
     return res
 
 
+DUMP_SAMPLE = 1 << 20          # elements kept per parameter / gradient vector (fixed seeded positions)
+
+
+def dump_outputs(out_dir, losses, trainer):
+    """What the last timed step handed back: its four losses (total, photometric, smoothness, geometry) and the networks'
+    updated parameters and their gradients (the step from the seeded initial state, see the module docstring).  The parameter and gradient vectors are sampled at fixed seeded positions
+    (4 MB each), so two builds run with the same arguments can be compared array by array."""
+    import numpy as np
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "losses.npy"), torch.stack([torch.as_tensor(x).float().reshape(()) for x in losses]).cpu().numpy())
+    for name, net in (("disp", trainer.disp_net), ("pose", trainer.pose_net)):
+        for kind, vec in (("params", net.flat_params()), ("grads", net.flat_grads())):
+            v = vec.detach().float().reshape(-1)
+            idx = np.sort(np.random.default_rng(0).choice(v.numel(), min(DUMP_SAMPLE, v.numel()), replace=False))
+            np.save(os.path.join(out_dir, "%s_%s.npy" % (name, kind)), v[torch.from_numpy(idx).to(v.device)].cpu().numpy())
+
+
 def run_ours(args):
     import models
     from scsfm import lib as L
@@ -282,7 +307,7 @@ def run_ours(args):
     L.load()          # fails loudly if libscsfm.so is missing
     h_tgt, h_refs, h_K = synthetic_batch(cfg, rank, pinned=True)
     d_tgt, d_refs, d_K = h_tgt.to(dev), [r.to(dev) for r in h_refs], h_K.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
     B = cfg["batch"]
 
     def make_trainer(mode, overlap=True):
@@ -297,11 +322,13 @@ def run_ours(args):
             dist.barrier()
         torch.cuda.synchronize()
 
-    def timed(fn, steps):
-        """device time of `steps` calls (L2 flushed before each), max over ranks, in ms"""
+    def timed(fn, steps, before=None):
+        """device time of `steps` calls (L2 flushed before each, after the untimed `before()`), max over ranks, in ms"""
         evs = []
         barrier()
         for _ in range(steps):
+            if before is not None:
+                before()
             flush.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
@@ -359,6 +386,12 @@ def run_ours(args):
     L.PROF.update(enabled=False, only=None, events=[])
     del trainer
     trainer = make_trainer(args.conv_mode)
+    initial = trainer.optimizer.snapshot()       # the state every timed step starts from
+
+    def reset_state():
+        trainer.optimizer.restore(initial)
+        for n in trainer.optimizer.nets:         # the TF32 operand mirrors of the restored parameters
+            n.refresh_operand_weights()
     for _ in range(2):
         trainer.step(d_tgt, d_refs, d_K)
 
@@ -385,8 +418,14 @@ def run_ours(args):
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    ms = timed(lambda: trainer.step(d_tgt, d_refs, d_K), args.steps)
+    last = []
+
+    def timed_step():
+        last[:] = [trainer.step(d_tgt, d_refs, d_K)]
+    ms = timed(timed_step, args.steps, before=reset_state)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0], trainer)
     launches = trainer.launches_per_step * args.steps if graphed else (L.launch_count() - launches0)
 
     # ---- end to end: pinned host inputs copied in, loss read back, every step ----------------------
@@ -477,7 +516,7 @@ def run_ours(args):
     if tf32_extra is not None:
         line["tf32"] = tf32_extra
     if world == 1 and not args.no_gpu_reference:
-        # the "existing Blackwell kernel" bar (SURVEY.md 2.3, BASELINE.md 3): the UNMODIFIED reference step through stock
+        # the stock-library bar: the UNMODIFIED reference step through stock
         # PyTorch/cuDNN on this same GPU, as shipped (cudnn.benchmark on, TF32 convolutions allowed, anomaly mode on) and with
         # anomaly mode off
         torch.cuda.empty_cache()
@@ -487,7 +526,7 @@ def run_ours(args):
             r = run_ref_driver("cuda", args.config, max(5, min(args.steps, 20)), 3, extra=extra, timeout=600)
             gref[name] = r if "unavailable" in r else {"frames_per_s": r["frames_per_s"], "ms_per_step": r["ms_per_step"], "steps": r["steps"],
                                                        "tf32": r["tf32"], "anomaly": r["anomaly"]}
-        gref["what"] = ("unmodified reference train.train() (baseline/_ref, stock torch %s / cuDNN, cudnn.benchmark=True) on the same B200, "
+        gref["what"] = ("unmodified reference train.train() (oracle/_ref, stock torch %s / cuDNN, cudnn.benchmark=True) on the same GPU, "
                         "wall clock per iteration incl. its own host syncs and CSV write; inputs resident on the host as in train.py:254-257"
                         % torch.__version__)
         line["gpu_reference"] = gref
@@ -547,8 +586,8 @@ def main():
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--config", choices=sorted(CONFIGS), default="kitti_r18")
     ap.add_argument("--conv-mode", choices=["fp32", "tf32", "tf32x3"], default="tf32x3",
-                    help="tf32x3 = tcgen05 convolutions with split-accumulate operands (fp32-level, the 1e-4 parity mode; default); "
-                         "tf32 = tcgen05 single TF32 product (cuDNN's default arithmetic); fp32 = exact CUDA-core convolutions")
+                    help="tf32x3 = wgmma convolutions with split-accumulate operands (fp32-level, the 1e-4 parity mode; default); "
+                         "tf32 = wgmma single TF32 product (cuDNN's default arithmetic); fp32 = exact CUDA-core convolutions")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-tf32-extra", action="store_true")
@@ -556,6 +595,9 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="time the eager step instead of the CUDA-graph replay")
     ap.add_argument("--overlap-wgrad", type=int, default=1, help="1 (default): weight gradients on a side stream per network (Trainer(overlap_wgrad=True))")
     ap.add_argument("--overlap-nets", type=int, default=1, help="1 (default): PoseResNet on a side stream next to DispResNet (Trainer(overlap_nets=True))")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's losses and a fixed sample of the updated parameters and "
+                         "their gradients as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * scsfm.h -- C ABI of libscsfm.so: hand-written sm_100a kernels for the SC-SfMLearner
+ * scsfm.h -- C ABI of libscsfm.so: hand-written sm_90a kernels for the SC-SfMLearner
  * training hot path (SURVEY.md section 8).
  *
  * The reference (JiawangBian/SC-SfMLearner-Release) is pure Python and has no FFI of its
@@ -178,7 +178,7 @@ typedef struct ScsfmConv {
     /* Split-accumulate ("3xTF32") operands of the tensor-core entry points, each optional (NULL = plain TF32):
      * X_lo = tf32(X - trunc_tf32(X)) of the matching tensor (scsfm_split_tf32).  kind::tf32 reads only the upper 19 bits
      * of an fp32 operand, so the raw tensor IS the high part; with the low parts given the kernel accumulates
-     * hi*hi + lo*hi + hi*lo into the same TMEM accumulator (the dropped lo*lo term is 2^-22 relative), which restores
+     * hi*hi + lo*hi + hi*lo into short fp32 accumulation chains (the dropped lo*lo term is 2^-22 relative), which restores
      * fp32-level accuracy of the products (cuDNN's/torch's "highest" matmul precision on the same hardware).
      *   fwd:   in_lo, w_lo      dgrad: dout_lo, w_lo (flipped like w)      wgrad: in_lo, dout_lo */
     const float* in_lo;
@@ -195,14 +195,14 @@ typedef struct ScsfmConv {
 #define SCSFM_TUNE_MT(mt) (((unsigned)(mt) & 3u) << 4)       /* TMA kernel: 1|2 stacked 128-pixel sub-tiles (0 = auto) */
 #define SCSFM_TUNE_TW(l2) (((unsigned)((l2) ? (l2) - 2 : 0) & 3u) << 6)   /* TMA kernel: tile width log2 3|4 (0 = auto) */
 #define SCSFM_TUNE_BN(bn) (((bn) == 16 ? 1u : (bn) == 32 ? 2u : (bn) == 64 ? 3u : (bn) == 128 ? 4u : 0u) << 8)  /* weight rows in smem */
-#define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 cp.async kernel, 2 TMA kernel, 3 thin-layer fp32 kernel */
+#define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 or 2 tensor-core kernel, 3 thin-layer fp32 kernel */
 
 /* Exact-fp32 implicit-GEMM convolution on CUDA cores (every shape). */
 int scsfm_conv2d_fwd_simt(const ScsfmConv* p, void* stream);
 int scsfm_conv2d_dgrad_simt(const ScsfmConv* p, void* stream);
 int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream);
 
-/* tcgen05 (kind::tf32, fp32 accumulation in TMEM) implicit-GEMM convolution; needs Cin % 4 == 0.
+/* wgmma (tf32 operands, fp32 accumulation in registers) implicit-GEMM convolution; needs Cin % 4 == 0.
  * dgrad_tc: stride 1 or 2; p->w must hold the flipped/transposed weights [Cin,kh,kw,Cout] produced by
  * scsfm_weight_flip (the data gradient is the forward kernel run on dout). */
 /* Stride-1 (sub-)convolutions with kh, kw <= 3 run the TMA halo-patch kernel (conv_tma.cu: one 4-D tiled TMA load

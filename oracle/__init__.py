@@ -9,8 +9,8 @@ reference` leg do.
 
 Parity status: PINNED.  The reference holds no golden vectors or tests of its own
 (SURVEY.md section 4), so the oracle is pinned against the reference code itself:
-`tests/golden/make_golden.py` imports the unmodified reference from /root/reference
-in the build container, runs it on seeded inputs and commits the input/output
+`tests/golden/make_golden.py` imports the unmodified reference from a checkout of the
+original project, runs it on seeded inputs and commits the input/output
 vectors under `tests/golden/`; `tests/test_oracle_golden.py` checks every oracle
 function against those vectors.  Third-party arithmetic the reference relies on
 (`F.grid_sample`, `avg_pool2d`, `ReflectionPad2d`, torchvision ResNet, Adam: PyTorch

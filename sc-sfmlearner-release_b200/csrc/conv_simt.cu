@@ -2,7 +2,7 @@
 //
 // This is the exact-fp32 ("parity") path for every conv shape of DispResNet / PoseResNet
 // (SURVEY.md appendix A) and the production path for the layers that are too thin for the
-// tcgen05 kernels (7x7 stem with Cin 3/6, Cout 1/6 heads).  Activations are NHWC, weights
+// tensor-core kernels (7x7 stem with Cin 3/6, Cout 1/6 heads).  Activations are NHWC, weights
 // [Cout][kh][kw][Cin] (K-major), so the GEMM K index runs over (tap, channel) with channels
 // contiguous: every operand fetch is a 16-byte load.
 //
@@ -471,7 +471,7 @@ int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStrea
     if ((C & 3) == 0 && gpr <= 64 && (gpr & (gpr - 1)) == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0) {
         const long long nvec = (long long)rows * gpr;
         long long ctas = (nvec + 8 * CT - 1) / (8 * CT);          // >= 8 float4 per thread
-        if (ctas > 148 * 8) ctas = 148 * 8;
+        if (ctas > 132 * 8) ctas = 132 * 8;
         if (ctas < 1) ctas = 1;
         bias_grad_vec_kernel<<<(int)ctas, CT, 0, st>>>(dout, nvec, gpr, dbias);
         SCSFM_CHECK_LAUNCH();
@@ -536,7 +536,7 @@ extern "C" int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream) {
     }
     auto plan = [&](int bm, int bn, dim3& grid, int& kps) {
         const int tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-        int splits = (148 * 4 + tiles - 1) / tiles;
+        int splits = (132 * 4 + tiles - 1) / tiles;
         const int max_splits = (Kall + 511) / 512;
         if (splits > max_splits) splits = max_splits;
         if (splits < 1) splits = 1;

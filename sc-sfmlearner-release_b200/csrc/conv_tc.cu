@@ -1,16 +1,17 @@
-// Implicit-GEMM convolution on the 5th-generation tensor cores (tcgen05, kind::tf32, fp32 accumulate in TMEM).
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma, tf32 operands, fp32 accumulation in registers).
 //
 //   C[M = B*Ho*Wo, N = Cout] = A[M, K = kh*kw*Cin] (im2col gather of the NHWC input) x W[N, K]^T
 //
-// CTA = one 128 x BN output tile, 5 warps:
-//   warps 0-3  producers: gather 128 x 32-float A slices (any stride / zero or reflection padding) and BN x 32 W
-//              slices with 16-byte loads, write them into the 128B-swizzled K-major layout the UMMA descriptors
-//              expect, fence.proxy.async, arrive on the stage's "full" mbarrier; afterwards they are the epilogue
-//              (tcgen05.ld 32x32b -> bias / activation / residual addend / BatchNorm partial sums -> 16B stores)
-//   warp 4     allocates TMEM, one elected lane issues 4 x tcgen05.mma (M128 x BN x K8) per stage and
-//              tcgen05.commit's to the stage's "empty" mbarrier / the accumulator-ready mbarrier.
+// CTA = one 64 x BN output tile, 8 warps:
+//   warps 0-3  producers: gather 64 x 32-float A slices (any stride / zero or reflection padding) with 16-byte cp.async
+//              into the 128B-swizzled K-major layout the wgmma descriptors expect (completion on the stage's "full"
+//              mbarrier); thread 0 also issues the BN x 32 weight slice as one TMA box
+//   warps 4-7  one consumer warpgroup: 4 x wgmma (M64 x BN x K8) per stage, accumulators in registers, stage released
+//              on its "empty" mbarrier once the wgmma that read it have retired
+//   afterwards all 8 warps are the epilogue (accumulator tile through shared memory -> bias / activation / residual
+//   addend / BatchNorm partial sums -> 16B stores).
 // A software gather is used instead of TMA-im2col because the same loader folds in reflection padding and the
-// transposed-convolution view used for the data gradient; the tile still never touches registers twice.
+// transposed-convolution view used for the data gradient.
 //
 // dgrad (stride 1) is the same kernel run on dout with flipped/transposed weights (weight_flip_kernel below);
 // for reflection-padded layers it returns the gradient of the padded tensor (pad' = 2), folded afterwards.
@@ -21,6 +22,44 @@
 #include "conv_tc.cuh"
 
 namespace scsfm {
+
+// Consumer warpgroup of the gather kernels: waits for each stage, runs its 4 wgmma (K = 8 each) into the chain accumulator
+// `part`, releases the stage once those wgmma have retired, and adds `part` into `acc` (fp32, round-to-nearest) at the end
+// of every chain of `chain` k-blocks.  A stage is [GBM rows][32 floats] of A followed by [BN rows][32 floats] of B.
+template <int BN, int STAGES, int A_BYTES, int B_BYTES>
+__device__ __forceinline__ void gather_consume(float (&acc)[BN / 2], uint8_t* sA, uint8_t* sB, uint64_t* bar_full, uint64_t* bar_empty,
+                                               int total, int chain) {
+    float part[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int pend = -1;                                       // stage whose wgmma group may still be in flight
+    for (int it = 0; it < total; ++it) {
+        const int s = it % STAGES;
+        tc::mbar_wait(bar_full + s, (it / STAGES) & 1);
+        tc::fence_proxy_async();                         // cp.async / st.shared (generic proxy) writes -> wgmma (async proxy) reads
+        const uint32_t a_addr = tc::smem_u32(sA + s * A_BYTES), b_addr = tc::smem_u32(sB + s * B_BYTES);
+        const bool first = it % chain == 0;
+        tc::reg_fence(part);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < TBK / 8; ++j)
+            tc::wgmma_tf32<BN>(part, tc::make_desc_sw128(a_addr + j * 32), tc::make_desc_sw128(b_addr + j * 32), (first && j == 0) ? 0u : 1u);
+        tc::wgmma_commit();
+        if (it % chain == chain - 1 || it == total - 1) {
+            tc::wgmma_wait<0>();
+            tc::reg_fence(part);
+            if (pend >= 0) tc::mbar_arrive(bar_empty + pend);
+            tc::mbar_arrive(bar_empty + s);
+            pend = -1;
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        } else {
+            tc::wgmma_wait<1>();                         // the previous stage's group has retired
+            if (pend >= 0) tc::mbar_arrive(bar_empty + pend);
+            pend = s;
+        }
+    }
+}
 
 // STACK = true (split mode, Cout <= BN / 2): the weight tile holds W in rows [0, BN/2) and lo(W) in rows [BN/2, BN), so the two
 // passes lo(in) and in give all four products (accumulator columns n and BN/2 + n are added in the epilogue): 2 passes, not 3.
@@ -33,53 +72,44 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;
     uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
-    uint64_t* bar_full = reinterpret_cast<uint64_t*>(sB + STAGES * Cfg::B_STAGE_BYTES);
+    uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + (Cfg::OPERANDS > Cfg::EPI ? Cfg::OPERANDS : Cfg::EPI));
     uint64_t* bar_empty = bar_full + STAGES;
-    uint64_t* bar_acc = bar_empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_acc + 1);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rows_per_img = v.border ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo;
     const int M = p.B * rows_per_img, N = p.Cout, K = v.kh * v.kw * p.Cin;
-    const int m0 = blockIdx.x * TBM, n0 = blockIdx.y * BN;
+    const int m0 = blockIdx.x * GBM, n0 = blockIdx.y * BN;
     const int KB = (K + TBK - 1) / TBK;
     // split-accumulate passes over the whole K range (ScsfmConv.in_lo / w_lo): raw x raw, lo(in) x raw(w), raw(in) x lo(w)
     const int npass = STACK ? 2 : 1 + (p.in_lo != nullptr ? 1 : 0) + (p.w_lo != nullptr ? 1 : 0);
-    // round-robin accumulators only in split mode (plain TF32 is bounded by its operand rounding: one accumulator, fewer TMEM
-    // columns, more resident CTAs)
-    const int nacc_rt = npass > 1 ? Cfg::NACC : 1;
-    const uint32_t tmem_cols = (uint32_t)(nacc_rt * Cfg::ACC_COLS);
+    const int chain = npass > 1 ? CHAIN_KB : KB * npass;
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) {
             tc::mbar_init(bar_full + s, FW_PWARPS * 32 + 1);      // cp.async arrivals (activations) + 1 expect_tx arrival (weights, TMA)
-            tc::mbar_init(bar_empty + s, 1);
+            tc::mbar_init(bar_empty + s, 128);                    // every thread of the consumer warpgroup
         }
-        tc::mbar_init(bar_acc, 1);
         tc::fence_barrier_init();
         tc::tma_prefetch_desc(&wmap);
         if (p.w_lo != nullptr) tc::tma_prefetch_desc(&wmap_lo);
     }
-    if (warp == FW_PWARPS) tc::tmem_alloc(tmem_slot, tmem_cols);
-    tc::fence_before_thread_sync();
     __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem_base = *tmem_slot;
+    float acc[BN / 2];
 
     if (warp < FW_PWARPS) {
         // ------------------------------------------------------------------ producers
         // Per k-block every thread fetches 4 A chunks (16 B each); the BN x 32 weight slice is one TMA box.  The loop is software-pipelined:
         // the loads of k-block kb+1 are in flight while k-block kb is written to shared memory, all addressing is
         // 32-bit offset arithmetic and out-of-image taps are handled without branches (clamped address + select).
-        constexpr int ROWS = TBM / (FW_PWARPS * 4);    // A rows per thread (4): rows r0 + 32*i
+        constexpr int ROWS = GBM / (FW_PWARPS * 4);    // A rows per thread (4): rows r0 + 16*i
         const int c = tid & 7;               // 16-byte chunk column inside the 128-byte row
-        const int r0 = tid >> 3;             // 0..31
-        const int cs = c ^ (r0 & 7);         // 128B swizzle: chunk ^= row % 8 (rows r0+32i share row % 8)
+        const int r0 = tid >> 3;             // 0..15
+        const int cs = c ^ (r0 & 7);         // 128B swizzle: chunk ^= row % 8 (rows r0+16i share row % 8)
         const bool reflect = p.pad_mode == PADMODE_REFLECT;
         int hi0[ROWS], wi0[ROWS], rbase[ROWS];   // first-tap input coordinates and the image offset of each row
 #pragma unroll
         for (int i = 0; i < ROWS; ++i) {
-            const int m = m0 + r0 + 32 * i;
+            const int m = m0 + r0 + 16 * i;
             if (m < M) {
                 const int b = m / rows_per_img, rem = m - b * rows_per_img;
                 int ho, wo;
@@ -99,7 +129,7 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
         int kc, dy, dx, ch;
         // Asynchronous copies (cp.async / LDGSTS, 16 B, zero-fill for out-of-image taps): no register staging, so the
         // loads of all pipeline stages are in flight at once; the stage's "full" mbarrier gets this thread's arrival
-        // when its copies have landed (cp.async.mbarrier.arrive.noinc).  The MMA thread issues fence.proxy.async after
+        // when its copies have landed (cp.async.mbarrier.arrive.noinc).  The consumers issue fence.proxy.async after
         // waiting on the barrier to order these generic-proxy writes before the tensor core's async-proxy reads.
         // Row offsets / validity only change with the tap, i.e. every Cin/32 k-blocks: they are cached in between.
         int aoff[ROWS];
@@ -156,7 +186,7 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
 #pragma unroll
             for (int i = 0; i < ROWS; ++i) {
                 const bool ok = kok && ((okm >> i) & 1u);
-                tc::cp_async_16(a_st + i * 4096, a_base + (ok ? aoff[i] + ch : 0), ok ? 16u : 0u);
+                tc::cp_async_16(a_st + i * 2048, a_base + (ok ? aoff[i] + ch : 0), ok ? 16u : 0u);
             }
             tc::cp_async_arrive_noinc(bar_full + s);
             // advance this thread's K index by one k-block
@@ -168,11 +198,30 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
             }
         }
         }
+    } else {
+        // ------------------------------------------------------------------ consumer warpgroup (warps 4-7)
+        gather_consume<BN, STAGES, A_STAGE_BYTES, Cfg::B_STAGE_BYTES>(acc, sA, sB, bar_full, bar_empty, KB * npass, chain);
+    }
 
-        // ------------------------------------------------------------------ epilogue (same 4 warps)
-        tc::mbar_wait(bar_acc, 0);
-        tc::fence_after_thread_sync();
-        const int quarter = warp & 3, half = warp >> 2;      // TMEM lane quarter / which half of the column chunks
+    // ------------------------------------------------------------------ epilogue (all 8 warps)
+    // every wgmma has retired and every cp.async / TMA write has landed: the operand ring is free for the accumulator tile
+    __syncthreads();
+    constexpr int TS = BN + 1;                                // tile row stride (odd: conflict-free column reads)
+    float* T = reinterpret_cast<float*>(smem);
+    if (warp >= FW_PWARPS) {
+        const int t = tid - FW_PWARPS * 32;
+        const int r = 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+            T[r * TS + 8 * i + c] = acc[4 * i];
+            T[r * TS + 8 * i + c + 1] = acc[4 * i + 1];
+            T[(r + 8) * TS + 8 * i + c] = acc[4 * i + 2];
+            T[(r + 8) * TS + 8 * i + c + 1] = acc[4 * i + 3];
+        }
+    }
+    __syncthreads();
+    {
+        const int quarter = warp & 1, half = warp >> 1;      // 32-row group of the tile / which quarter of the column chunks
         const int m = m0 + quarter * 32 + lane;
         const bool row_ok = m < M;
         size_t out_row = (size_t)m;          // row of the output / addend tensors
@@ -183,36 +232,25 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
             else { ho = rem / p.Wo; wo = rem - ho * p.Wo; }
             out_row = ((size_t)b * v.out_H + (ho * v.out_sy + v.out_oy)) * v.out_W + (wo * v.out_sx + v.out_ox);
         }
-        float* stage = reinterpret_cast<float*>(sA) + warp * (32 * 33);    // all MMAs retired: operand smem is free
+        float* stage = T + GBM * TS + warp * (32 * 33);
         constexpr int CREAL = STACK ? BN / 2 : BN;                // accumulator columns holding output channels
         constexpr int CW = CREAL < 32 ? CREAL : 32;
-        const int nacc = min(nacc_rt, KB * npass);              // accumulators that received at least one k-block
         constexpr int NCH = CREAL / CW;                           // column chunks of real output channels
+        const float* trow = T + (quarter * 32 + lane) * TS;
 #pragma unroll 1
-        for (int cc = half; cc < NCH; cc += FW_PWARPS / 4) {
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(cc * CW);
-            if (CW == 32) tc::tmem_ld32(taddr, r);
-            else tc::tmem_ld16(taddr, r);
-            tc::tmem_ld_wait();
-            // the round-robin partial accumulators (and, stacked, the lo(W) columns BN/2 further on), added in fp32 (RN)
-            for (int a = 0; a < nacc; ++a) {
-                for (int h = 0; h < (STACK ? 2 : 1); ++h) {
-                    if (a == 0 && h == 0) continue;
-                    uint32_t q[32];
-                    const uint32_t src = taddr + (uint32_t)(a * Cfg::ACC_COLS + h * (BN / 2));
-                    if (CW == 32) tc::tmem_ld32(src, q);
-                    else tc::tmem_ld16(src, q);
-                    tc::tmem_ld_wait();
+        for (int cc = half; cc < NCH; cc += (FW_PWARPS + 4) / 2) {
+            float r[32];
 #pragma unroll
-                    for (int j = 0; j < CW; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(q[j]));
-                }
+            for (int j = 0; j < CW; ++j) r[j] = trow[cc * CW + j];
+            if (STACK) {                                          // + the lo(W) products in columns BN/2 further on (fp32, RN)
+#pragma unroll
+                for (int j = 0; j < CW; ++j) r[j] += trow[BN / 2 + cc * CW + j];
             }
             float v[32];
 #pragma unroll
             for (int j = 0; j < CW; ++j) {
                 const int n = n0 + cc * CW + j;
-                float x = __uint_as_float(r[j]);
+                float x = r[j];
                 if (row_ok && n < N) {
                     if (p.bias) x += __ldg(p.bias + n);
                     if (p.addend) x += __ldg(p.addend + out_row * N + n);
@@ -251,7 +289,7 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
                     int g_cur = row_base / rows_per_group;
                     int next_edge = (g_cur + 1) * rows_per_group - row_base;      // first row index of the next group
                     // fp64 accumulation: var = E[x^2] - mean^2 cancels catastrophically when |mean| >> std, so the
-                    // partial sums must not carry fp32 rounding (B200 issues DFMA at half the FFMA rate: negligible here)
+                    // partial sums must not carry fp32 rounding (a handful of DFMA per output value: negligible here)
                     double s1 = 0.0, s2 = 0.0;
                     for (int rr = 0; rr <= 32; ++rr) {
                         if (rr == 32 || rr == next_edge) {
@@ -273,34 +311,7 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
                 __syncwarp();
             }
         }
-    } else {
-        // ------------------------------------------------------------------ MMA issuer (warp 4)
-        constexpr uint32_t idesc = tc::make_idesc_tf32(TBM, BN, 0, 0);
-        if (lane == 0) {                                 // one thread waits, issues and commits
-            for (int kb = 0; kb < KB * npass; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t ph = (kb / STAGES) & 1;
-                tc::mbar_wait(bar_full + s, ph);
-                tc::fence_proxy_async();                 // cp.async (generic proxy) writes -> UMMA (async proxy) reads
-                tc::fence_after_thread_sync();
-                const uint32_t a_addr = tc::smem_u32(sA + s * A_STAGE_BYTES);
-                const uint32_t b_addr = tc::smem_u32(sB + s * Cfg::B_STAGE_BYTES);
-#pragma unroll
-                for (int j = 0; j < TBK / 8; ++j) {
-                    const uint64_t da = tc::make_smem_desc(a_addr + j * 32, 16, 1024, tc::LAYOUT_SW128);
-                    const uint64_t db = tc::make_smem_desc(b_addr + j * 32, 16, 1024, tc::LAYOUT_SW128);
-                    tc::mma_tf32(tmem_base + (uint32_t)((kb % nacc_rt) * Cfg::ACC_COLS), da, db, idesc, (kb >= nacc_rt || j != 0) ? 1u : 0u);
-                }
-                tc::mma_commit(bar_empty + s);           // frees the stage once these MMAs have read it
-            }
-            tc::mma_commit(bar_acc);                     // accumulator complete
-        }
-        __syncwarp();
     }
-
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == FW_PWARPS) tc::tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // w [Co][kh][kw][Ci] -> wt [Ci][jh][jw][Co] with wt[c][jy][jx][o] = w[o][dy_max - step*jy][dx_max - step*jx][c]:
@@ -323,30 +334,23 @@ __global__ void weight_flip_kernel(const float* __restrict__ w, int Co, int kh, 
 
 // ---------------------------------------------------------------------------------------------------------
 // weight gradient on the tensor cores:  dW^T[(tap,c), o] += sum_pix  in[pix (+) tap, c] * dout[pix, o]
-//   GEMM  M = kh*kw*Cin (gathered input, "MN-major": channels contiguous),  N = Cout (dout, "MN-major"),
-//   K = B*Ho*Wo pixels, split over gridDim.z; partial tiles are added into dw with fp32 atomics.
-// Both operands are MN-major (channels contiguous).  For 32-bit MN-major operands the only shared-memory layout the
-// UMMA unit accepts is SWIZZLE_128B_BASE32B (layout type 1): atom = 4 pixels (K) x 32 channels (128-byte rows),
-// 32-byte chunks XOR-swizzled with (pixel % 4); atoms along M/N at LBO = 512 B, 4-pixel groups at SBO.  One
-// tcgen05.mma (K = 8 for tf32) therefore consumes two pixel groups.
+//   GEMM  M = kh*kw*Cin (gathered input),  N = Cout (dout),  K = B*Ho*Wo pixels, split over gridDim.z; partial tiles are
+//   added into dw with fp32 atomics.
+// Both tensors are channel-contiguous ("MN-major" for this GEMM), but wgmma takes 32-bit operands only K-major.  So the
+// producers load 16-byte channel vectors into registers and store them transposed into the 128B-swizzled K-major stage
+// ([row = (tap,c) or o][32 pixels]); lane = pixel, so every scalar store of a warp hits 32 different banks.
 // ---------------------------------------------------------------------------------------------------------
 template <int BN>
 struct WgCfg {
-    static constexpr int STAGES = 3;
-    static constexpr int A_BYTES = 32 * TBM * 4;        // 32 pixels x 128 (tap,c)
-    static constexpr int B_BYTES = 32 * BN * 4;         // 32 pixels x BN output channels
-    static constexpr int NACC = BN >= 128 ? 1 : (BN >= 64 ? 2 : 4);      // round-robin accumulators (see TcCfg); 3 CTAs per SM fit
-    static constexpr int ACC_COLS = BN < 32 ? 32 : BN;
-    static constexpr int TMEM_COLS = NACC * ACC_COLS;   // 128
+    static constexpr int STAGES = 4;
+    static constexpr int A_BYTES = GBM * 128;           // 64 (tap,c) rows x 32 pixels
+    static constexpr int B_BYTES = BN * 128;            // BN output channels x 32 pixels
     static constexpr size_t SMEM = 1024 + (size_t)STAGES * (A_BYTES + B_BYTES) + 256;
 };
 
-// BORDER = true (used after the zero-padding TMA weight-gradient kernel on a reflection-padded layer): the K dimension only
-// runs over the 2*(Ho+Wo)-4 border pixels of every image and only the taps that fall OUTSIDE the image contribute, read
-// at their reflected positions -- exactly the part of the gradient the zero-padded pass left out.
-// STACK = true (split mode, Cout <= BN / 2): the N-side tile holds dout in columns [0, BN/2) and lo(dout) in [BN/2, BN), so the two
+// STACK = true (split mode, Cout <= BN / 2): the N-side tile holds dout in rows [0, BN/2) and lo(dout) in [BN/2, BN), so the two
 // passes lo(in) and in give all four products (columns o and BN/2 + o are both added into dw[o]): 2 passes instead of 3.
-template <int BN, bool BORDER = false, bool STACK = false>
+template <int BN, bool STACK = false>
 __global__ void __launch_bounds__(FW_THREADS)
 conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split) {
     using Cfg = WgCfg<BN>;
@@ -357,187 +361,142 @@ conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split) {
     uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
     uint64_t* bar_full = reinterpret_cast<uint64_t*>(sB + STAGES * Cfg::B_BYTES);
     uint64_t* bar_empty = bar_full + STAGES;
-    uint64_t* bar_acc = bar_empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_acc + 1);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int nb = BORDER ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo;        // K pixels per image
-    const int Mtot = p.kh * p.kw * p.Cin, N = p.Cout, npix = p.B * nb;
-    const int m0 = blockIdx.x * TBM, n0 = blockIdx.y * BN;
+    const int HWo = p.Ho * p.Wo;
+    const int Mtot = p.kh * p.kw * p.Cin, N = p.Cout, npix = p.B * HWo;
+    const int m0 = blockIdx.x * GBM, n0 = blockIdx.y * BN;
     const int pix_begin = blockIdx.z * pix_per_split, pix_end = min(npix, pix_begin + pix_per_split);
     const int KB = (pix_end - pix_begin + 31) / 32;
     if (KB <= 0) return;
     // split-accumulate passes over the CTA's pixel range (ScsfmConv.in_lo / dout_lo): raw x raw, lo(in) x raw(dout), raw(in) x lo(dout)
     const int npass = STACK ? 2 : 1 + (p.in_lo != nullptr ? 1 : 0) + (p.dout_lo != nullptr ? 1 : 0);
-    const int nacc_rt = npass > 1 ? Cfg::NACC : 1;            // round-robin accumulators only in split mode
-    const uint32_t tmem_cols = (uint32_t)(nacc_rt * Cfg::ACC_COLS);
+    const int chain = npass > 1 ? CHAIN_KB : KB * npass;
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) {
             tc::mbar_init(bar_full + s, FW_PWARPS * 32);
-            tc::mbar_init(bar_empty + s, 1);
+            tc::mbar_init(bar_empty + s, 128);
         }
-        tc::mbar_init(bar_acc, 1);
         tc::fence_barrier_init();
     }
-    if (warp == FW_PWARPS) tc::tmem_alloc(tmem_slot, tmem_cols);
-    tc::fence_before_thread_sync();
     __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp < FW_PWARPS) {
         // ------------------------------------------------------------------ producers
-        // A: chunk c4 = tid % 32 (4 consecutive (tap,c) entries, fixed for the whole kernel) x PPT CONSECUTIVE pixels
-        // starting at PPT * (tid / 32): a warp reads 512 contiguous bytes per pixel, and stepping to the next pixel is
-        // one add (+ a rare row wrap).  cp.async with zero-fill, completion on the stage's mbarrier.
-        constexpr int PPT = 32 / FW_PWARPS;                   // pixels per thread per k-block (4)
-        const int c4 = tid & 31, kq = tid >> 5;              // kq: which group of PPT pixels of the 32-pixel k-block
-        const int mm = m0 + 4 * c4;
-        const bool a_ok = mm < Mtot;
-        int a_dy = 0, a_dx = 0, a_ch = 0;
-        if (a_ok) {
-            const int tap = mm / p.Cin;
-            a_ch = mm - tap * p.Cin;
-            a_dy = tap / p.kw - p.pad;
-            a_dx = tap - (tap / p.kw) * p.kw - p.pad;
-        }
+        // Thread (warp w, lane l) handles pixel l of every 32-pixel k-block: A channel chunks w, w + 4, ... (4 (tap,c) rows
+        // each) and B chunks the same way.  The pixel's coordinates advance by 32 per k-block.
+        constexpr int A_IT = GBM / 4 / FW_PWARPS;            // A chunks per thread and k-block (4)
+        constexpr int B_IT = BN / 4 / FW_PWARPS;             // B chunks per thread and k-block (1 .. 8)
         const bool reflect = p.pad_mode == PADMODE_REFLECT;
-        // smem byte offsets of this thread's 8 A chunks inside a stage: pixel k = 8*kq + i -> group k/4, row k%4
-        const uint32_t a_smem = tc::smem_u32(sA) + (uint32_t)((c4 >> 3) * 512);
-        const int a_chunk = c4 & 7;
-        // B: BN/4 chunks per pixel row
-        constexpr int BCH = BN / 4;                          // chunks per row: 8, 16 or 32
-        constexpr int B_IT = (32 * BCH) / (FW_PWARPS * 32);  // per-thread chunk loads: 1, 2, 4
-        constexpr int B_STEP = (FW_PWARPS * 32) / BCH;       // pixel-row step between a thread's B chunks
-        const int b_c4 = tid % BCH, b_kr0 = tid / BCH;
-        // stacked: chunk columns >= BN/2 read lo(dout) at channel (column - BN/2)
-        const bool b_lo_half = STACK && 4 * b_c4 >= BN / 2;
-        const int nn = STACK ? (4 * b_c4 - (b_lo_half ? BN / 2 : 0)) : n0 + 4 * b_c4;
-        const bool b_ok = nn < N;
-        const uint32_t b_smem = tc::smem_u32(sB) + (uint32_t)((b_c4 >> 3) * 512);
-        // pixel (b, ho, wo) of this thread's first A row in the current k-block, advanced by 32 per block
-        int pb, pho, pwo;
-        int it = 0;                                  // k-block counter across the passes: stage = it % STAGES
-        for (int q = 0; q < npass; ++q) {
-        const int ps = (q + 1) % npass;              // low-part passes first (added while the accumulators are small), raw x raw last
-        const float* a_base = (ps == 1 && p.in_lo != nullptr) ? p.in_lo : p.in;
-        const float* b_base = STACK ? (b_lo_half ? p.dout_lo : p.dout)
-                                    : ((ps == npass - 1 && ps > 0 && p.dout_lo != nullptr) ? p.dout_lo : p.dout);
-        {
-            const int px = pix_begin + PPT * kq;
-            pb = px / (p.Ho * p.Wo);
-            const int rem = px - pb * p.Ho * p.Wo;
-            pho = rem / p.Wo;
-            pwo = rem - pho * p.Wo;
-        }
-        int pix0 = pix_begin;
-        for (int kb = 0; kb < KB; ++kb, ++it) {
-            const int s = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            if (lane == 0) tc::mbar_wait(bar_empty + s, ph ^ 1);
-            __syncwarp();
-            const uint32_t a_st = a_smem + (uint32_t)(s * Cfg::A_BYTES), b_st = b_smem + (uint32_t)(s * Cfg::B_BYTES);
-            int b = pb, ho = pho, wo = pwo;
+        int a_dy[A_IT], a_dx[A_IT], a_ch[A_IT];
 #pragma unroll
-            for (int i = 0; i < PPT; ++i) {
-                const int k = PPT * kq + i;                 // pixel row inside the block: group k/4, row k%4
-                const int px = pix0 + k;
-                bool ok = a_ok && px < pix_end;
-                if (BORDER) {
-                    // k-th border pixel of the block; only taps leaving the image count, at their mirrored position
-                    b = px / nb;
-                    border_pixel(px - b * nb, p.Ho, p.Wo, ho, wo);
-                }
-                int hi = ho * p.stride + a_dy, wi = wo * p.stride + a_dx;
-                if (BORDER) {
-                    ok = ok && !((unsigned)hi < (unsigned)p.Hi && (unsigned)wi < (unsigned)p.Wi);
-                    hi = reflect_index(hi, p.Hi); wi = reflect_index(wi, p.Wi);
-                } else if (reflect) { hi = reflect_index(hi, p.Hi); wi = reflect_index(wi, p.Wi); }
+        for (int i = 0; i < A_IT; ++i) {
+            const int mm = m0 + 4 * (warp + FW_PWARPS * i);
+            a_ch[i] = -1;                                    // -1: rows beyond M
+            a_dy[i] = a_dx[i] = 0;
+            if (mm < Mtot) {
+                const int tap = mm / p.Cin;
+                a_ch[i] = mm - tap * p.Cin;
+                a_dy[i] = tap / p.kw - p.pad;
+                a_dx[i] = tap - (tap / p.kw) * p.kw - p.pad;
+            }
+        }
+        const uint32_t a_smem = tc::smem_u32(sA), b_smem = tc::smem_u32(sB);
+        // Software-pipelined: the global loads of k-block it+1 are in flight while this thread waits for k-block it's stage
+        // and stores it transposed.  (fq, fpx, fb, fho, fwo) is the position of the next k-block to fetch, across the
+        // passes (low-part passes first: added while the sums are small; raw x raw last).
+        int fq = 0, fkb = 0, fpx = pix_begin + lane, fb, fho, fwo;
+        {
+            const int rem = fpx - (fb = fpx / HWo) * HWo;
+            fho = rem / p.Wo;
+            fwo = rem - fho * p.Wo;
+        }
+        auto fetch = [&](float4 (&va)[A_IT], float4 (&vb)[B_IT]) {
+            const int ps = (fq + 1) % npass;
+            const float* a_base = (ps == 1 && p.in_lo != nullptr) ? p.in_lo : p.in;
+            const float* b_main = STACK ? p.dout : ((ps == npass - 1 && ps > 0 && p.dout_lo != nullptr) ? p.dout_lo : p.dout);
+            const bool px_ok = fpx < pix_end;
+#pragma unroll
+            for (int i = 0; i < A_IT; ++i) {
+                int hi = fho * p.stride + a_dy[i], wi = fwo * p.stride + a_dx[i];
+                bool ok = px_ok && a_ch[i] >= 0;
+                if (reflect) { hi = reflect_index(hi, p.Hi); wi = reflect_index(wi, p.Wi); }
                 else ok = ok && (unsigned)hi < (unsigned)p.Hi && (unsigned)wi < (unsigned)p.Wi;
-                const int off = ok ? ((b * p.Hi + hi) * p.Wi + wi) * p.Cin + a_ch : 0;
-                tc::cp_async_16(a_st + (k >> 2) * (4 * 512) + (k & 3) * 128 + (((((a_chunk >> 1) ^ (k & 3)) << 1) | (a_chunk & 1)) * 16),
-                                a_base + off, ok ? 16u : 0u);
-                if (!BORDER) { if (++wo == p.Wo) { wo = 0; if (++ho == p.Ho) { ho = 0; ++b; } } }
+                va[i] = ok ? __ldg(reinterpret_cast<const float4*>(a_base + ((size_t)(fb * p.Hi + hi) * p.Wi + wi) * p.Cin + a_ch[i]))
+                           : make_float4(0.f, 0.f, 0.f, 0.f);
             }
 #pragma unroll
             for (int i = 0; i < B_IT; ++i) {
-                const int k = b_kr0 + B_STEP * i;
-                const int px = pix0 + k;
-                const bool ok = b_ok && px < pix_end;
-                size_t row = (size_t)px;                       // row of dout
-                if (BORDER && ok) {
-                    const int bb = px / nb;
-                    int bho, bwo;
-                    border_pixel(px - bb * nb, p.Ho, p.Wo, bho, bwo);
-                    row = ((size_t)bb * p.Ho + bho) * p.Wo + bwo;
-                }
-                tc::cp_async_16(b_st + (k >> 2) * ((BN / 32) * 512) + (k & 3) * 128 + ((((((b_c4 & 7) >> 1) ^ (k & 3)) << 1) | (b_c4 & 1)) * 16),
-                                b_base + (ok ? row * N + nn : 0), ok ? 16u : 0u);
+                const int col = 4 * (warp + FW_PWARPS * i);      // first tile row (output channel column) of this chunk
+                const bool lo_half = STACK && col >= BN / 2;     // stacked: rows >= BN/2 read lo(dout) at channel col - BN/2
+                const int nn = STACK ? col - (lo_half ? BN / 2 : 0) : n0 + col;
+                const bool ok = px_ok && nn < N;
+                const float* bb = lo_half ? p.dout_lo : b_main;
+                vb[i] = ok ? __ldg(reinterpret_cast<const float4*>(bb + (size_t)fpx * N + nn)) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
-            tc::cp_async_arrive_noinc(bar_full + s);
-            pix0 += 32;
-            pwo += 32;
-            while (pwo >= p.Wo) { pwo -= p.Wo; if (++pho == p.Ho) { pho = 0; ++pb; } }
-        }
-        }
-
-        // ------------------------------------------------------------------ epilogue: dw[o][mm] += D[mm][o]
-        tc::mbar_wait(bar_acc, 0);
-        tc::fence_after_thread_sync();
-        const int quarter = warp & 3, half = warp >> 2;
-        const int row = m0 + quarter * 32 + lane;
-        const int nacc = min(nacc_rt, KB * npass);
-#pragma unroll 1
-        for (int cc = half; cc < BN / 32; cc += FW_PWARPS / 4) {
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(cc * 32);
-            tc::tmem_ld32(taddr, r);
-            tc::tmem_ld_wait();
-            for (int a = 1; a < nacc; ++a) {                   // round-robin partial accumulators, added in fp32 (RN)
-                uint32_t q[32];
-                tc::tmem_ld32(taddr + (uint32_t)(a * Cfg::ACC_COLS), q);
-                tc::tmem_ld_wait();
+            // advance to the next k-block: 32 pixels further, or the first k-block of the next pass
+            if (++fkb == KB) {
+                fkb = 0;
+                ++fq;
+                fpx = pix_begin + lane;
+                const int rem = fpx - (fb = fpx / HWo) * HWo;
+                fho = rem / p.Wo;
+                fwo = rem - fho * p.Wo;
+            } else {
+                fpx += 32;
+                fwo += 32;
+                while (fwo >= p.Wo) { fwo -= p.Wo; if (++fho == p.Ho) { fho = 0; ++fb; } }
+            }
+        };
+        const int total = KB * npass;
+        float4 va[A_IT], vb[B_IT];
+        fetch(va, vb);
+        for (int it = 0; it < total; ++it) {
+            float4 na[A_IT], nb[B_IT];
+            if (it + 1 < total) fetch(na, nb);
+            const int s = it % STAGES;
+            tc::mbar_wait(bar_empty + s, ((it / STAGES) & 1) ^ 1);
+            const uint32_t a_st = a_smem + (uint32_t)(s * Cfg::A_BYTES), b_st = b_smem + (uint32_t)(s * Cfg::B_BYTES);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(q[j]));
+            for (int i = 0; i < A_IT; ++i) {
+                const int r = 4 * (warp + FW_PWARPS * i);
+                tc::st_shared_f32(a_st + tc::sw128_offset(r, lane), va[i].x);
+                tc::st_shared_f32(a_st + tc::sw128_offset(r + 1, lane), va[i].y);
+                tc::st_shared_f32(a_st + tc::sw128_offset(r + 2, lane), va[i].z);
+                tc::st_shared_f32(a_st + tc::sw128_offset(r + 3, lane), va[i].w);
             }
-            if (row < Mtot) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int col = cc * 32 + j;
-                    const int o = STACK ? (col >= BN / 2 ? col - BN / 2 : col) : n0 + col;
-                    if (o < N) red_add(p.dw + (size_t)o * Mtot + row, __uint_as_float(r[j]));
-                }
+            for (int i = 0; i < B_IT; ++i) {
+                const int r = 4 * (warp + FW_PWARPS * i);
+                tc::st_shared_f32(b_st + tc::sw128_offset(r, lane), vb[i].x);
+                tc::st_shared_f32(b_st + tc::sw128_offset(r + 1, lane), vb[i].y);
+                tc::st_shared_f32(b_st + tc::sw128_offset(r + 2, lane), vb[i].z);
+                tc::st_shared_f32(b_st + tc::sw128_offset(r + 3, lane), vb[i].w);
             }
+            tc::fence_proxy_async();                         // generic-proxy stores -> wgmma (async proxy) reads
+            tc::mbar_arrive(bar_full + s);
+#pragma unroll
+            for (int i = 0; i < A_IT; ++i) va[i] = na[i];
+#pragma unroll
+            for (int i = 0; i < B_IT; ++i) vb[i] = nb[i];
         }
     } else {
-        // ------------------------------------------------------------------ MMA issuer (warp 4)
-        constexpr uint32_t idesc = tc::make_idesc_tf32(TBM, BN, 1, 1);       // both operands MN-major
-        if (lane == 0) {
-            for (int kb = 0; kb < KB * npass; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t ph = (kb / STAGES) & 1;
-                tc::mbar_wait(bar_full + s, ph);
-                tc::fence_proxy_async();
-                tc::fence_after_thread_sync();
-                const uint32_t a_addr = tc::smem_u32(sA + s * Cfg::A_BYTES);
-                const uint32_t b_addr = tc::smem_u32(sB + s * Cfg::B_BYTES);
+        // ------------------------------------------------------------------ consumer warpgroup: dw[o][mm] += D[mm][o]
+        float acc[BN / 2];
+        gather_consume<BN, STAGES, Cfg::A_BYTES, Cfg::B_BYTES>(acc, sA, sB, bar_full, bar_empty, KB * npass, chain);
+        const int t = tid - FW_PWARPS * 32;
+        const int r = m0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {               // 4 x (2 pixel groups of 4): UMMA K = 8 for tf32
-                    // LBO = 512 B between 32-channel atoms, SBO = distance between 4-pixel groups; 2 groups per MMA
-                    const uint64_t da = tc::make_smem_desc(a_addr + j * (2 * 4 * 512), 512, 4 * 512, tc::LAYOUT_SW128_BASE32B);
-                    const uint64_t db = tc::make_smem_desc(b_addr + j * (2 * (BN / 32) * 512), 512, (BN / 32) * 512, tc::LAYOUT_SW128_BASE32B);
-                    tc::mma_tf32(tmem_base + (uint32_t)((kb % nacc_rt) * Cfg::ACC_COLS), da, db, idesc, (kb >= nacc_rt || j != 0) ? 1u : 0u);
-                }
-                tc::mma_commit(bar_empty + s);
+        for (int i = 0; i < BN / 8; ++i) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int row = r + 8 * (e >> 1), col = 8 * i + c + (e & 1);
+                const int o = STACK ? (col >= BN / 2 ? col - BN / 2 : col) : n0 + col;
+                if (row < Mtot && o < N) red_add(p.dw + (size_t)o * Mtot + row, acc[4 * i + e]);
             }
-            tc::mma_commit(bar_acc);
         }
-        __syncwarp();
     }
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == FW_PWARPS) tc::tmem_dealloc(tmem_base, tmem_cols);
 }
 
 CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, cuuint32_t rank, void* gaddr, const cuuint64_t* gdim,
@@ -559,28 +518,37 @@ CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, cuuint32_t ra
 
 int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStream_t st);   // conv_simt.cu
 
-template <int BN, bool BORDER = false, bool STACK = false>
+static int sm_count() {
+    static int n = 0;
+    if (n == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    }
+    return n;
+}
+
+template <int BN, bool STACK = false>
 static int launch_wgrad_tc(const ScsfmConv& p, cudaStream_t st) {
     using Cfg = WgCfg<BN>;
-    static const cudaError_t attr_rc = cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, BORDER, STACK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
+    static const cudaError_t attr_rc = cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, STACK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     SCSFM_CHECK_CUDA(attr_rc);
-    const int Mtot = p.kh * p.kw * p.Cin, npix = p.B * (BORDER ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo);
-    const int mt = (Mtot + TBM - 1) / TBM, nt = STACK ? 1 : (p.Cout + BN - 1) / BN;
-    int splits = (148 * 3 + mt * nt - 1) / (mt * nt);          // 3 CTAs per SM fit
+    const int Mtot = p.kh * p.kw * p.Cin, npix = p.B * p.Ho * p.Wo;
+    const int mt = (Mtot + GBM - 1) / GBM, nt = STACK ? 1 : (p.Cout + BN - 1) / BN;
+    static int per_sm = 0;                                   // resident CTAs per SM (shared memory bound: 2 for BN = 128)
+    if (per_sm == 0) {
+        SCSFM_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_wgrad_tc_kernel<BN, STACK>, FW_THREADS, Cfg::SMEM));
+        if (per_sm < 1) per_sm = 1;
+    }
+    // Three CTAs' worth of pixel splits per SM although only two BN = 128 CTAs are resident at once (shared memory): the
+    // extra split-K CTAs keep the transposing producers of more tiles in flight.  Measured on H100 over the layers of
+    // tools/conv_layers.py (tf32x3 weight gradients): 20.0 ms with this count, 28.6 ms with exactly one resident wave.
+    int splits = (sm_count() * 3 + mt * nt - 1) / (mt * nt);
     const int max_splits = (npix + 1023) / 1024;             // at least 32 k-blocks per CTA
     if (splits > max_splits) splits = max_splits;
     if (splits < 1) splits = 1;
-    const int npass = STACK ? 2 : 1 + (p.in_lo != nullptr ? 1 : 0) + (p.dout_lo != nullptr ? 1 : 0);
-    if (npass > 1) {
-        // split-accumulate (parity) mode: bound every accumulation chain to ~160 tcgen05.mma (truncation bias ~5e-6):
-        // chain = k-blocks * 4 MMAs * passes / NACC.  More, shorter CTAs; their partial tiles are added with fp32 atomics (RN)
-        const int kb_max = 160 * Cfg::NACC / (4 * npass);
-        const int need = (npix + 32 * kb_max - 1) / (32 * kb_max);
-        if (splits < need) splits = need;
-    }
     const int pps = ((npix + splits - 1) / splits + 31) / 32 * 32;
     dim3 grid(mt, nt, (npix + pps - 1) / pps);
-    conv_wgrad_tc_kernel<BN, BORDER, STACK><<<grid, FW_THREADS, Cfg::SMEM, st>>>(p, pps);
+    conv_wgrad_tc_kernel<BN, STACK><<<grid, FW_THREADS, Cfg::SMEM, st>>>(p, pps);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
@@ -614,7 +582,7 @@ static int launch_fwd_tc(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
             return SCSFM_ERR_CUDA;
         }
     }
-    dim3 grid((M + TBM - 1) / TBM, STACK ? 1 : (p.Cout + BN - 1) / BN);
+    dim3 grid((M + GBM - 1) / GBM, STACK ? 1 : (p.Cout + BN - 1) / BN);
     conv_fwd_tc_kernel<BN, STACK><<<grid, FW_THREADS, Cfg::SMEM, st>>>(p, v, wmap, wmap_lo);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
@@ -637,7 +605,7 @@ static int tc_dispatch_gather(const ScsfmConv& p, const TcView& v, cudaStream_t 
     if (N <= 64 || N % 128 != 0) return launch_fwd_tc<64>(p, v, st);
     // prefer more CTAs when the M extent is small (deep layers at 8x26 / 16x52)
     const int M = p.B * (v.border ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo);
-    if (((M + TBM - 1) / TBM) * (N / 128) < 148) return launch_fwd_tc<64>(p, v, st);
+    if (((M + GBM - 1) / GBM) * (N / 128) < sm_count()) return launch_fwd_tc<64>(p, v, st);
     return launch_fwd_tc<128>(p, v, st);
 }
 
@@ -683,7 +651,7 @@ extern "C" int scsfm_weight_flip(const float* w, int Cout, int kh, int kw, int C
     SCSFM_CHECK_ARG(w && wt && Cout > 0 && kh > 0 && kw > 0 && Cin > 0 && operand >= 0 && operand <= 2, "weight_flip: bad arguments");
     const long long total = (long long)Cout * kh * kw * Cin;
     int grid = (int)((total + 255) / 256);
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > sm_count() * 16) grid = sm_count() * 16;
     weight_flip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, Cout, kh, kw, Cin, kh, kw, kh - 1, kw - 1, 1, wt, operand);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
@@ -753,7 +721,7 @@ extern "C" int scsfm_weight_flip_s2(const float* w, int Cout, int kh, int kw, in
             const long long total = (long long)Cout * jh * jw * Cin;
             if (total > 0) {
                 int grid = (int)((total + 255) / 256);
-                if (grid > 148 * 16) grid = 148 * 16;
+                if (grid > sm_count() * 16) grid = sm_count() * 16;
                 weight_flip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, Cout, kh, kw, Cin, jh, jw, dy_max, dx_max, 2, wt4 + off, operand);
                 SCSFM_CHECK_LAUNCH();
             }
@@ -834,38 +802,17 @@ extern "C" int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream) {
     SCSFM_CHECK_ARG((long long)p->B * p->Ho * p->Wo < (1LL << 31), "conv2d_wgrad_tc: too many pixels");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    ScsfmConv zp = *p;                         // the same layer with zero padding (what the TMA kernel computes)
-    zp.pad_mode = SCSFM_PADMODE_ZERO;
-    int kernel = (int)((p->tune >> 12) & 3u);       // SCSFM_TUNE_WGRAD: 0 auto, 1 cp.async kernel, 2 TMA kernel, 3 thin-layer fp32 kernel
+    // SCSFM_TUNE_WGRAD: 0 auto, 1 or 2 the tensor-core kernel above, 3 the thin-layer fp32 kernel
+    int kernel = (int)((p->tune >> 12) & 3u);
     if (kernel == 3 && !conv_wgrad_thin_eligible(*p)) kernel = 0;
-    if (kernel == 0) {
-        // split-accumulate (parity) mode: the TMA kernel drains its accumulation chains into registers, so it needs no extra
-        // split-K to bound the truncation bias; the cp.async kernel does (cheap only when dW is small, i.e. thin layers).
-        // Plain TF32: the cp.async kernel is as fast or faster everywhere (profiles/r02_wgrad_tma_check.txt).
-        const bool split = p->in_lo != nullptr || p->dout_lo != nullptr;
-        // (measured per layer, profiles/r02_layers_tf32x3_wgrad.txt: from 64 output channels up the TMA kernel wins, below
-        // that the cp.async kernel with dout / lo(dout) stacked on its N side)
-        kernel = (split && p->Cout >= 64) ? 2 : 1;
-        // the 16-output-channel decoder layers are bound by the MMA instruction count (K = 8 pixels per tcgen05.mma, 16 of 128 rows
-        // used) and in split mode read four tensors: the fp32 FMA kernel reads two and is exact per product (conv_wgrad_thin.cu)
-        if (split && conv_wgrad_thin_eligible(*p)) kernel = 3;
-    }
-    if (kernel == 3) {
-        rc = launch_conv_wgrad_thin(*p, st);
-    } else if (kernel == 2 && p->pad_mode == PADMODE_ZERO && conv_wgrad_tma_eligible(*p)) {
-        rc = launch_conv_wgrad_tma(*p, st);
-    } else if (kernel == 2 && p->pad_mode == PADMODE_REFLECT && p->pad == 1 && p->Ho >= 3 && p->Wo >= 3 &&
-               p->Ho * p->Wo >= 64 * 208 && conv_wgrad_tma_eligible(zp)) {
-        // reflection padding: zero-padded pass + the contributions of the taps that leave the image (border pixels only)
-        rc = launch_conv_wgrad_tma(zp, st);
-        if (rc == SCSFM_OK) {
-            if (p->Cout <= 32) rc = launch_wgrad_tc<32, true>(*p, st);
-            else if (p->Cout <= 64) rc = launch_wgrad_tc<64, true>(*p, st);
-            else rc = launch_wgrad_tc<128, true>(*p, st);
-        }
-    } else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 16) rc = launch_wgrad_tc<32, false, true>(*p, st);
-    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 32) rc = launch_wgrad_tc<64, false, true>(*p, st);
-    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 64) rc = launch_wgrad_tc<128, false, true>(*p, st);
+    // the 16-output-channel decoder layers in split mode read four tensors and use 16 of the MMA's columns: the fp32 FMA
+    // kernel reads two and is exact per product (conv_wgrad_thin.cu)
+    if (kernel == 0 && (p->in_lo != nullptr || p->dout_lo != nullptr) && conv_wgrad_thin_eligible(*p)) kernel = 3;
+    if (kernel == 3) rc = launch_conv_wgrad_thin(*p, st);
+    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 16) rc = launch_wgrad_tc<32, true>(*p, st);
+    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 32) rc = launch_wgrad_tc<64, true>(*p, st);
+    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 64) rc = launch_wgrad_tc<128, true>(*p, st);
+    else if (p->Cout <= 16) rc = launch_wgrad_tc<16>(*p, st);
     else if (p->Cout <= 32) rc = launch_wgrad_tc<32>(*p, st);
     else if (p->Cout <= 64) rc = launch_wgrad_tc<64>(*p, st);
     else rc = launch_wgrad_tc<128>(*p, st);

@@ -8,29 +8,31 @@
 
 namespace scsfm {
 
-constexpr int TBM = 128;            // tile rows (UMMA M)
+constexpr int TBM = 128;            // pixel tile of the TMA kernel (two consumer warpgroups of 64 rows)
+constexpr int GBM = 64;             // tile rows of the cp.async gather kernels (one wgmma M = 64 warpgroup)
 constexpr int TBK = 32;             // floats per k-block = one 128-byte swizzle row
-constexpr int TC_THREADS = 160;       // wgrad kernel: 4 producer/epilogue warps + 1 MMA warp
-constexpr int FW_PWARPS = 8;          // forward/dgrad kernel: 8 producer/epilogue warps + 1 MMA warp
-constexpr int FW_THREADS = (FW_PWARPS + 1) * 32;
-constexpr int A_STAGE_BYTES = TBM * 128;
+constexpr int FW_PWARPS = 4;        // gather kernels: 4 producer warps + 1 consumer warpgroup (wgmma issue and accumulators)
+constexpr int FW_THREADS = (FW_PWARPS + 4) * 32;
+constexpr int A_STAGE_BYTES = GBM * 128;
 
-// The tensor core adds into a TMEM accumulator with truncation: a chain of n tcgen05.mma carries a systematic relative error
-// of ~3e-8 * n (measured; 1e-4 after a few thousand).  The kernels whose epilogue warps are busy producing (cp.async gather
-// kernels) therefore spread consecutive k-blocks round-robin over NACC accumulators (chains NACC times shorter) and add them
-// up in registers (round-to-nearest) in the epilogue.
+// The tensor core adds into the accumulator with truncation: a long chain of MMAs into one accumulator carries a
+// systematic relative error that grows with its length.  In split mode the consumer therefore accumulates CHAIN k-blocks
+// (4 wgmma each) into a scratch accumulator started from zero and adds it to the running sum in fp32 registers
+// (round-to-nearest); plain TF32 is bounded by its operand rounding and runs one chain.
+constexpr int CHAIN_KB = 2;
+
 template <int BN>
 struct TcCfg {
-    static constexpr int STAGES = 3;
+    static constexpr int STAGES = 4;
     static constexpr int B_STAGE_BYTES = BN * 128;
-    static constexpr int NACC = BN >= 128 ? 2 : 4;
-    static constexpr int ACC_COLS = BN < 32 ? 32 : BN;      // column stride between accumulators
-    static constexpr int TMEM_COLS = NACC * ACC_COLS;       // 64 .. 256: two CTAs per SM still fit in the 512 columns
-    static constexpr size_t SMEM = 1024 + (size_t)STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 256;
+    static constexpr size_t OPERANDS = (size_t)STAGES * (A_STAGE_BYTES + B_STAGE_BYTES);
+    // epilogue: the accumulator tile [GBM][BN + 1] plus a 32 x 33 transpose scratch per warp, over the free operand ring
+    static constexpr size_t EPI = (size_t)GBM * (BN + 1) * 4 + (size_t)(FW_PWARPS + 4) * 32 * 33 * 4;
+    static constexpr size_t SMEM = 1024 + (OPERANDS > EPI ? OPERANDS : EPI) + 256;
 };
 
-// Operand precision: kind::tf32 TRUNCATES the low 13 mantissa bits of whatever fp32 pattern sits in shared memory
-// (measured: a systematic -7e-4 relative bias per dot product).  Converting with cvt.rna inside the loaders costs
+// Operand precision: the tf32 MMA ignores the low 13 mantissa bits of whatever fp32 pattern sits in shared memory
+// (a systematic bias per dot product if the operands were not rounded).  Converting with cvt.rna inside the loaders costs
 // ~50% of the loader-bound kernel time, so the operands are rounded ONCE where they are produced instead: every
 // kernel that writes a tensor later consumed by a convolution takes the SCSFM_ROUND_TF32 flag, and the weights are
 // rounded per optimizer step (scsfm_round_tf32).  The loaders below therefore copy bits unchanged.
@@ -74,10 +76,6 @@ CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, cuuint32_t ra
 bool conv_tma_eligible(const ScsfmConv& p, const TcView& v);
 bool conv_tma_forced(const ScsfmConv& p);      // a tile configuration is being forced through ScsfmConv.tune (tests / experiments)
 int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st);
-
-// conv_wgrad_tma.cu: stride-1 zero-padded weight gradient with TMA-delivered operands
-bool conv_wgrad_tma_eligible(const ScsfmConv& p);
-int launch_conv_wgrad_tma(const ScsfmConv& p, cudaStream_t st);
 
 // conv_wgrad_thin.cu: 3x3 stride-1 pad-1 layers with Cout = 16 and Cin in {16, 32} on the fp32 FMA pipes (exact products: no low parts)
 bool conv_wgrad_thin_eligible(const ScsfmConv& p);

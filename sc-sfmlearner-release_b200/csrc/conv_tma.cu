@@ -1,32 +1,23 @@
-// Stride-1 convolution on the tensor cores: persistent CTAs, TMA halo-patch producer, double-buffered TMEM accumulators
-// (tcgen05 kind::tf32, fp32 accumulation), weights on the M side of the MMA.
+// Stride-1 convolution on the tensor cores: persistent CTAs, TMA halo-patch producer, two consumer warpgroups
+// (wgmma, tf32 operands, fp32 accumulation in registers).
 //
-//   D^T[Cout tile (M = 128 TMEM lanes), pixels (N = 128 or 256 TMEM columns)] = W[Cout, K] x im2col(x)[pixels, K]^T
+//   D[pixels (M = 64 per wgmma), Cout tile (N = BNW)] = im2col(x)[pixels, K] x W[Cout, K]^T
 //
-// Why this shape.  Measured on B200 (tools/tma_profile.py, profiles/r01_tma_roles.txt): with both operands in shared
-// memory a tcgen05.mma with M = 128 takes ~130-140 cycles whatever N is (the M-side operand streams from shared memory
-// one 32-byte row per cycle), so an M128 x N64 x K8 instruction runs the tensor pipe at a quarter of its rate.  The
-// layers here have 16..128 output channels (only the deepest have 256/512) but >= 10^4 pixels, so the PIXELS go on the
-// N side (up to 256 per instruction) and the output channels on the M side (rows beyond Cout compute garbage lanes that
-// nobody reads and cost nothing extra).  The accumulator comes out channel-major: TMEM lane = output channel, column =
-// pixel, which also makes the epilogue stores coalesced along NHWC channels and the BatchNorm sums a per-lane loop.
-//
-// Versus the cp.async kernel of conv_tc.cu (one 128 x 32-float im2col slice gathered per (tap, channel chunk) by 256
-// threads, one CTA per 128-pixel tile):
+// Versus the cp.async kernel of conv_tc.cu (one 64 x 32-float im2col slice gathered per (tap, channel chunk), one CTA per
+// 64-pixel tile):
 //  * the output tile is a 2-D patch of ONE image (MT*TH rows x TW columns, TH*TW = 128, TW in {8, 16}); per (channel
 //    chunk, dx) ONE 4-D tiled TMA load brings the (MT*TH + kh - 1) x TW x 32-channel input patch in the 128B-swizzled
-//    K-major layout the UMMA descriptors expect.  TW is a multiple of 8, so the operand of tap row dy is the SAME patch
+//    K-major layout the wgmma descriptors expect.  TW is a multiple of 8, so the operand of tap row dy is the SAME patch
 //    shifted by dy*TW rows = dy*TW*128 bytes (a multiple of the 1024-byte swizzle atom): the kh vertical taps reuse one
 //    load.  Zero padding is the TMA's out-of-bounds fill; channels beyond Cin in the last 32-wide chunk are zero-filled
 //    the same way (the matching weight columns then multiply zeros) and all-zero K8 slices are not issued at all;
 //  * one CTA per SM walks the (tile, Cout tile) work list; the shared-memory stage ring and the mbarrier phases run
-//    across tiles, so the producer prefetches the next tile's patches while the current one is still being multiplied;
-//  * two TMEM accumulator buffers: the epilogue warps drain tile j (tcgen05.ld -> bias / residual addend / activation /
-//    TF32 rounding / BatchNorm sums -> global) while the MMA warp already accumulates tile j+1.
+//    across tiles, so the producer prefetches the next tile's patches while the current one is multiplied and stored;
+//  * the accumulator comes out pixel-major (a thread holds 2 consecutive channels of a pixel per fragment), so the
+//    epilogue writes NHWC straight from registers: bias / residual addend / activation / TF32 rounding / BatchNorm sums.
 //
-//   warps 0-7   epilogue (warp w reads TMEM lanes 32*(w%4).., i.e. channels; w/4 picks every other 32-pixel chunk)
+//   warps 0-7   two consumer warpgroups; warpgroup g owns the pixels [64 MT g, 64 MT (g + 1)) of the tile
 //   warp 8      lane 0: TMA producer (1 activation box + kh weight boxes per stage, mbarrier expect_tx)
-//   warp 9      TMEM allocation; lane 0: MMA issuer (kh * <=4 tcgen05.mma M128 x N(128|256) x K8 per stage)
 //
 // Used for: forward of every stride-1 layer with kh, kw <= 3 (reflection-padded layers run it with zero padding and
 // the cp.async kernel then recomputes the 2*(H+W)-4 border pixels per image, see tc_dispatch in conv_tc.cu), stride-1
@@ -37,11 +28,11 @@
 
 namespace scsfm {
 
-constexpr int TMA_EWARPS = 8;
-constexpr int TMA_THREADS = (TMA_EWARPS + 2) * 32;
+constexpr int TMA_CWARPS = 8;
+constexpr int TMA_THREADS = (TMA_CWARPS + 1) * 32;
 constexpr int TMA_MAX_KH = 3;
 constexpr int TMA_MAX_STAGES = 8;
-constexpr int TMA_SMEM_MAX = 232448;                         // 227 KB: the most one CTA may opt into on sm_100
+constexpr int TMA_SMEM_MAX = 232448;                         // 227 KB: the most one CTA may opt into on sm_90
 
 struct TmaGeom {
     int tw_log2;             // TW = 1 << tw_log2 (3 or 4), TH = 128 >> tw_log2
@@ -52,40 +43,25 @@ struct TmaGeom {
     // split-accumulate passes per (channel chunk, dx): pass i multiplies (activations: lo if a_lo bit i else raw) by
     // (weights: lo if w_lo bit i else raw); plain TF32 = one pass with both masks 0
     int npass, a_lo, w_lo;
-    // split mode with <= 64 output channels: the weight tile stacks W (rows 0..) and lo(W) (rows 64..) on the M side of ONE
-    // tcgen05.mma, so the two passes lo(x) and x produce all four products (TMEM lanes c and 64 + c are added in the epilogue):
-    // two MMAs per K8 slice instead of three
-    int stack;
-    // accumulation chunks: the tensor core adds into the TMEM accumulator with truncation (measured: relative error ~ 3e-8 per
-    // tcgen05.mma of the chain, a systematic bias), so a chain is cut after `cpg` channel chunks (~100 MMAs) and the epilogue
-    // warps add the partial accumulators in registers (round-to-nearest).  cpg >= chunks: one chain per tile (plain TF32 mode).
+    // accumulation chunks: channel chunks whose passes the producer issues together (low parts first).  In split mode the
+    // consumers also add every stage's wgmma into the running sum in fp32 registers (round-to-nearest): the tensor core adds
+    // into its accumulator with truncation, a systematic bias that grows with the chain.  Plain TF32: one chain per tile.
     int cpg;
     unsigned long long* dbg; // optional per-CTA cycle counters (ScsfmConv.debug), 8 per CTA; NULL = off
 };
 
-__device__ __forceinline__ long long tma_clock() { return clock64(); }
-
-// BNW: rows of the weight tile kept in shared memory (16/32/64/128 >= the Cout tile); the MMA always reads 128 rows from
-// the tile start (M = 128), the rows past BNW are whatever follows in shared memory and only feed unread lanes.
-// MT: 128-pixel sub-tiles stacked vertically, N = MT * 128 pixels per instruction.
+// BNW: Cout tile = weight rows kept in shared memory = N of the wgmma (16/32/64/128).
+// MT: 128-pixel sub-tiles stacked vertically; each consumer warpgroup runs MT wgmma of M = 64 per K8 slice.
 template <int BNW, int MT>
 __global__ void __launch_bounds__(TMA_THREADS, 1)
 conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap wmap,
                 const __grid_constant__ CUtensorMap amap_lo, const __grid_constant__ CUtensorMap wmap_lo) {
-    constexpr int NPIX = MT * TBM;                           // TMEM columns of one accumulator buffer
-    constexpr int TMEM_COLS = 2 * NPIX;                      // 256 or 512
-    const int W_TILE = g.stack ? TBM * 128 : BNW * 128;      // one tap: BNW rows x 32 floats (stacked: W at row 0, lo(W) at row 64)
+    constexpr int W_TILE = BNW * 128;                        // one tap: BNW rows x 32 floats
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    // barriers live in FRONT of the stage ring: the MMA's 128-row read of a BNW-row weight tile may run past the last stage
     uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem);
     uint64_t* bar_empty = bar_full + TMA_MAX_STAGES;
-    uint64_t* acc_full = bar_empty + TMA_MAX_STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
     uint8_t* ring = smem + 1024;
-    // epilogue transpose buffer T[64 pixels][BNW + 4] behind the ring and the over-read pad
-    float* T = reinterpret_cast<float*>(ring + (size_t)g.stages * g.stage_bytes + (g.stack ? 0 : (TBM - BNW) * 128));
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int TW = 1 << g.tw_log2, TH = TBM >> g.tw_log2;
@@ -96,36 +72,28 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
     if (tid == 0) {
         for (int s = 0; s < g.stages; ++s) {
             tc::mbar_init(bar_full + s, 1);              // the producer's expect_tx arrival; TMA completes the bytes
-            tc::mbar_init(bar_empty + s, 1);             // tcgen05.commit of the MMAs that read the stage
-        }
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(acc_full + i, 1);              // tcgen05.commit after the tile's last MMA
-            tc::mbar_init(acc_empty + i, TMA_EWARPS);    // one arrival per epilogue warp
+            tc::mbar_init(bar_empty + s, TMA_CWARPS * 32);   // every consumer thread, once the wgmma that read the stage retired
         }
         tc::fence_barrier_init();
     }
-    if (warp == TMA_EWARPS + 1) tc::tmem_alloc(tmem_slot, TMEM_COLS);
-    tc::fence_before_thread_sync();
     __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem_base = *tmem_slot;
     const uint32_t ring_base = tc::smem_u32(ring);
 
-    if (warp == TMA_EWARPS) {
+    if (warp == TMA_CWARPS) {
         // ------------------------------------------------------------------ TMA producer
         if (lane == 0) {
             tc::tma_prefetch_desc(&amap);
             tc::tma_prefetch_desc(&wmap);
             if (g.a_lo) tc::tma_prefetch_desc(&amap_lo);
             if (g.w_lo) tc::tma_prefetch_desc(&wmap_lo);
-            const uint32_t tx_bytes = (uint32_t)(patch_rows * TW * 128 + v.kh * (g.stack ? 2 : 1) * BNW * 128);
+            const uint32_t tx_bytes = (uint32_t)(patch_rows * TW * 128 + v.kh * W_TILE);
             int s = 0;
             uint32_t ph = 0;
             long long t_wait = 0;
-            const long long t_begin = tma_clock();
+            const long long t_begin = clock64();
             for (int w = blockIdx.x; w < g.num_work; w += gridDim.x) {
                 int t = w / g.n_tiles;
-                const int n0 = (w - t * g.n_tiles) * TBM;
+                const int n0 = (w - t * g.n_tiles) * BNW;
                 const int tx = t % g.tiles_x; t /= g.tiles_x;
                 const int ty = t % g.tiles_y;
                 const int b = t / g.tiles_y;
@@ -140,22 +108,14 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
                     const CUtensorMap* wm = ((g.w_lo >> ps) & 1) ? &wmap_lo : &wmap;
                     for (int ck = ck0; ck < min(chunks, ck0 + g.cpg); ++ck) {
                         for (int dx = 0; dx < v.kw; ++dx) {
-                            const long long t0 = g.dbg ? tma_clock() : 0;
+                            const long long t0 = g.dbg ? clock64() : 0;
                             tc::mbar_wait(bar_empty + s, ph ^ 1);
-                            if (g.dbg) t_wait += tma_clock() - t0;
+                            if (g.dbg) t_wait += clock64() - t0;
                             const uint32_t st = ring_base + (uint32_t)(s * g.stage_bytes);
                             tc::mbar_arrive_expect_tx(bar_full + s, tx_bytes);
                             tc::tma_load_4d(st, am, ck * TBK, x0 + dx, y0, b, bar_full + s);
-                            for (int dy = 0; dy < v.kh; ++dy) {
-                                const uint32_t wdst = st + (uint32_t)(g.a_bytes + dy * W_TILE);
-                                const int kcol = (dy * v.kw + dx) * p.Cin + ck * TBK;
-                                if (g.stack) {
-                                    tc::tma_load_2d(wdst, &wmap, kcol, n0, bar_full + s);
-                                    tc::tma_load_2d(wdst + 64 * 128, &wmap_lo, kcol, n0, bar_full + s);
-                                } else {
-                                    tc::tma_load_2d(wdst, wm, kcol, n0, bar_full + s);
-                                }
-                            }
+                            for (int dy = 0; dy < v.kh; ++dy)
+                                tc::tma_load_2d(st + (uint32_t)(g.a_bytes + dy * W_TILE), wm, (dy * v.kw + dx) * p.Cin + ck * TBK, n0, bar_full + s);
                             if (++s == g.stages) { s = 0; ph ^= 1; }
                         }
                     }
@@ -163,217 +123,165 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
             }
             if (g.dbg) {
                 g.dbg[blockIdx.x * 8 + 0] = (unsigned long long)t_wait;
-                g.dbg[blockIdx.x * 8 + 1] = (unsigned long long)(tma_clock() - t_begin);
-            }
-        }
-        __syncwarp();
-    } else if (warp == TMA_EWARPS + 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        constexpr uint32_t idesc = tc::make_idesc_tf32(TBM, NPIX, 0, 0);      // M = 128 weight rows, N = NPIX pixels
-        if (lane == 0) {
-            const uint32_t dy_bytes = (uint32_t)(TW * 128);
-            // descriptor = constant fields (LBO 16, SBO 1024, 128B swizzle) + (shared address >> 4) in the low 14 bits
-            const uint64_t desc0 = tc::make_smem_desc(0, 16, 1024, tc::LAYOUT_SW128);
-            int s = 0;
-            uint32_t ph = 0;
-            int j = 0;
-            long long t_full = 0, t_acc = 0;
-            const long long t_begin = tma_clock();
-            int jc = 0;                                    // accumulation chunks issued so far: TMEM buffer jc & 1
-            for (int w = blockIdx.x; w < g.num_work; w += gridDim.x, ++j) {
-                for (int ck0 = 0; ck0 < chunks; ck0 += g.cpg) {          // one accumulation chain (same loop nest as the producer)
-                    const int buf = jc & 1;
-                    const long long ta = g.dbg ? tma_clock() : 0;
-                    tc::mbar_wait(acc_empty + buf, ((jc >> 1) & 1) ^ 1);      // the epilogue has drained this buffer
-                    if (g.dbg) t_acc += tma_clock() - ta;
-                    tc::fence_after_thread_sync();
-                    const uint32_t acc = tmem_base + (uint32_t)(buf * NPIX);
-                for (int q = 0; q < g.npass; ++q) {
-                    for (int ck = ck0; ck < min(chunks, ck0 + g.cpg); ++ck) {
-                    const bool first_of_chain = q == 0 && ck == ck0;
-                    const int rem = p.Cin - ck * TBK;
-                    const int k8 = rem >= TBK ? TBK / 8 : (rem + 7) / 8;           // K8 slices holding real channels
-                        for (int dx = 0; dx < v.kw; ++dx) {
-                            const long long t0 = g.dbg ? tma_clock() : 0;
-                            tc::mbar_wait(bar_full + s, ph);
-                            if (g.dbg) t_full += tma_clock() - t0;
-                            tc::fence_after_thread_sync();
-                            const uint32_t x_addr = ring_base + (uint32_t)(s * g.stage_bytes);
-                            const uint32_t w_addr = x_addr + (uint32_t)g.a_bytes;
-                            for (int dy = 0; dy < v.kh; ++dy) {
-                                uint64_t dw = desc0 + (uint64_t)((w_addr + (uint32_t)(dy * W_TILE)) >> 4);      // M side: weights
-                                uint64_t dx_ = desc0 + (uint64_t)((x_addr + (uint32_t)dy * dy_bytes) >> 4);    // N side: pixels
-                                for (int q8 = 0; q8 < k8; ++q8) {
-                                    tc::mma_tf32(acc, dw, dx_, idesc, (!first_of_chain || (dx | dy | q8) != 0) ? 1u : 0u);
-                                    dw += 2;                     // next K8 slice: +32 bytes inside the 128-byte swizzle row
-                                    dx_ += 2;
-                                }
-                            }
-                            tc::mma_commit(bar_empty + s);
-                            if (++s == g.stages) { s = 0; ph ^= 1; }
-                        }
-                    }
-                }
-                    tc::mma_commit(acc_full + buf);          // end of the chain: hand the buffer to the epilogue warps
-                    ++jc;
-                }
-            }
-            if (g.dbg) {
-                g.dbg[blockIdx.x * 8 + 2] = (unsigned long long)t_full;
-                g.dbg[blockIdx.x * 8 + 3] = (unsigned long long)t_acc;
-                g.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(tma_clock() - t_begin);
-                g.dbg[blockIdx.x * 8 + 7] = (unsigned long long)j;
+                g.dbg[blockIdx.x * 8 + 1] = (unsigned long long)(clock64() - t_begin);
             }
         }
         __syncwarp();
     } else {
-        // ------------------------------------------------------------------ epilogue (warps 0-7, 256 threads)
-        // The accumulator is channel-major (TMEM lane = output channel, column = pixel) but the tensor is NHWC, and a thin
-        // layer occupies only 16 or 32 of the 128 lanes.  So the tile is transposed through shared memory in rounds of 64
-        // pixels: the warps whose lane quarter holds real channels copy tcgen05.ld results into T[pixel][channel], then
-        // ALL 256 threads walk T as float4 channel groups: bias / residual addend / activation / TF32 rounding, 16-byte
-        // coalesced stores, BatchNorm partial sums per thread (a thread always owns the same 4 channels).
-        constexpr int CT = BNW;                      // channels per T row
-        constexpr int TS = CT + 4;                   // row stride in floats (keeps rows 16-byte aligned)
-        constexpr int GPR = CT / 4;                  // float4 groups per pixel
-        constexpr int ITER = (64 * GPR) / 256;       // groups per thread per round (CT / 16)
-        constexpr int PXSTEP = 256 / GPR;            // pixel distance between a thread's groups
-        const int quarter = warp & 3, half = warp >> 2;
-        const int c4 = tid % GPR, px0 = tid / GPR;   // this thread's channel group and first pixel of a round
+        // ------------------------------------------------------------------ consumer warpgroups (warps 0-7)
+        const int wg = warp >> 2, t = tid & 127;
+        const int fr = 16 * (t >> 5) + ((t & 31) >> 2), fc = 2 * (t & 3);   // fragment row / column of d[0]
         const int groups = p.bn_groups > 0 ? p.bn_groups : 1;
         const int act = p.act & 0xff;
         const bool round = (p.act & ROUND_TF32) != 0;
-        const int Ho = p.Ho, Wo = p.Wo;
         const long long img_step = (long long)v.out_H * v.out_W * N;       // elements between images
         const int row_step = v.out_sy * v.out_W * N;                        // ... between tile rows
         const int px_step = v.out_sx * N;                                   // ... between tile columns
-        constexpr int RPT = NPIX / 64;               // 32-column groups of the accumulator this warp owns: (2 * rd + half) * 32
-        const int nchains = (chunks + g.cpg - 1) / g.cpg;
-        float accr[RPT][32];                         // the tile's sums (this thread's TMEM lane = channel, RPT * 32 pixels)
-        int j = 0, jc = 0;
-        long long t_wait = 0, t_ld = 0;
-        const long long t_begin = tma_clock();
+        float acc[MT][BNW / 2], part[MT][BNW / 2];
+        int s = 0;
+        uint32_t ph = 0;
+        int pend = -1;
+        int j = 0;
+        long long t_full = 0;
+        const long long t_begin = clock64();
         for (int w = blockIdx.x; w < g.num_work; w += gridDim.x, ++j) {
-            int t = w / g.n_tiles;
-            const int n0 = (w - t * g.n_tiles) * TBM;
-            const int tx = t % g.tiles_x; t /= g.tiles_x;
-            const int ty = t % g.tiles_y;
-            const int b = t / g.tiles_y;
+            int tt = w / g.n_tiles;
+            const int n0 = (w - tt * g.n_tiles) * BNW;
+            const int tx = tt % g.tiles_x; tt /= g.tiles_x;
+            const int ty = tt % g.tiles_y;
+            const int b = tt / g.tiles_y;
             const int y0 = ty * (MT * TH), x0 = tx * TW;
-            const int cv = min(TBM, N - n0);                     // real channels of this Cout tile (multiple of 4)
-            // warp-uniform: this lane quarter holds real channels (stacked: quarters 2, 3 hold the lo(W) products of channels 0..63)
-            const bool loader = (g.stack ? (quarter & 1) : quarter) * 32 < cv;
-            // ---- drain the tile's accumulation chains into registers (TMEM -> registers, fp32 round-to-nearest adds)
-            for (int c = 0; c < nchains; ++c, ++jc) {
-                const int buf = jc & 1;
-                const long long t0 = g.dbg ? tma_clock() : 0;
-                tc::mbar_wait(acc_full + buf, (jc >> 1) & 1);
-                if (g.dbg) t_wait += tma_clock() - t0;
-                tc::fence_after_thread_sync();
-                if (loader) {
-                    const uint32_t src = tmem_base + (uint32_t)(buf * NPIX) + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(half * 32);
-                    const long long tl0 = g.dbg ? tma_clock() : 0;
-                    if (c == 0) {
 #pragma unroll
-                        for (int rd = 0; rd < RPT; ++rd) {
-                            uint32_t r[32];
-                            tc::tmem_ld32(src + (uint32_t)(rd * 64), r);
-                            tc::tmem_ld_wait();
+            for (int mb = 0; mb < MT; ++mb)
 #pragma unroll
-                            for (int i = 0; i < 32; ++i) accr[rd][i] = __uint_as_float(r[i]);
-                        }
-                    } else {
+                for (int i = 0; i < BNW / 2; ++i) acc[mb][i] = 0.f;
+            for (int ck0 = 0; ck0 < chunks; ck0 += g.cpg) {          // one accumulation chain (same loop nest as the producer)
+                bool first = true;
+                for (int q = 0; q < g.npass; ++q) {
+                    for (int ck = ck0; ck < min(chunks, ck0 + g.cpg); ++ck) {
+                        const int rem = p.Cin - ck * TBK;
+                        const int k8 = rem >= TBK ? TBK / 8 : (rem + 7) / 8;           // K8 slices holding real channels
+                        for (int dx = 0; dx < v.kw; ++dx) {
+                            const long long t0 = g.dbg ? clock64() : 0;
+                            tc::mbar_wait(bar_full + s, ph);
+                            if (g.dbg) t_full += clock64() - t0;
+                            const uint32_t x_addr = ring_base + (uint32_t)(s * g.stage_bytes);
+                            const uint32_t w_addr = x_addr + (uint32_t)g.a_bytes;
 #pragma unroll
-                        for (int rd = 0; rd < RPT; ++rd) {
-                            uint32_t r[32];
-                            tc::tmem_ld32(src + (uint32_t)(rd * 64), r);
-                            tc::tmem_ld_wait();
+                            for (int mb = 0; mb < MT; ++mb) tc::reg_fence(part[mb]);
+                            tc::wgmma_fence();
+                            for (int dy = 0; dy < v.kh; ++dy) {
+                                for (int q8 = 0; q8 < k8; ++q8) {
+                                    const uint64_t dw = tc::make_desc_sw128(w_addr + (uint32_t)(dy * W_TILE + q8 * 32));
 #pragma unroll
-                            for (int i = 0; i < 32; ++i) accr[rd][i] += __uint_as_float(r[i]);
+                                    for (int mb = 0; mb < MT; ++mb) {
+                                        const uint32_t a = x_addr + (uint32_t)((dy * TW + 64 * (wg * MT + mb)) * 128 + q8 * 32);
+                                        tc::wgmma_tf32<BNW>(part[mb], tc::make_desc_sw128(a), dw, first ? 0u : 1u);
+                                    }
+                                    first = false;
+                                }
+                            }
+                            tc::wgmma_commit();
+                            if (g.npass > 1) {
+                                // split mode: every stage is a chain of its own (kh * k8 <= 12 wgmma), added in fp32 registers
+                                tc::wgmma_wait<0>();
+#pragma unroll
+                                for (int mb = 0; mb < MT; ++mb) {
+                                    tc::reg_fence(part[mb]);
+#pragma unroll
+                                    for (int i = 0; i < BNW / 2; ++i) acc[mb][i] += part[mb][i];
+                                }
+                                tc::mbar_arrive(bar_empty + s);
+                                first = true;
+                            } else {
+                                tc::wgmma_wait<1>();         // the previous stage's group has retired
+                                if (pend >= 0) tc::mbar_arrive(bar_empty + pend);
+                                pend = s;
+                            }
+                            if (++s == g.stages) { s = 0; ph ^= 1; }
                         }
                     }
-                    if (g.dbg) t_ld += tma_clock() - tl0;
                 }
-                tc::fence_before_thread_sync();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(acc_empty + buf);      // this warp's tcgen05.ld of the buffer are done
+                if (pend >= 0) {
+                    tc::wgmma_wait<0>();
+#pragma unroll
+                    for (int mb = 0; mb < MT; ++mb) {
+                        tc::reg_fence(part[mb]);
+#pragma unroll
+                        for (int i = 0; i < BNW / 2; ++i) acc[mb][i] += part[mb][i];
+                    }
+                    tc::mbar_arrive(bar_empty + pend);
+                    pend = -1;
+                }
             }
-            const bool ch_ok = 4 * c4 < cv;
-            const int n = n0 + 4 * c4;                            // first of this thread's 4 channels
-            float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias != nullptr && ch_ok) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n));
+            // ---- epilogue straight from the registers: fragment i of sub-tile mb holds channels n0 + 8i + fc (+1) of the
+            // pixels fr and fr + 8 of the warpgroup's 64-pixel block
+            const int cv = min(BNW, N - n0);                     // real channels of this Cout tile (multiple of 4)
+            float bs1[BNW / 4], bs2[BNW / 4];
+#pragma unroll
+            for (int i = 0; i < BNW / 4; ++i) { bs1[i] = 0.f; bs2[i] = 0.f; }
             const long long tile_off = (long long)b * img_step + (long long)(y0 * v.out_sy + v.out_oy) * (v.out_W * N) +
-                                       (long long)(x0 * v.out_sx + v.out_ox) * N + n;
-            float bs1[4] = {0.f, 0.f, 0.f, 0.f}, bs2[4] = {0.f, 0.f, 0.f, 0.f};
+                                       (long long)(x0 * v.out_sx + v.out_ox) * N + n0;
 #pragma unroll
-            for (int rd = 0; rd < RPT; ++rd) {
-                asm volatile("bar.sync 1, 256;" ::: "memory");      // A: everybody has finished reading the previous round
-                if (loader) {
-                    const int tq = g.stack ? (quarter & 1) : quarter, plane = g.stack ? (quarter >> 1) : 0;
-                    float* dst = T + plane * (64 * TS) + (32 * half) * TS + tq * 32 + lane;
-                    if (tq * 32 + lane < CT) {            // (a 16-channel tile only has 16 real lanes)
+            for (int mb = 0; mb < MT; ++mb) {
 #pragma unroll
-                        for (int i = 0; i < 32; ++i) dst[i * TS] = accr[rd][i];     // consecutive lanes = consecutive words
-                    }
-                }
-                asm volatile("bar.sync 1, 256;" ::: "memory");      // B: the round's 64 x cv values are in T
-#pragma unroll
-                for (int k = 0; k < ITER; ++k) {
-                    const int px = px0 + k * PXSTEP;
-                    const int l = rd * 64 + px;                 // pixel index inside the tile
+                for (int h = 0; h < 2; ++h) {
+                    const int l = 64 * (wg * MT + mb) + fr + 8 * h;       // pixel index inside the tile
                     const int row = l >> g.tw_log2, col = l & (TW - 1);
-                    if (ch_ok && y0 + row < Ho && x0 + col < Wo) {
-                        float4 x = *reinterpret_cast<const float4*>(T + px * TS + 4 * c4);
-                        if (g.stack) {                          // + the lo(W) products from TMEM lanes 64 + c
-                            const float4 x2 = *reinterpret_cast<const float4*>(T + 64 * TS + px * TS + 4 * c4);
-                            x.x += x2.x; x.y += x2.y; x.z += x2.z; x.w += x2.w;
-                        }
-                        x.x += bias4.x; x.y += bias4.y; x.z += bias4.z; x.w += bias4.w;
-                        const long long off = tile_off + (long long)row * row_step + (long long)col * px_step;
+                    if (y0 + row >= p.Ho || x0 + col >= p.Wo) continue;
+                    const long long off = tile_off + (long long)row * row_step + (long long)col * px_step;
+#pragma unroll
+                    for (int i = 0; i < BNW / 8; ++i) {
+                        const int c = 8 * i + fc;
+                        if (c >= cv) continue;
+                        float2 x = make_float2(acc[mb][4 * i + 2 * h], acc[mb][4 * i + 2 * h + 1]);
+                        if (p.bias != nullptr) { const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)); x.x += bb.x; x.y += bb.y; }
                         if (p.addend != nullptr) {
-                            const float4 a = __ldg(reinterpret_cast<const float4*>(p.addend + off));
-                            x.x += a.x; x.y += a.y; x.z += a.z; x.w += a.w;
+                            const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + off + c));
+                            x.x += a.x; x.y += a.y;
                         }
-                        if (act != ACT_NONE) { x.x = tc_act(x.x, act); x.y = tc_act(x.y, act); x.z = tc_act(x.z, act); x.w = tc_act(x.w, act); }
-                        if (round) { x.x = tf32_round(x.x); x.y = tf32_round(x.y); x.z = tf32_round(x.z); x.w = tf32_round(x.w); }
-                        *reinterpret_cast<float4*>(p.out + off) = x;
-                        bs1[0] += x.x; bs1[1] += x.y; bs1[2] += x.z; bs1[3] += x.w;
-                        bs2[0] += x.x * x.x; bs2[1] += x.y * x.y; bs2[2] += x.z * x.z; bs2[3] += x.w * x.w;
+                        if (act != ACT_NONE) { x.x = tc_act(x.x, act); x.y = tc_act(x.y, act); }
+                        if (round) { x.x = tf32_round(x.x); x.y = tf32_round(x.y); }
+                        *reinterpret_cast<float2*>(p.out + off + c) = x;
+                        bs1[2 * i] += x.x; bs1[2 * i + 1] += x.y;
+                        bs2[2 * i] += x.x * x.x; bs2[2 * i + 1] += x.y * x.y;
                     }
                 }
             }
             if (p.bn_sums != nullptr) {
-                // lanes l, l + GPR, l + 2 GPR ... of a warp own the same 4 channels: butterfly them together, then one fp64
-                // atomic pair per (warp, channel).  The tile lies in one image, hence in one BatchNorm group.
+                // lanes with the same lane % 4 own the same channels: butterfly them together, then one fp64 atomic pair per
+                // (warp, channel).  The tile lies in one image, hence in one BatchNorm group.
 #pragma unroll
-                for (int o = GPR; o < 32; o <<= 1) {
+                for (int o = 4; o < 32; o <<= 1) {
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        bs1[q] += __shfl_xor_sync(0xffffffffu, bs1[q], o);
-                        bs2[q] += __shfl_xor_sync(0xffffffffu, bs2[q], o);
+                    for (int i = 0; i < BNW / 4; ++i) {
+                        bs1[i] += __shfl_xor_sync(0xffffffffu, bs1[i], o);
+                        bs2[i] += __shfl_xor_sync(0xffffffffu, bs2[i], o);
                     }
                 }
-                if (lane < GPR && ch_ok) {
+                if (lane < 4) {
                     const int grp = b / (p.B / groups);
-                    double* d = p.bn_sums + (((size_t)(w % SCSFM_BN_SLOTS) * groups + grp) * N + n) * 2;
+                    double* d = p.bn_sums + (((size_t)(w % SCSFM_BN_SLOTS) * groups + grp) * N + n0) * 2;
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        atomicAdd(d + 2 * q, (double)bs1[q]);
-                        atomicAdd(d + 2 * q + 1, (double)bs2[q]);
+                    for (int i = 0; i < BNW / 8; ++i) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int c = 8 * i + fc + e;
+                            if (c < cv) {
+                                atomicAdd(d + 2 * c, (double)bs1[2 * i + e]);
+                                atomicAdd(d + 2 * c + 1, (double)bs2[2 * i + e]);
+                            }
+                        }
                     }
                 }
             }
         }
         if (g.dbg && tid == 0) {
-            g.dbg[blockIdx.x * 8 + 5] = (unsigned long long)t_wait;
-            g.dbg[blockIdx.x * 8 + 6] = (unsigned long long)(tma_clock() - t_begin);
-            g.dbg[blockIdx.x * 8 + 0] = (unsigned long long)t_ld;        // (overwrites the producer's wait counter)
+            g.dbg[blockIdx.x * 8 + 2] = (unsigned long long)t_full;
+            g.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(clock64() - t_begin);
+            g.dbg[blockIdx.x * 8 + 7] = (unsigned long long)j;
         }
     }
-
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == TMA_EWARPS + 1) tc::tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -398,7 +306,7 @@ static int sm_count() {
     static int n = 0;
     if (n == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     }
     return n;
 }
@@ -413,15 +321,11 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
     g.tw_log2 = tw_log2;
     g.tiles_x = (p.Wo + TW - 1) / TW;
     g.tiles_y = (p.Ho + MT * TH - 1) / (MT * TH);
-    g.n_tiles = (p.Cout + TBM - 1) / TBM;
+    g.n_tiles = (p.Cout + BNW - 1) / BNW;
     g.num_work = g.tiles_x * g.tiles_y * p.B * g.n_tiles;
     g.a_bytes = ((MT * TH + v.kh - 1) * TW * 128 + 1023) / 1024 * 1024;
-    // split mode with a single <= 64-channel Cout tile: W and lo(W) stacked on the M side (see TmaGeom.stack)
-    g.stack = (BNW <= 64 && p.Cout <= 64 && p.in_lo != nullptr && p.w_lo != nullptr) ? 1 : 0;
-    g.stage_bytes = g.a_bytes + v.kh * (g.stack ? TBM : BNW) * 128;
-    // 1024 alignment slack + 1024 barrier block + ring + the MMA's over-read past a BNW-row weight tile (M = 128 rows) +
-    // the epilogue's transpose buffer T[64][BNW + 4] (two planes when stacked)
-    const int fixed = 1024 + 1024 + (g.stack ? 0 : (TBM - BNW) * 128) + (g.stack ? 2 : 1) * 64 * (BNW + 4) * 4;
+    g.stage_bytes = g.a_bytes + v.kh * BNW * 128;
+    const int fixed = 1024 + 1024;                          // 1024 alignment slack + 1024 barrier block
     g.stages = (TMA_SMEM_MAX - fixed) / g.stage_bytes;
     if (g.stages > TMA_MAX_STAGES) g.stages = TMA_MAX_STAGES;
     if (g.stages < 2) {
@@ -432,11 +336,11 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
     // split-accumulate passes: raw x raw, then lo(activations) x raw(weights), then raw(activations) x lo(weights)
     g.npass = 1; g.a_lo = 0; g.w_lo = 0;
     if (p.in_lo != nullptr) { g.a_lo |= 1 << g.npass; ++g.npass; }
-    if (p.w_lo != nullptr && !g.stack) { g.w_lo |= 1 << g.npass; ++g.npass; }
+    if (p.w_lo != nullptr) { g.w_lo |= 1 << g.npass; ++g.npass; }
     {
         const int chunks = (p.Cin + TBK - 1) / TBK;
         const int mma_per_chunk = v.kw * g.npass * v.kh * (TBK / 8);
-        // split mode: chains of ~100 MMAs (bias ~3e-6); plain TF32 (operand rounding 3e-4 dominates): one chain per tile
+        // split mode: chains of ~100 wgmma; plain TF32 (operand rounding 3e-4 dominates): one chain per tile
         g.cpg = g.npass > 1 ? (96 + mma_per_chunk - 1) / mma_per_chunk : chunks;
         if (g.cpg < 1) g.cpg = 1;
     }
@@ -486,20 +390,21 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
 
 int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
     const int N = p.Cout;
-    // weight rows kept in shared memory: the smallest of 16/32/64/128 covering Cout (Cout > 128: 128-row tiles)
+    // weight rows kept in shared memory (= wgmma N): the smallest of 16/32/64/128 covering Cout (Cout > 128: 128-row tiles)
     int bnw;
     if (N <= 16) bnw = 16;
     else if (N <= 32) bnw = 32;
     else if (N <= 64) bnw = 64;
     else bnw = 128;
-    // Pixel tile: 1 or 2 stacked 128-pixel sub-tiles (N = 128 / 256 of the MMA), TW = 8 or 16.  An MMA costs the same
-    // for N = 128 and N = 256 (measured), so a tile costs the same either way: minimise the number of waves of the
-    // persistent CTAs, then the padded area (halo rows included), then prefer the smaller tile.
+    // Pixel tile: 1 or 2 stacked 128-pixel sub-tiles, TW = 8 or 16: minimise the number of waves of the persistent CTAs,
+    // then the padded area (halo rows included), then prefer the smaller tile.  256-pixel tiles hold 2 x BNW / 2
+    // accumulators plus as many chain registers per consumer thread, so they are built for BNW <= 64 only (the heuristic
+    // picks them for Cout <= 64; forced on a wider layer they run over 64-channel Cout tiles).
     const int nsm = sm_count();
     const long nt = (N + TBM - 1) / TBM;
     int best_mt = 1, best_tw = 4;
     double best_cost = -1.0;
-    for (int mt = 1; mt <= 2; ++mt)
+    for (int mt = 1; mt <= (bnw <= 64 ? 2 : 1); ++mt)
         for (int twl = 4; twl >= 3; --twl) {
             const int tw = 1 << twl, th = mt * (TBM >> twl);
             const long ty = (p.Ho + th - 1) / th, tx = (p.Wo + tw - 1) / tw;
@@ -512,6 +417,15 @@ int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
     if (tune_mt(p)) best_mt = tune_mt(p);
     if (tune_tw(p)) best_tw = tune_tw(p);
     if (tune_bn(p)) bnw = tune_bn(p) < bnw ? bnw : tune_bn(p);       // never fewer rows than the Cout tile needs
+    if (best_mt == 2 && bnw > 64) {
+        // a forced 256-pixel tile on a wide layer: it runs over Cout tiles of 64 channels (the register budget of its
+        // 2 x 64-row accumulators); a forced wider weight tile cannot be combined with it
+        if (tune_bn(p) > 64) {
+            set_error("conv_tma: 256-pixel tiles take weight tiles of at most 64 rows (%d requested)", tune_bn(p));
+            return SCSFM_ERR_ARG;
+        }
+        bnw = 64;
+    }
     if (best_mt == 1) {
         switch (bnw) {
             case 16: return launch_tma_cfg<16, 1>(p, v, best_tw, st);
@@ -523,8 +437,7 @@ int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
     switch (bnw) {
         case 16: return launch_tma_cfg<16, 2>(p, v, best_tw, st);
         case 32: return launch_tma_cfg<32, 2>(p, v, best_tw, st);
-        case 64: return launch_tma_cfg<64, 2>(p, v, best_tw, st);
-        default: return launch_tma_cfg<128, 2>(p, v, best_tw, st);
+        default: return launch_tma_cfg<64, 2>(p, v, best_tw, st);
     }
 }
 

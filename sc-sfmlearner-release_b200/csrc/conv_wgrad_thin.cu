@@ -1,10 +1,9 @@
 // Weight gradient of the thin 3x3 decoder layers (Cout = 16, Cin in {16, 32}: SC-SfMLearner's upconv(0,0) / upconv(0,1) at
 // half / full resolution) on the fp32 FMA pipes.
 //
-// Why not the tensor cores: with pixels as the K dimension (8 per tcgen05.mma for tf32) and 16 output channels on a 128-row
-// MMA, the instruction count -- not the math -- bounds these layers (measured: ~230 cycles per MMA, 1.04 ms for the
-// 16 -> 16 layer at 12 x 256 x 832 in split mode, 11 TFLOP/s, profiles/r02_layers_tf32x3.txt), and the split-accumulate
-// passes read four tensors (x, lo(x), dout, lo(dout)).  The layer is only 11.8 GFLOP: plain fp32 FMAs need neither the low
+// Why not the tensor cores: with pixels as the K dimension (8 per tf32 MMA) and only 16 output channels per MMA, the
+// instruction count -- not the math -- bounds these layers, and the split-accumulate passes read four tensors
+// (x, lo(x), dout, lo(dout)).  The layer is only 11.8 GFLOP: plain fp32 FMAs need neither the low
 // parts (half the bytes) nor the passes, and are exact per product.
 //
 //   dW[o][dy][dx][c] += sum over the pixels (b, y, x)   dout[b, y, x, o] * in[b, y + dy - 1, x + dx - 1, c]
@@ -199,7 +198,7 @@ static int launch_thin(const ScsfmConv& p, cudaStream_t st) {
     const int tiles_x = (p.Wo + TW - 1) / TW, tiles_y = (p.Ho + Cfg::TH - 1) / Cfg::TH;
     const long long total = (long long)p.B * tiles_y * tiles_x;
     SCSFM_CHECK_ARG(total < (1LL << 31), "conv_wgrad_thin: too many tiles");
-    int nsm = 148;
+    int nsm = 132;
     {
         int dev = 0, v = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) nsm = v;

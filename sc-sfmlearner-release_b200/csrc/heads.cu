@@ -159,7 +159,7 @@ extern "C" int scsfm_head_conv_fwd(const float* in, const float* w, const float*
     const long long total = (long long)B * H * W;
     const int ppb = HT / (C / 4);
     long long g = (total + ppb - 1) / ppb;
-    if (g > 148 * 16) g = 148 * 16;
+    if (g > 132 * 16) g = 132 * 16;
     cudaStream_t st = (cudaStream_t)stream;
     switch (C / 4) {
         case 1: head_fwd_kernel<1><<<(int)g, HT, 0, st>>>(in, w, bias, out, B, H, W, act); break;
@@ -178,7 +178,7 @@ extern "C" int scsfm_head_conv_wgrad(const float* in, const float* dpre, float* 
     const int lanes = HT / (C / 4);
     const long long total = (long long)B * H * W;
     long long g = (total + (long long)lanes * 64 - 1) / ((long long)lanes * 64);     // >= 64 pixels per lane
-    if (g > 148 * 4) g = 148 * 4;
+    if (g > 132 * 4) g = 132 * 4;
     if (g < 1) g = 1;
     head_wgrad_kernel<<<(int)g, HT, 0, (cudaStream_t)stream>>>(in, dpre, dw, dbias, B, H, W, C);
     SCSFM_CHECK_LAUNCH();
@@ -189,7 +189,7 @@ extern "C" int scsfm_head_conv_dgrad(const float* dpre, const float* w, float* d
     SCSFM_CHECK_ARG(dpre && w && dpad && B > 0 && H >= 2 && W >= 2 && C >= 4 && (C & 3) == 0 && C <= 1024, "head_conv_dgrad: bad arguments");
     const long long total = (long long)B * (H + 2) * (W + 2) * (C / 4);
     long long g = (total + HT - 1) / HT;
-    if (g > 148 * 32) g = 148 * 32;
+    if (g > 132 * 32) g = 132 * 32;
     head_dgrad_kernel<<<(int)g, HT, 9 * C * sizeof(float), (cudaStream_t)stream>>>(dpre, w, dpad, B, H, W, C);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;

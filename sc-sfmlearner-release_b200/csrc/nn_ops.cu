@@ -13,7 +13,7 @@ constexpr int NT = 256;
 
 static inline int grid_for(long long n, int per_cta = NT) {
     long long g = (n + per_cta - 1) / per_cta;
-    if (g > 148LL * 32) g = 148 * 32;   // grid-stride beyond 32 CTAs per SM
+    if (g > 132LL * 32) g = 132 * 32;   // grid-stride beyond 32 CTAs per SM
     return (int)(g < 1 ? 1 : g);
 }
 
@@ -650,7 +650,7 @@ static void bn_grid(long long rpg, int C, int groups, dim3& grid, int& rpc) {
     const int slab4 = (C / 4) < NT ? (C / 4) : NT;
     const int slabs = (C / 4 + slab4 - 1) / slab4;
     const int row_lanes = NT / slab4;
-    long long want = (148LL * 6 + (long long)groups * slabs - 1) / ((long long)groups * slabs);
+    long long want = (132LL * 6 + (long long)groups * slabs - 1) / ((long long)groups * slabs);
     long long max_chunks = (rpg + 4LL * row_lanes - 1) / (4LL * row_lanes);
     if (want > max_chunks) want = max_chunks;
     if (want < 1) want = 1;
@@ -687,7 +687,7 @@ extern "C" int scsfm_bn_backward(const float* dz, const float* z, const float* y
     const int slabs = (C / 4 + slab4 - 1) / slab4;
     const int row_lanes = NT / slab4;
     // enough CTAs to fill the machine (4 per SM), at least 8 rows per row-lane per CTA
-    long long want = (148LL * 4 + (long long)groups * slabs - 1) / ((long long)groups * slabs);
+    long long want = (132LL * 4 + (long long)groups * slabs - 1) / ((long long)groups * slabs);
     long long max_chunks = (rpg + 8LL * row_lanes - 1) / (8LL * row_lanes);
     if (want > max_chunks) want = max_chunks;
     if (want < 1) want = 1;

@@ -1,6 +1,6 @@
-// Raw PTX wrappers for the Blackwell tensor-core path (sm_100a): mbarrier, tcgen05 (alloc / mma / commit /
-// ld / fences), shared-memory matrix descriptors and the instruction descriptor for kind::tf32.
-// Field layouts follow the PTX ISA "tcgen05 shared memory descriptor" / "instruction descriptor" tables.
+// Raw PTX wrappers for the Hopper tensor-core path (sm_90a): mbarrier, cp.async, TMA, wgmma (tf32, fp32 accumulate)
+// and its shared-memory matrix descriptor.  Field layouts follow the PTX ISA "warpgroup-level matrix shared memory
+// layout" / "matrix descriptor" sections.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -12,6 +12,10 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 
 __device__ __forceinline__ void st_shared_v4(uint32_t saddr, const float4& v) {
     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
+__device__ __forceinline__ void st_shared_f32(uint32_t saddr, float v) {
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory");
 }
 
 // 16-byte asynchronous global->shared copy (LDGSTS); src_bytes = 0 zero-fills the destination (out-of-image taps)
@@ -44,7 +48,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// make generic-proxy shared-memory writes visible to the async proxy (tcgen05.mma operand reads)
+// make generic-proxy shared-memory writes visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----- TMA (cp.async.bulk.tensor) ------------------------------------------------------------------
@@ -68,79 +72,110 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* tensor_map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tensor_map)) : "memory");
 }
 
-// ----- tcgen05 ------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {   // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ----- wgmma (sm_90a warpgroup MMA) -----------------------------------------------------------------
+// D[regs] (+)= A[smem] * B[smem], m64 x N x k8, tf32 operands, fp32 accumulation in the registers of the 128 threads of a
+// warpgroup.  Both operands K-major (the only layout wgmma takes for 32-bit types).  Accumulator fragment of thread t:
+// d[4i + e] holds row 16 * (t / 32) + (t % 32) / 4 + 8 * (e / 2), column 8 * i + 2 * (t % 4) + (e % 2).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_thread_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_thread_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float (&d)[8], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// TMEM -> registers: lane i of the warp gets 32 (or 16) consecutive columns of TMEM lane (lane_base + i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[32]) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
 
 // ----- descriptors ----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit):
+// wgmma shared-memory matrix descriptor (64 bit):
 //   [0,14) start address >> 4 | [16,30) leading-dim byte offset >> 4 | [32,46) stride-dim byte offset >> 4 |
-//   [46,48) version = 1 (Blackwell) | [49,52) base offset | [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
+//   [49,52) base offset | [62,64) layout: 0 none, 1 = 128B swizzle, 2 = 64B, 3 = 32B
+// K-major, 128B swizzle: rows of 128 bytes (32 floats), 8-row atoms SBO = 1024 bytes apart, LBO unused.  The K8 slice j
+// of a 32-float row starts at +32 j bytes (start address + 2 j), the swizzle being a function of the address bits.
+__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout_type & 7) << 61;
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-constexpr uint32_t LAYOUT_SW128 = 2;
-constexpr uint32_t LAYOUT_SW128_BASE32B = 1;   // 128-byte rows, 32-byte swizzle granularity: MN-major 32-bit operands
 
-// Instruction descriptor (32 bit) for kind::tf32 with fp32 accumulation:
-//   [4,6) D format (1 = F32) | [7,10) A format (2 = TF32) | [10,13) B format (2 = TF32) | [15] A major (0 = K) |
-//   [16] B major (0 = K) | [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// byte offset of element (row r, column k) of a K-major tile of 128-byte rows in the 128B-swizzled layout above
+// (16-byte chunk index XOR row % 8); the tile base must be 1024-byte aligned
+__host__ __device__ __forceinline__ uint32_t sw128_offset(int r, int k) {
+    return (uint32_t)(r * 128 + ((((k >> 2) ^ r) & 7) << 4) + ((k & 3) << 2));
 }
 
 }  // namespace tc

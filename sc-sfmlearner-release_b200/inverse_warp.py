@@ -1,6 +1,6 @@
-"""Drop-in for the reference's `inverse_warp` module (reference inverse_warp.py), B200 path.
+"""Drop-in for the reference's `inverse_warp` module (reference inverse_warp.py), H100 path.
 
-`inverse_warp2` and `pose_vec2mat` run hand-written sm_100a kernels from libscsfm
+`inverse_warp2` and `pose_vec2mat` run hand-written sm_90a kernels from libscsfm
 (csrc/warp_loss.cu) -- tensors must live on the GPU, there is no CPU fallback.  The small
 geometric helpers that the training path no longer calls separately (they are fused inside
 the loss kernel) are kept with the reference's names and argument meaning as thin device-side

@@ -1,8 +1,8 @@
-"""Drop-in for the reference's `loss_functions` module (reference loss_functions.py), B200 path.
+"""Drop-in for the reference's `loss_functions` module (reference loss_functions.py), H100 path.
 
 `compute_photo_and_geometry_loss`, `compute_pairwise_loss` and `compute_smooth_loss` keep the
 reference signatures and return zero-dim autograd-connected tensors, but each is ONE fused
-sm_100a kernel forward and one backward (csrc/warp_loss.cu, csrc/smooth.cu) instead of ~180
+sm_90a kernel forward and one backward (csrc/warp_loss.cu, csrc/smooth.cu) instead of ~180
 ATen ops per pair.  GPU tensors only: there is no CPU fallback.
 """
 import torch

@@ -87,7 +87,7 @@ class GpuAugment:
 
     def __call__(self, images, intrinsics, draws=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("GpuAugment needs a CUDA device: the B200 path has no CPU fallback")
+            raise RuntimeError("GpuAugment needs a CUDA device: the H100 path has no CPU fallback")
         if isinstance(images, (list, tuple)):
             images = torch.stack([torch.as_tensor(im) for im in images])
         images = torch.as_tensor(images)

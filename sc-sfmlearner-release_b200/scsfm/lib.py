@@ -84,7 +84,7 @@ def ptr(t):
 def dev_f32(t, name):
     """Contiguous fp32 CUDA tensor or a loud error (no silent CPU path)."""
     if not t.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor: the B200 path has no CPU fallback" % name)
+        raise RuntimeError("%s must be a CUDA tensor: the H100 path has no CPU fallback" % name)
     if t.dtype != torch.float32:
         raise TypeError("%s must be float32, got %s" % (name, t.dtype))
     return t.contiguous()

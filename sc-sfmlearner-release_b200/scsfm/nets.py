@@ -216,7 +216,7 @@ class ArenaNet(nn.Module):
         return self.ctx.mode
 
     def set_conv_mode(self, mode):
-        """"fp32" (exact CUDA-core kernels), "tf32" (tcgen05, single TF32 product) or "tf32x3" (tcgen05 with
+        """"fp32" (exact CUDA-core kernels), "tf32" (wgmma, single TF32 product) or "tf32x3" (wgmma with
         split-accumulate operands: fp32-level products, the parity mode on the tensor cores).  Returns self."""
         if mode != self.ctx.mode:
             pool, ws = self.ctx.sums_pool, self.ctx.wgrad_stream
@@ -246,7 +246,7 @@ class ArenaNet(nn.Module):
         params = list(self.parameters())
         dev = params[0].device
         if dev.type != "cuda":
-            raise RuntimeError("the B200 networks run on CUDA only (no CPU fallback): move the module with .to('cuda')")
+            raise RuntimeError("the networks run on CUDA only (no CPU fallback): move the module with .to('cuda')")
         n = sum(_aligned(p.numel()) for p in params)      # every tensor starts on a 256-byte boundary (float4 loads)
         flat = torch.zeros(n, device=dev, dtype=torch.float32)
         gflat = torch.zeros(n, device=dev, dtype=torch.float32)

@@ -17,8 +17,8 @@ OPERAND_TF32, OPERAND_RAW, OPERAND_LO = 0, 1, 2      # SCSFM_OPERAND_*
 
 # Arithmetic of the convolutions (a property of each network, see ConvCtx -- there is no process-global mode):
 #   "fp32"    exact CUDA-core kernels everywhere
-#   "tf32"    tcgen05 tensor-core kernels, single TF32 product (the reference's cuDNN default on a GPU; ~1e-3 per layer)
-#   "tf32x3"  tcgen05 kernels with split-accumulate operands: hi*hi + lo*hi + hi*lo into the same TMEM accumulator
+#   "tf32"    wgmma tensor-core kernels, single TF32 product (the reference's cuDNN default on a GPU; ~1e-3 per layer)
+#   "tf32x3"  wgmma kernels with split-accumulate operands: hi*hi + lo*hi + hi*lo, short chains added in fp32 registers
 #             (fp32-level products; the 1e-4 parity mode on the tensor cores)
 MODES = ("fp32", "tf32", "tf32x3")
 
@@ -109,7 +109,7 @@ def empty(shape, like):
 
 
 def tc_supported(kind, Cin, Cout, kh, stride):
-    """Shapes the tcgen05 kernels take; everything else runs the CUDA-core kernel."""
+    """Shapes the tensor-core kernels take; everything else runs the CUDA-core kernel."""
     if kind == "fwd":
         return Cin % 4 == 0 and Cout >= 16
     if kind == "dgrad":                      # forward kernel on dout: its "Cin" is Cout, its "Cout" is Cin

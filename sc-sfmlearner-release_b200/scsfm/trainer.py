@@ -1,5 +1,5 @@
 """One optimisation step of the reference training loop (reference train.py:259-282, 426-444) on one
-B200, and its data-parallel form: one process per GPU, each rank runs the complete step on its shard of
+H100, and its data-parallel form: one process per GPU, each rank runs the complete step on its shard of
 the batch, the two gradient arenas are all-reduced (NCCL over NVLink) as soon as the backward of the
 owning network has finished, then every rank applies the identical fused Adam update.
 """

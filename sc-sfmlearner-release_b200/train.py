@@ -1,4 +1,4 @@
-"""Training entry with the reference's command line (reference train.py:24-61) on the B200 path.
+"""Training entry with the reference's command line (reference train.py:24-61) on the H100 path.
 
     python train.py DIR --name EXP [--resnet-layers 18 -b 4 -s 0.1 -c 0.5 --with-auto-mask 1 ...]
     torchrun --nproc-per-node 8 train.py DIR --name EXP ...        # data parallel, one process per GPU
@@ -32,7 +32,7 @@ from loss_functions import compute_errors, compute_photo_and_geometry_loss, comp
 from scsfm import nnops, synth
 from scsfm.trainer import Trainer, compute_depth, compute_pose_with_inv
 
-parser = argparse.ArgumentParser(description="SC-SfMLearner training on KITTI / NYU (B200 path)",
+parser = argparse.ArgumentParser(description="SC-SfMLearner training on KITTI / NYU (H100 path)",
                                  formatter_class=argparse.ArgumentDefaultsHelpFormatter)
 parser.add_argument("data", metavar="DIR", help="path to dataset, or 'synthetic'")
 parser.add_argument("--folder-type", type=str, choices=["sequence", "pair"], default="sequence", help="the dataset dype to train")
@@ -70,8 +70,8 @@ parser.add_argument("--padding-mode", type=str, choices=["zeros", "border"], def
 parser.add_argument("--with-gt", action="store_true", help="use ground truth for validation (npy depth maps, see the reference's data/kitti_raw_loader.py)")
 # additions of this implementation
 parser.add_argument("--conv-mode", choices=["fp32", "tf32", "tf32x3"], default="tf32x3",
-                    help="tf32x3 = tcgen05 tensor cores with split-accumulate operands (fp32-level results, the parity mode); tf32 = "
-                         "tcgen05 single TF32 product (cuDNN's default arithmetic, fastest); fp32 = exact CUDA-core convolutions")
+                    help="tf32x3 = wgmma tensor cores with split-accumulate operands (fp32-level results, the parity mode); tf32 = "
+                         "wgmma single TF32 product (cuDNN's default arithmetic, fastest); fp32 = exact CUDA-core convolutions")
 parser.add_argument("--cuda-graph", type=int, default=1, help="capture the training step in a CUDA graph (single GPU)")
 parser.add_argument("--overlap", type=int, default=1, help="run PoseResNet next to DispResNet and the weight gradients on side streams")
 parser.add_argument("--synthetic-size", type=int, nargs=2, default=[256, 832], metavar=("H", "W"))
@@ -233,7 +233,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("train.py drives the B200 kernels: a CUDA device is required (no CPU fallback)")
+        raise SystemExit("train.py drives the H100 kernels: a CUDA device is required (no CPU fallback)")
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     if world > 1:

@@ -1,8 +1,8 @@
 """Writes tests/golden/augment.npz: inputs, random draws and outputs of the UNMODIFIED reference transform chain
 (custom_transforms.py: RandomHorizontalFlip, RandomScaleCrop, ArrayToTensor, Normalize) on small seeded samples.
 
-Run in the build container (needs /root/reference; Pillow does the resize inside the reference code):
-    python tests/golden/make_golden_augment.py
+Needs a checkout of the original project (Pillow does the resize inside its code):
+    python tests/golden/make_golden_augment.py /path/to/SC-SfMLearner-Release
 The draws are recorded by replaying the reference's RNG call order (random.random(); np.random.uniform(1, 1.15, 2);
 np.random.randint(scaled_h - in_h + 1); np.random.randint(scaled_w - in_w + 1)) from the same seeds.
 """
@@ -13,7 +13,7 @@ import sys
 import numpy as np
 
 sys.dont_write_bytecode = True
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.abspath(sys.argv[1]))
 import custom_transforms as T  # noqa: E402  (the reference's)
 
 HERE = os.path.dirname(os.path.abspath(__file__))

@@ -7,19 +7,38 @@ def t(a, dtype=torch.float32, device="cpu"):
     return torch.from_numpy(np.asarray(a)).to(device=device, dtype=dtype)
 
 
+SUB = (Ellipsis, slice(None, None, 2), slice(None, None, 2))      # the stored maps keep every second row and column
+
+
+def _warp_inputs():
+    """The seeded inputs the golden vectors of warp_loss.npz were computed from (tests/golden/make_golden.py)."""
+    from scsfm import synth
+    d = synth.loss_inputs(7, 2, 64, 128, n_ref=2, n_scales=2)
+    return (d["tgt_img"], d["ref_imgs"], d["intrinsics"], d["tgt_depth"], d["ref_depths"], [p * 3 for p in d["poses"]],
+            [p * 3 for p in d["poses_inv"]])
+
+
 def golden_loss_inputs(g, dtype=torch.float32, device="cpu", n_scales=2, requires_grad=False):
-    """Rebuild the (tgt_img, ref_imgs, K, tgt_depth, ref_depths, poses, poses_inv) tuple of warp_loss.npz."""
-    def leaf(a):
-        x = t(a, dtype, device)
-        return x.requires_grad_(True) if requires_grad else x
-    tgt = t(g["in_tgt_img"], dtype, device)
-    refs = [t(g[f"in_ref_img{i}"], dtype, device) for i in range(2)]
-    K = t(g["in_K"], dtype, device)
-    td = [leaf(g[f"in_tgt_depth_s{s}"]) for s in range(n_scales)]
-    rd = [[leaf(g[f"in_ref_depth{i}_s{s}"]) for s in range(n_scales)] for i in range(2)]
-    ps = [leaf(g[f"in_pose{i}"]) for i in range(2)]
-    pi = [leaf(g[f"in_pose_inv{i}"]) for i in range(2)]
-    return tgt, refs, K, td, rd, ps, pi
+    """Rebuild the (tgt_img, ref_imgs, K, tgt_depth, ref_depths, poses, poses_inv) tuple behind warp_loss.npz, checked against
+    the stored checksums."""
+    tgt, refs, K, td, rd, ps, pi = _warp_inputs()
+    flat = [tgt, *refs, K, *td, *[x for r in rd for x in r], *ps, *pi]
+    np.testing.assert_allclose([float(x.double().abs().sum()) for x in flat], g["in_checksum"], rtol=1e-6)
+
+    def conv(x, leaf=False):
+        x = x.detach().to(device=device, dtype=dtype)
+        return x.requires_grad_(True) if leaf and requires_grad else x
+    return (conv(tgt), [conv(r) for r in refs], conv(K), [conv(x, True) for x in td[:n_scales]],
+            [[conv(x, True) for x in r[:n_scales]] for r in rd], [conv(x, True) for x in ps], [conv(x, True) for x in pi])
+
+
+def error_pair():
+    """The synthetic ground truth / prediction pair of the compute_errors golden values."""
+    g = torch.Generator().manual_seed(3)
+    gt = torch.rand(2, 64, 128, generator=g) * 90
+    gt[gt < 9] = 0
+    pred = (gt * (1 + 0.2 * torch.randn(2, 64, 128, generator=g))).abs() * 0.37 + 0.05
+    return gt, pred
 
 
 def rel_l2(a, b):
@@ -59,13 +78,14 @@ def make_disk_dataset(root, H=128, W=160, scenes=("scene_a", "scene_b", "scene_v
 
 
 def reference_loader_env():
-    """Environment for a subprocess in which the reference's host-side loaders (datasets/*.py, custom_transforms.py: the
-    unmodified copy under baseline/_ref, plus the stand-ins for path / imageio under baseline/stubs) are importable from
-    PYTHONPATH, as train.py expects for real datasets.  None if baseline/_ref is absent (python __graft_entry__.py makes it)."""
+    """Environment for a subprocess in which the original project's host-side loaders (datasets/*.py, custom_transforms.py as
+    installed by __graft_entry__.build() into oracle/_ref/, or $SCSFM_REFERENCE_DIR, plus the stand-ins for path / imageio under
+    baseline/stubs) are importable from PYTHONPATH, as train.py expects for real datasets.  None if neither holds them."""
     import os
+    from oracle import reference
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    ref, stubs = os.path.join(root, "baseline", "_ref"), os.path.join(root, "baseline", "stubs")
-    if not os.path.exists(os.path.join(ref, "datasets", "sequence_folders.py")):
+    ref, stubs = reference.installed(), os.path.join(root, "baseline", "stubs")
+    if ref is None:
         return None
     env = dict(os.environ)
     env["PYTHONPATH"] = os.pathsep.join([stubs, ref] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))

@@ -169,7 +169,7 @@ def _build(kind, layers, mode="fp32"):
 @pytest.mark.parametrize("kind", ["disp", "pose"])
 def test_networks_vs_reference_vectors_and_oracle(golden_nets, layers, kind, mode):
     """Train-mode forward, backward (every parameter gradient), BN running stats and eval-mode forward, in both 1e-4
-    parity modes: exact CUDA-core convolutions ("fp32") and split-accumulate tcgen05 convolutions ("tf32x3")."""
+    parity modes: exact CUDA-core convolutions ("fp32") and split-accumulate tensor-core convolutions ("tf32x3")."""
     from oracle import nets as N
     g = golden_nets
     tag = f"{kind}{layers}"
@@ -217,7 +217,7 @@ def test_networks_vs_reference_vectors_and_oracle(golden_nets, layers, kind, mod
     # this GPU with TF32 off.  These deliberately ill-conditioned test networks (random weights, BatchNorm over 12 samples at the
     # deepest stage) amplify fp32 rounding by 1e2..1e4 and a single ReLU / max-pool decision that flips on a ~0 activation moves
     # every upstream gradient at once: the round-1 "ResNet-50 drift" (1.5e-3 vs 1.5e-4) was exactly that -- tools/diag_grad_error.py
-    # shows the CPU oracle itself at 4.4e-3 on another run (profiles/r02_diag_disp50_fp32.txt).  Hence two yardsticks, no per-depth slack.
+    # shows the CPU oracle itself at 4.4e-3 on another run.  Hence two yardsticks, no per-depth slack.
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     g64, g32, g32gpu = oracle_grads(torch.float64), oracle_grads(torch.float32), oracle_grads(torch.float32, DEV)
@@ -319,9 +319,10 @@ TC_CASES = [
 
 
 # ScsfmConv.tune words (nnops.tune): the heuristic, the cp.async gather kernel alone (+ the cp.async weight-gradient
-# kernel), and two forced tilings of the persistent TMA kernel (128 / 256 pixels per MMA, 8- / 16-pixel-wide tiles;
-# forcing also sends small reflection-padded layers through the zero-padded TMA pass + border-ring pass), the second one
-# together with the TMA weight-gradient kernel
+# kernel), and two forced tilings of the persistent TMA kernel (128 / 256-pixel tiles -- the latter over 64-channel Cout
+# tiles on the wider layers; 8- / 16-pixel-wide tiles; forcing also sends small reflection-padded layers through the
+# zero-padded TMA pass + border-ring pass), the second one with the weight-gradient selector value 2, which selects the
+# tensor-core weight-gradient kernel (the id keeps its historical name "wgradtma")
 TMA_CONFIGS = {"auto": dict(), "gather": dict(no_tma=1, wgrad=1), "tma-128px-tw8": dict(mt=1, tw_log2=3),
                "tma-256px-tw16-wgradtma": dict(mt=2, tw_log2=4, wgrad=2)}
 
@@ -330,9 +331,9 @@ TMA_CONFIGS = {"auto": dict(), "gather": dict(no_tma=1, wgrad=1), "tma-128px-tw8
 @pytest.mark.parametrize("tma", sorted(TMA_CONFIGS))
 @pytest.mark.parametrize("case", TC_CASES)
 def test_tcgen05_conv_fwd_and_dgrad_vs_fp64(case, tma, mode):
-    """tcgen05 kernels.  "tf32": operands rounded to nearest TF32 by their producers, one product, fp32 accumulation:
-    expected relative L2 error ~3e-4, bound 1e-3.  "tf32x3": raw fp32 operands + their low parts, three products into the
-    same TMEM accumulator: fp32-level accuracy, bound 1e-5 (north_star: 1e-4)."""
+    """Tensor-core (wgmma) kernels.  "tf32": operands rounded to nearest TF32 by their producers, one product, fp32 accumulation:
+    expected relative L2 error ~3e-4, bound 1e-3.  "tf32x3": raw fp32 operands + their low parts, three products into
+    short accumulation chains: fp32-level accuracy, bound 1e-5 (north_star: 1e-4)."""
     O = _ops()
     cx = O.ConvCtx(mode)
     cx.tune = O.tune(**TMA_CONFIGS[tma])
@@ -394,7 +395,7 @@ THIN_CASES = [
     (4, 64, 320, 16, 1),     # 320 tiles: more than one tile per CTA (double-buffered staging)
     (2, 9, 21, 32, 1),       # Cin 32: 16-pixel-wide tiles
     (2, 16, 16, 32, 0),
-    (3, 64, 208, 32, 1),     # 312 tiles on 148 CTAs
+    (3, 64, 208, 32, 1),     # 312 tiles: more than two per CTA
 ]
 
 

@@ -5,7 +5,7 @@ import pytest
 import torch
 
 from golden_util import det_image, det_weights
-from helpers import frac_within, golden_loss_inputs, rel_l2, t
+from helpers import SUB, error_pair, frac_within, golden_loss_inputs, rel_l2, t
 from oracle import geometry as G
 from oracle import losses as L
 from oracle import nets as N
@@ -16,6 +16,7 @@ def test_inverse_warp2_maps(golden_warp, pm):
     g = golden_warp
     tgt, refs, K, td, rd, ps, pi = golden_loss_inputs(g)
     w, v, pd, cd = G.inverse_warp2(refs[0], td[0], rd[0][0], ps[0], K, pm)
+    w, v, pd, cd = w[SUB], v[SUB], pd[SUB], cd[SUB]
     assert torch.equal(v, t(g[f"{pm}_valid"]))
     np.testing.assert_allclose(w.numpy(), g[f"{pm}_warped"], atol=2e-5)
     np.testing.assert_allclose(pd.numpy(), g[f"{pm}_proj_depth"], atol=2e-6)
@@ -59,9 +60,9 @@ def test_gradients_fp32_and_fp64(golden_warp, pm, flags):
                 return rel_l2(a, b) < tol
             return frac_within(a, b, 1e-4) > 0.995
         for sidx in range(2):
-            assert close(td[sidx].grad, g[f"{tag}_tgt_depth_s{sidx}"])
+            assert close(td[sidx].grad[SUB], g[f"{tag}_tgt_depth_s{sidx}"])
             for i in range(2):
-                assert close(rd[i][sidx].grad, g[f"{tag}_ref_depth{i}_s{sidx}"])
+                assert close(rd[i][sidx].grad[SUB], g[f"{tag}_ref_depth{i}_s{sidx}"])
         for i in range(2):
             assert rel_l2(ps[i].grad, g[f"{tag}_pose{i}"]) < (1e-3 if dtype == torch.float32 else 5e-2)
             assert rel_l2(pi[i].grad, g[f"{tag}_pose_inv{i}"]) < (1e-3 if dtype == torch.float32 else 5e-2)
@@ -85,13 +86,13 @@ def test_pose_matrices_and_legacy_warp(golden_warp):
     np.testing.assert_allclose(G.pose_to_matrix(vec, "quat").numpy(), g["pose_mat_quat"], atol=1e-6)
     tgt, refs, K, td, rd, ps, pi = golden_loss_inputs(g)
     w, v = G.inverse_warp(refs[0], td[0][:, 0], ps[0], K, "euler", "zeros")
-    np.testing.assert_allclose(w.numpy(), g["legacy_warped"], atol=2e-5)
-    assert np.array_equal(v.numpy(), g["legacy_valid"])
+    np.testing.assert_allclose(w[SUB].numpy(), g["legacy_warped"], atol=2e-5)
+    assert np.array_equal(v[SUB].numpy(), g["legacy_valid"])
 
 
 def test_compute_errors(golden_warp):
     g = golden_warp
-    gt, pred = t(g["err_gt"]), t(g["err_pred"])
+    gt, pred = error_pair()
     np.testing.assert_allclose(L.compute_errors(gt, pred, "kitti"), g["err_kitti"], rtol=1e-5)
     np.testing.assert_allclose(L.compute_errors(gt.clamp(max=12), pred, "nyu"), g["err_nyu"], rtol=1e-5)
 

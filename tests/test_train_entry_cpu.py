@@ -1,5 +1,5 @@
-"""Host-side behaviour of the train.py entry that needs no GPU: checkpoint files (reference utils.py:57-66 layout, loadable by
-the reference's own modules), CLI defaults, ImageNet initialisation from a local file."""
+"""Host-side behaviour of the train.py entry that needs no GPU: checkpoint files (reference utils.py:57-66 layout, with the
+reference modules' state_dict keys and shapes), CLI defaults, ImageNet initialisation from a local file."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,6 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
 
 
 def test_save_checkpoint_layout_and_roundtrip(tmp_path):
@@ -29,24 +28,28 @@ def test_save_checkpoint_layout_and_roundtrip(tmp_path):
         assert w.is_contiguous() and tuple(w.shape) == (64, 64, 3, 3)      # plain OIHW tensors, not arena views
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(REF, "models", "DispResNet.py")), reason="baseline/_ref (copy of the reference) not installed")
 @pytest.mark.parametrize("layers", [18, 50])
-def test_checkpoints_load_into_the_unmodified_reference_modules(tmp_path, layers):
-    """The files train.py writes must be usable by the reference's test / inference scripts (strict load_state_dict into the
-    reference's own models.DispResNet / PoseResNet), in a clean interpreter so that the two `models` packages do not mix."""
+def test_checkpoints_load_into_the_unmodified_reference_modules(tmp_path, golden_nets, layers):
+    """The files train.py writes must be usable by the reference's test / inference scripts, i.e. load strictly into the
+    reference's own models.DispResNet / PoseResNet: the same state_dict keys in the same order with the same shapes as those
+    modules have (recorded from them in tests/golden/nets.npz), and the networks rebuilt from the files give outputs of the
+    reference's shapes."""
     import models
     import train as T
     disp, pose = models.DispResNet(layers, False), models.PoseResNet(18, False)
     T.save_checkpoint(str(tmp_path), {"epoch": 1, "state_dict": disp.state_dict()}, {"epoch": 1, "state_dict": pose.state_dict()}, False)
-    code = ("import sys, torch; sys.dont_write_bytecode = True; sys.path.insert(0, %r); import models\n"
-            "d = models.DispResNet(%d, False); d.load_state_dict(torch.load(%r)['state_dict'])\n"
-            "p = models.PoseResNet(18, False); p.load_state_dict(torch.load(%r)['state_dict'])\n"
-            "x = torch.zeros(1, 3, 64, 96); d.eval(); p.eval()\n"
-            "print('OK', tuple(d(x).shape), tuple(p(x, x).shape))\n"
-            % (REF, layers, os.path.join(tmp_path, "dispnet_checkpoint.pth.tar"), os.path.join(tmp_path, "exp_pose_checkpoint.pth.tar")))
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert "OK (1, 1, 64, 96) (1, 6)" in out.stdout
+    for prefix, tag in (("dispnet", "disp%d" % layers), ("exp_pose", "pose18")):
+        sd = torch.load(os.path.join(tmp_path, prefix + "_checkpoint.pth.tar"))["state_dict"]
+        assert list(sd.keys()) == list(golden_nets[tag + "_keys"])
+        assert ["x".join(map(str, v.shape)) for v in sd.values()] == list(golden_nets[tag + "_shapes"])
+    from oracle import nets as N
+    d, p = N.DispResNet(layers), N.PoseResNet(18)
+    d.load_state_dict(torch.load(os.path.join(tmp_path, "dispnet_checkpoint.pth.tar"))["state_dict"])
+    p.load_state_dict(torch.load(os.path.join(tmp_path, "exp_pose_checkpoint.pth.tar"))["state_dict"])
+    d.eval(); p.eval()
+    x = torch.zeros(1, 3, 64, 96)
+    with torch.no_grad():
+        assert tuple(d(x).shape) == (1, 1, 64, 96) and tuple(p(x, x).shape) == (1, 6)
 
 
 def test_cli_defaults_and_pretrained_weights(tmp_path, monkeypatch):
@@ -80,12 +83,12 @@ def test_real_dataset_loaders_host_side(tmp_path):
     from helpers import make_disk_dataset, reference_loader_env
     env = reference_loader_env()
     if env is None:
-        pytest.skip("baseline/_ref (copy of the reference made by __graft_entry__.build()) is not present")
+        pytest.skip("the original project's modules are not installed (oracle/_ref/, made by __graft_entry__.build())")
     data = make_disk_dataset(str(tmp_path / "data"))
     pkg = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "sc-sfmlearner-release_b200")
     code = ("import sys; sys.path.insert(0, %r)\n"
             "import numpy as np, torch, train as T\n"
-            "SF = T._reference_dataset_module('sequence_folders'); assert 'baseline' in SF.__file__, SF.__file__\n"
+            "SF = T._reference_dataset_module('sequence_folders'); assert SF.__file__.startswith(%r), SF.__file__\n"
             "for g in (0, 1):\n"
             "    args = T.parser.parse_args([%r, '--name', 'x', '-b', '2', '-j', '0', '--gpu-augment', str(g)])\n"
             "    class NoGpu(T.GpuAugmentLoader):\n"
@@ -103,7 +106,7 @@ def test_real_dataset_loaders_host_side(tmp_path):
             "        print('VAL', tuple(tgt.shape), len(refs), len(vl))\n"
             "    else:\n"
             "        frames, K = next(iter(vl.loader))\n"
-            "        print('VALRAW', tuple(frames.shape), frames.dtype, len(vl.loader))\n" % (pkg, data))
+            "        print('VALRAW', tuple(frames.shape), frames.dtype, len(vl.loader))\n" % (pkg, env["PYTHONPATH"].split(os.pathsep)[1], data))
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, env=env)
     assert out.returncode == 0, out.stderr[-3000:]
     lines = out.stdout.strip().splitlines()

@@ -13,7 +13,7 @@ DEV = "cuda"
 
 @pytest.mark.parametrize("mode", ["fp32", "tf32x3"])
 def test_two_training_steps_match_the_oracle(mode):
-    """Both 1e-4 parity modes: exact CUDA-core convolutions and split-accumulate tcgen05 convolutions."""
+    """Both 1e-4 parity modes: exact CUDA-core convolutions and split-accumulate tensor-core convolutions."""
     import models
     from oracle import nets as N
     from oracle import step as OS

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import frac_within, golden_loss_inputs, rel_l2, t
+from helpers import SUB, error_pair, frac_within, golden_loss_inputs, rel_l2, t
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -30,6 +30,7 @@ def test_inverse_warp2_maps_vs_reference(golden_warp, pm):
     g = golden_warp
     tgt, refs, K, td, rd, ps, pi = golden_loss_inputs(g, device=DEV)
     w, v, pd, cd = iw.inverse_warp2(refs[0], td[0], rd[0][0], ps[0], K, pm)
+    w, v, pd, cd = w[SUB], v[SUB], pd[SUB], cd[SUB]
     v_ref = t(g[f"{pm}_valid"], device=DEV)
     flips = (v != v_ref)
     assert int(flips.sum()) <= 4
@@ -76,8 +77,8 @@ def test_gradients_vs_reference_and_fp64_oracle(golden_warp, pm, flags):
     (po + 0.5 * qo + 0.1 * so).backward()
 
     def dense(mine, ref32, ref64):
-        assert frac_within(mine.grad, ref32, 1e-4) > 0.995
-        assert rel_l2(mine.grad, ref64.grad) < 3 * rel_l2(ref32, ref64.grad) + 1e-4
+        assert frac_within(mine.grad[SUB], ref32, 1e-4) > 0.995
+        assert rel_l2(mine.grad[SUB], ref64.grad[SUB]) < 3 * rel_l2(ref32, ref64.grad[SUB]) + 1e-4
 
     def small(mine, ref32, ref64):
         assert rel_l2(mine.grad, ref64.grad) < 3 * rel_l2(ref32, ref64.grad) + 2e-4
@@ -202,8 +203,8 @@ def test_pose_matrices_and_legacy_warp(golden_warp):
     np.testing.assert_allclose(iw.pose_vec2mat(vec).detach().cpu().numpy(), g["pose_mat_euler"], atol=1e-6)
     tgt, refs, K, td, rd, ps, pi = golden_loss_inputs(g, device=DEV)
     w, v = iw.inverse_warp(refs[0], td[0][:, 0], ps[0], K, "euler", "zeros")
-    np.testing.assert_allclose(w.cpu().numpy(), g["legacy_warped"], atol=1e-4)
-    assert int((v.cpu().numpy() != g["legacy_valid"]).sum()) <= 4
+    np.testing.assert_allclose(w[SUB].cpu().numpy(), g["legacy_warped"], atol=1e-4)
+    assert int((v[SUB].cpu().numpy() != g["legacy_valid"]).sum()) <= 4
 
 
 def test_error_behaviour_matches_reference():
@@ -226,11 +227,12 @@ def test_compute_errors_and_ssim_module(golden_warp):
     from oracle import losses as OL
     _, lf = _api()
     g = golden_warp
-    gt, pred = t(g["err_gt"], device=DEV), t(g["err_pred"], device=DEV)
+    gt, pred = (x.to(DEV) for x in error_pair())
     np.testing.assert_allclose(lf.compute_errors(gt, pred, "kitti"), g["err_kitti"], rtol=1e-4)
     np.testing.assert_allclose(lf.compute_errors(gt.clamp(max=12), pred, "nyu"), g["err_nyu"], rtol=1e-4)
-    x, y = t(g["in_tgt_img"], device=DEV), t(g["in_ref_img0"], device=DEV)
-    want = OL.ssim_dissimilarity(t(g["in_tgt_img"]), t(g["in_ref_img0"]))
+    c = golden_loss_inputs(g)
+    x, y = c[0].to(DEV), c[1][0].to(DEV)
+    want = OL.ssim_dissimilarity(c[0], c[1][0])
     np.testing.assert_allclose(lf.compute_ssim_loss(x, y).cpu().numpy(), want.numpy(), atol=1e-5)
 
 

@@ -91,7 +91,8 @@ def main():
     g = torch.Generator().manual_seed(0)
     bad = 0
     totals = {(c, p): 0.0 for c, _ in cfgs for p in passes}
-    names = ["epi tmem-ld | prod wait-empty (wgrad)", "prod total", "mma wait-full", "mma wait-acc", "mma total", "epi wait-acc", "epi total", "tiles"]
+    # the counters conv_tma_kernel writes per CTA (slot: meaning, in cycles); slot 7 = tiles
+    names = {0: "producer wait-empty", 1: "producer total", 2: "consumer wait-full", 4: "consumer total"}
     for (name, B, H, W, Cin, Cout, k, s, pad, reflect) in LAYERS:
         if args.only and args.only not in name:
             continue
@@ -164,7 +165,7 @@ def main():
                     if d_.shape[0]:
                         m = d_.mean(0)
                         print("      roles (%d CTAs, %.1f tiles/CTA): " % (d_.shape[0], m[7]) +
-                              "  ".join("%s=%.0f" % (n, v) for n, v in zip(names[:7], m[:7].tolist())), flush=True)
+                              "  ".join("%s=%.0f" % (n, float(m[k])) for k, n in names.items()), flush=True)
     for (c, p), t in totals.items():
         print("total %-5s %-5s %.3f ms" % (c, p, t))
     print("MISMATCHES: %d" % bad)

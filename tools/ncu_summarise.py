@@ -13,7 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FAMILY_KERNELS = {          # bench.py family -> kernels that implement it (the TMA kernel serves fwd and dgrad alike)
-    "conv_wgrad_tc": ["conv_wgrad_tc_kernel", "conv_wgrad_tma_kernel", "conv_wgrad_thin_kernel"],
+    "conv_wgrad_tc": ["conv_wgrad_tc_kernel", "conv_wgrad_thin_kernel"],
     "conv_fwd_tc": ["conv_tma_kernel", "conv_fwd_tc_kernel"],
     "conv_dgrad_tc": ["conv_tma_kernel", "conv_fwd_tc_kernel"],
     "bn_bwd": ["bn_bwd_reduce_kernel", "bn_bwd_apply_kernel", "bn_param_grad_kernel"],
