@@ -195,7 +195,7 @@ typedef struct ScsfmConv {
 #define SCSFM_TUNE_MT(mt) (((unsigned)(mt) & 3u) << 4)       /* TMA kernel: 1|2 stacked 128-pixel sub-tiles (0 = auto) */
 #define SCSFM_TUNE_TW(l2) (((unsigned)((l2) ? (l2) - 2 : 0) & 3u) << 6)   /* TMA kernel: tile width log2 3|4 (0 = auto) */
 #define SCSFM_TUNE_BN(bn) (((bn) == 16 ? 1u : (bn) == 32 ? 2u : (bn) == 64 ? 3u : (bn) == 128 ? 4u : 0u) << 8)  /* weight rows in smem */
-#define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 or 2 tensor-core kernel, 3 thin-layer fp32 kernel */
+#define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 gather kernel, 2 TMA kernel, 3 thin-layer fp32 kernel */
 
 /* Exact-fp32 implicit-GEMM convolution on CUDA cores (every shape). */
 int scsfm_conv2d_fwd_simt(const ScsfmConv* p, void* stream);

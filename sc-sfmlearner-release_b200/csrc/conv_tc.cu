@@ -32,32 +32,29 @@ __device__ __forceinline__ void gather_consume(float (&acc)[BN / 2], uint8_t* sA
     float part[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int pend = -1;                                       // stage whose wgmma group may still be in flight
-    for (int it = 0; it < total; ++it) {
-        const int s = it % STAGES;
-        tc::mbar_wait(bar_full + s, (it / STAGES) & 1);
-        tc::fence_proxy_async();                         // cp.async / st.shared (generic proxy) writes -> wgmma (async proxy) reads
-        const uint32_t a_addr = tc::smem_u32(sA + s * A_BYTES), b_addr = tc::smem_u32(sB + s * B_BYTES);
-        const bool first = it % chain == 0;
-        tc::reg_fence(part);
-        tc::wgmma_fence();
-#pragma unroll
-        for (int j = 0; j < TBK / 8; ++j)
-            tc::wgmma_tf32<BN>(part, tc::make_desc_sw128(a_addr + j * 32), tc::make_desc_sw128(b_addr + j * 32), (first && j == 0) ? 0u : 1u);
-        tc::wgmma_commit();
-        if (it % chain == chain - 1 || it == total - 1) {
-            tc::wgmma_wait<0>();
+    // One chain per outer iteration.  Every wgmma sits on the same straight-line path and the only wgmma_wait<0> follows
+    // the inner loop: a wait that depends on a per-iteration branch makes ptxas serialise the wgmma (C7518).
+    for (int it0 = 0; it0 < total; it0 += chain) {
+        const int it1 = min(total, it0 + chain);
+        for (int it = it0; it < it1; ++it) {
+            const int s = it % STAGES;
+            tc::mbar_wait(bar_full + s, (it / STAGES) & 1);
+            tc::fence_proxy_async();                     // cp.async / st.shared (generic proxy) writes -> wgmma (async proxy) reads
+            const uint32_t a_addr = tc::smem_u32(sA + s * A_BYTES), b_addr = tc::smem_u32(sB + s * B_BYTES);
             tc::reg_fence(part);
-            if (pend >= 0) tc::mbar_arrive(bar_empty + pend);
-            tc::mbar_arrive(bar_empty + s);
-            pend = -1;
+            tc::wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-        } else {
+            for (int j = 0; j < TBK / 8; ++j)
+                tc::wgmma_tf32<BN>(part, tc::make_desc_sw128(a_addr + j * 32), tc::make_desc_sw128(b_addr + j * 32), (it == it0 && j == 0) ? 0u : 1u);
+            tc::wgmma_commit();
             tc::wgmma_wait<1>();                         // the previous stage's group has retired
-            if (pend >= 0) tc::mbar_arrive(bar_empty + pend);
-            pend = s;
+            if (it > it0) tc::mbar_arrive(bar_empty + (it - 1) % STAGES);
         }
+        tc::wgmma_wait<0>();
+        tc::reg_fence(part);
+        tc::mbar_arrive(bar_empty + (it1 - 1) % STAGES);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
     }
 }
 
@@ -350,9 +347,11 @@ struct WgCfg {
 
 // STACK = true (split mode, Cout <= BN / 2): the N-side tile holds dout in rows [0, BN/2) and lo(dout) in [BN/2, BN), so the two
 // passes lo(in) and in give all four products (columns o and BN/2 + o are both added into dw[o]): 2 passes instead of 3.
+// border = 1: the pixels (K) are only the 2*(Ho+Wo)-4 image-border pixels per image (border_pixel), the reflection-padded
+// ring that the TMA weight-gradient kernel leaves out.
 template <int BN, bool STACK = false>
 __global__ void __launch_bounds__(FW_THREADS)
-conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split) {
+conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split, int border) {
     using Cfg = WgCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -363,7 +362,7 @@ conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split) {
     uint64_t* bar_empty = bar_full + STAGES;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int HWo = p.Ho * p.Wo;
+    const int HWo = border ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo;
     const int Mtot = p.kh * p.kw * p.Cin, N = p.Cout, npix = p.B * HWo;
     const int m0 = blockIdx.x * GBM, n0 = blockIdx.y * BN;
     const int pix_begin = blockIdx.z * pix_per_split, pix_end = min(npix, pix_begin + pix_per_split);
@@ -406,12 +405,19 @@ conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split) {
         // Software-pipelined: the global loads of k-block it+1 are in flight while this thread waits for k-block it's stage
         // and stores it transposed.  (fq, fpx, fb, fho, fwo) is the position of the next k-block to fetch, across the
         // passes (low-part passes first: added while the sums are small; raw x raw last).
-        int fq = 0, fkb = 0, fpx = pix_begin + lane, fb, fho, fwo;
-        {
+        int fq = 0, fkb = 0, fpx = pix_begin + lane, fb, fho, fwo, frow;   // frow: dout row of the pixel
+        auto locate = [&]() {
             const int rem = fpx - (fb = fpx / HWo) * HWo;
-            fho = rem / p.Wo;
-            fwo = rem - fho * p.Wo;
-        }
+            if (border) {
+                border_pixel(rem, p.Ho, p.Wo, fho, fwo);
+                frow = (fb * p.Ho + fho) * p.Wo + fwo;
+            } else {
+                fho = rem / p.Wo;
+                fwo = rem - fho * p.Wo;
+                frow = fpx;
+            }
+        };
+        locate();
         auto fetch = [&](float4 (&va)[A_IT], float4 (&vb)[B_IT]) {
             const int ps = (fq + 1) % npass;
             const float* a_base = (ps == 1 && p.in_lo != nullptr) ? p.in_lo : p.in;
@@ -433,18 +439,20 @@ conv_wgrad_tc_kernel(ScsfmConv p, int pix_per_split) {
                 const int nn = STACK ? col - (lo_half ? BN / 2 : 0) : n0 + col;
                 const bool ok = px_ok && nn < N;
                 const float* bb = lo_half ? p.dout_lo : b_main;
-                vb[i] = ok ? __ldg(reinterpret_cast<const float4*>(bb + (size_t)fpx * N + nn)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                vb[i] = ok ? __ldg(reinterpret_cast<const float4*>(bb + (size_t)frow * N + nn)) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
             // advance to the next k-block: 32 pixels further, or the first k-block of the next pass
             if (++fkb == KB) {
                 fkb = 0;
                 ++fq;
                 fpx = pix_begin + lane;
-                const int rem = fpx - (fb = fpx / HWo) * HWo;
-                fho = rem / p.Wo;
-                fwo = rem - fho * p.Wo;
+                locate();
+            } else if (border) {
+                fpx += 32;
+                locate();
             } else {
                 fpx += 32;
+                frow = fpx;
                 fwo += 32;
                 while (fwo >= p.Wo) { fwo -= p.Wo; if (++fho == p.Ho) { fho = 0; ++fb; } }
             }
@@ -528,27 +536,23 @@ static int sm_count() {
 }
 
 template <int BN, bool STACK = false>
-static int launch_wgrad_tc(const ScsfmConv& p, cudaStream_t st) {
+static int launch_wgrad_tc(const ScsfmConv& p, int border, cudaStream_t st) {
     using Cfg = WgCfg<BN>;
     static const cudaError_t attr_rc = cudaFuncSetAttribute(conv_wgrad_tc_kernel<BN, STACK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     SCSFM_CHECK_CUDA(attr_rc);
-    const int Mtot = p.kh * p.kw * p.Cin, npix = p.B * p.Ho * p.Wo;
+    const int Mtot = p.kh * p.kw * p.Cin, npix = p.B * (border ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo);
     const int mt = (Mtot + GBM - 1) / GBM, nt = STACK ? 1 : (p.Cout + BN - 1) / BN;
-    static int per_sm = 0;                                   // resident CTAs per SM (shared memory bound: 2 for BN = 128)
-    if (per_sm == 0) {
-        SCSFM_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_wgrad_tc_kernel<BN, STACK>, FW_THREADS, Cfg::SMEM));
-        if (per_sm < 1) per_sm = 1;
-    }
-    // Three CTAs' worth of pixel splits per SM although only two BN = 128 CTAs are resident at once (shared memory): the
-    // extra split-K CTAs keep the transposing producers of more tiles in flight.  Measured on H100 over the layers of
-    // tools/conv_layers.py (tf32x3 weight gradients): 20.0 ms with this count, 28.6 ms with exactly one resident wave.
+    // Three CTAs' worth of pixel splits per SM although only one BN = 128 CTA is resident at a time (171-174 registers x
+    // 256 threads): the extra split-K CTAs queue behind it and fill the SM as the earlier ones drain.  Measured on H100
+    // over the layers of tools/conv_layers.py with every tf32x3 weight gradient on this kernel: 20.0 ms with this count,
+    // 28.6 ms with exactly one resident wave.
     int splits = (sm_count() * 3 + mt * nt - 1) / (mt * nt);
     const int max_splits = (npix + 1023) / 1024;             // at least 32 k-blocks per CTA
     if (splits > max_splits) splits = max_splits;
     if (splits < 1) splits = 1;
     const int pps = ((npix + splits - 1) / splits + 31) / 32 * 32;
     dim3 grid(mt, nt, (npix + pps - 1) / pps);
-    conv_wgrad_tc_kernel<BN, STACK><<<grid, FW_THREADS, Cfg::SMEM, st>>>(p, pps);
+    conv_wgrad_tc_kernel<BN, STACK><<<grid, FW_THREADS, Cfg::SMEM, st>>>(p, pps, border);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
@@ -792,6 +796,18 @@ extern "C" int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream) {
     return SCSFM_OK;
 }
 
+// cp.async gather weight-gradient kernel: any stride / padding mode; border = 1: the image-border ring pixels only
+static int wgrad_gather(const ScsfmConv& p, int border, cudaStream_t st) {
+    const bool split = p.in_lo != nullptr && p.dout_lo != nullptr;
+    if (split && p.Cout <= 16) return launch_wgrad_tc<32, true>(p, border, st);
+    if (split && p.Cout <= 32) return launch_wgrad_tc<64, true>(p, border, st);
+    if (split && p.Cout <= 64) return launch_wgrad_tc<128, true>(p, border, st);
+    if (p.Cout <= 16) return launch_wgrad_tc<16>(p, border, st);
+    if (p.Cout <= 32) return launch_wgrad_tc<32>(p, border, st);
+    if (p.Cout <= 64) return launch_wgrad_tc<64>(p, border, st);
+    return launch_wgrad_tc<128>(p, border, st);
+}
+
 // dw [Cout,kh,kw,Cin] += dout^T x gather(in); dbias += column sums of dout.  Needs Cin % 4 == 0 and Cout % 4 == 0.
 extern "C" int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream) {
     SCSFM_CHECK_ARG(p != nullptr && p->in && p->dout && p->dw, "conv2d_wgrad_tc: null tensor");
@@ -802,20 +818,23 @@ extern "C" int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream) {
     SCSFM_CHECK_ARG((long long)p->B * p->Ho * p->Wo < (1LL << 31), "conv2d_wgrad_tc: too many pixels");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    // SCSFM_TUNE_WGRAD: 0 auto, 1 or 2 the tensor-core kernel above, 3 the thin-layer fp32 kernel
+    // SCSFM_TUNE_WGRAD: 0 auto, 1 the gather kernel, 2 the TMA kernel (the gather kernel where it does not apply), 3 the
+    // thin-layer fp32 kernel
     int kernel = (int)((p->tune >> 12) & 3u);
     if (kernel == 3 && !conv_wgrad_thin_eligible(*p)) kernel = 0;
     // the 16-output-channel decoder layers in split mode read four tensors and use 16 of the MMA's columns: the fp32 FMA
     // kernel reads two and is exact per product (conv_wgrad_thin.cu)
     if (kernel == 0 && (p->in_lo != nullptr || p->dout_lo != nullptr) && conv_wgrad_thin_eligible(*p)) kernel = 3;
-    if (kernel == 3) rc = launch_conv_wgrad_thin(*p, st);
-    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 16) rc = launch_wgrad_tc<32, true>(*p, st);
-    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 32) rc = launch_wgrad_tc<64, true>(*p, st);
-    else if (p->in_lo != nullptr && p->dout_lo != nullptr && p->Cout <= 64) rc = launch_wgrad_tc<128, true>(*p, st);
-    else if (p->Cout <= 16) rc = launch_wgrad_tc<16>(*p, st);
-    else if (p->Cout <= 32) rc = launch_wgrad_tc<32>(*p, st);
-    else if (p->Cout <= 64) rc = launch_wgrad_tc<64>(*p, st);
-    else rc = launch_wgrad_tc<128>(*p, st);
+    const bool split = p->in_lo != nullptr && p->dout_lo != nullptr;
+    if ((kernel == 0 || kernel == 2) && conv_wgrad_tma_eligible(*p) && (split || (p->in_lo == nullptr && p->dout_lo == nullptr))) {
+        // reflection padding: the TMA kernel takes the interior with zero padding, the gather kernel the border ring
+        if ((rc = launch_conv_wgrad_tma(*p, st))) return rc;
+        rc = p->pad_mode == PADMODE_REFLECT ? wgrad_gather(*p, 1, st) : SCSFM_OK;
+    } else if (kernel == 3) {
+        rc = launch_conv_wgrad_thin(*p, st);
+    } else {
+        rc = wgrad_gather(*p, 0, st);
+    }
     if (rc) return rc;
     if (p->dbias) return launch_bias_grad(p->dout, p->B * p->Ho * p->Wo, p->Cout, p->dbias, st);
     return SCSFM_OK;

@@ -77,6 +77,11 @@ bool conv_tma_eligible(const ScsfmConv& p, const TcView& v);
 bool conv_tma_forced(const ScsfmConv& p);      // a tile configuration is being forced through ScsfmConv.tune (tests / experiments)
 int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st);
 
+// conv_wgrad_tma.cu: weight gradient of stride-1 layers with kh, kw <= 3 (TMA halo patch, register A operand); with
+// reflection padding it covers the interior pixels only (the ring goes through the gather kernel's border view)
+bool conv_wgrad_tma_eligible(const ScsfmConv& p);
+int launch_conv_wgrad_tma(const ScsfmConv& p, cudaStream_t st);
+
 // conv_wgrad_thin.cu: 3x3 stride-1 pad-1 layers with Cout = 16 and Cin in {16, 32} on the fp32 FMA pipes (exact products: no low parts)
 bool conv_wgrad_thin_eligible(const ScsfmConv& p);
 int launch_conv_wgrad_thin(const ScsfmConv& p, cudaStream_t st);
