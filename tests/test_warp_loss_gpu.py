@@ -193,6 +193,49 @@ def test_full_size_kitti_batch_vs_oracle():
     np.testing.assert_allclose(float(s2), float(s), rtol=1e-5)
 
 
+SMOOTH_CASES = [
+    # (B, H, W), references, upstream gradient, constant patch, which depths require a gradient (target first)
+    ((1, 2, 2), 0, 1.0, False, (True,)),
+    ((1, 2, 2), 2, -2.5, True, (True, False, True)),
+    ((3, 3, 257), 1, 0.1, True, (True, True)),
+    ((2, 37, 61), 2, -2.5, True, (True, False, True)),
+    ((2, 37, 61), 2, 0.1, False, (False, True, False)),
+    ((4, 256, 832), 2, 0.1, True, (True, True, True)),
+    ((4, 256, 832), 0, 1.0, False, (True,)),
+]
+
+
+@pytest.mark.parametrize("case", SMOOTH_CASES, ids=lambda c: "B%d_%dx%d_refs%d_up%g_patch%d_grad%s" % (
+    *c[0], c[1], c[2], c[3], "".join(str(int(r)) for r in c[4])))
+def test_smooth_loss_value_and_depth_gradients_vs_fp64_oracle(case):
+    """compute_smooth_loss against the fp64 oracle: the loss and the dense gradient of every depth that requires one.  A
+    constant patch makes neighbour differences exactly 0, where the gradient of |.| is 0 in both; depths without a gradient
+    get no buffer and must leave the others intact.  Bounds: fp32 sums of fp32 terms (1e-5)."""
+    from oracle import losses as OL
+    _, lf = _api()
+    (B, H, W), n_ref, upstream, patch, need = case
+    g = torch.Generator().manual_seed(B * H * W + n_ref)
+    depths, imgs = [], []
+    for _ in range(1 + n_ref):
+        d = 0.5 + 4.0 * torch.rand(B, 1, H, W, generator=g)
+        if patch:
+            d[:, :, H // 3:H // 3 + 5, W // 4:W // 4 + 7] = 1.75
+        depths.append(d)
+        imgs.append(torch.rand(B, 3, H, W, generator=g) * 2 - 1)
+    mine = [d.to(DEV).requires_grad_(r) for d, r in zip(depths, need)]
+    s = lf.compute_smooth_loss([mine[0]], imgs[0].to(DEV), [[d] for d in mine[1:]], [im.to(DEV) for im in imgs[1:]])
+    (upstream * s).backward()
+    ref = [d.double().requires_grad_(r) for d, r in zip(depths, need)]
+    so = OL.compute_smooth_loss([ref[0]], imgs[0].double(), [[d] for d in ref[1:]], [im.double() for im in imgs[1:]])
+    (upstream * so).backward()
+    np.testing.assert_allclose(float(s), float(so), rtol=1e-5)
+    for i, (a, b) in enumerate(zip(mine, ref)):
+        if not need[i]:
+            assert a.grad is None
+            continue
+        assert rel_l2(a.grad, b.grad) < 1e-5, (i, rel_l2(a.grad, b.grad))
+
+
 def test_pose_matrices_and_legacy_warp(golden_warp):
     iw, _ = _api()
     g = golden_warp
