@@ -165,7 +165,7 @@ typedef struct ScsfmConv {
     /* backward operands */
     const float* dout;    /* [B,Ho,Wo,Cout] gradient of the PRE-activation output */
     float* din;           /* dgrad result [B,Hi,Wi,Cin] (overwritten) */
-    const float* addend;  /* optional tensor added to din (residual branch gradient) */
+    const float* addend;  /* optional tensor added to din (residual branch gradient); forward: added to out before the activation (residual) */
     float* dw;            /* [Cout,kh,kw,Cin], accumulated into (atomic +=) */
     float* dbias;         /* [Cout] or NULL, accumulated into */
     /* fused BatchNorm statistics of the forward output: sums[slot][g][c] = {sum, sum of squares}, fp64,
@@ -188,6 +188,15 @@ typedef struct ScsfmConv {
      * process-global mutable state */
     unsigned tune;
     unsigned long long* debug;   /* device array of 8 x (number of SMs) cycle counters written by the TMA conv kernel, or NULL */
+    /* Eval-mode BatchNorm in the forward epilogue (NULL = off): z = act(fmaf(acc, bn_scale[c], bn_shift[c]) + addend), then
+     * SCSFM_ROUND_TF32 if flagged -- the arithmetic of scsfm_bn_apply without batch sums, so the fused result is bitwise the
+     * conv output followed by scsfm_bn_apply.  Per-output-channel [Cout] arrays from scsfm_bn_eval_prepare_batched.  Refused
+     * together with `bias` or `bn_sums`. */
+    const float* bn_scale;
+    const float* bn_shift;
+    /* forward only (NULL = off, 16-byte aligned, Cout % 4 == 0): also write tf32_lo(out) here, the split-accumulate low part a following tf32x3
+     * convolution reads as in_lo (what scsfm_split_tf32 of the output would produce) */
+    float* out_lo;
 } ScsfmConv;
 
 /* ScsfmConv.tune */
@@ -259,6 +268,11 @@ int scsfm_bn_prepare(const double* sums, int groups, int C, long long count_per_
 int scsfm_bn_apply(const float* y, const double* sums, const float* gamma, const float* beta, float* running_mean,
                    float* running_var, float momentum, float eps, float* saved, const float* residual, float* z, float* z_lo,
                    long long rows, int C, int groups, int flags, void* stream);   /* z_lo (optional): low part of z (see ScsfmConv.in_lo) */
+/* Eval-mode BatchNorm of every layer of a network in ONE launch: per layer, scale[c] = gamma[c] * invstd and
+ * shift[c] = beta[c] - running_mean[c] * scale[c] with invstd = 1 / sqrtf(running_var[c] + eps) -- the expressions
+ * scsfm_bn_apply uses in eval mode.  table: device array of n_layers x 8 int64 {gamma, beta, running_mean, running_var,
+ * scale (out), shift (out), C, eps as the bits of a float}; one CTA per layer.  scale / shift 8-byte aligned (the convolution epilogues read them as float2). */
+int scsfm_bn_eval_prepare_batched(const long long* table, int n_layers, void* stream);
 /* backward: given dz (gradient of z), z, y -> dy (overwrites `dy`), dres (= dz masked by relu; may be NULL or
  * alias dz), dgamma/dbeta accumulated into. `work` holds groups*C*2 doubles. */
 int scsfm_bn_backward(const float* dz, const float* z, const float* y, const float* saved, const float* gamma,

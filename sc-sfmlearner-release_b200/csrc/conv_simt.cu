@@ -168,7 +168,8 @@ conv_fwd_simt_kernel(ScsfmConv p) {
         __syncthreads();
     }
 
-    // epilogue: bias, activation, store, optional BatchNorm partial sums (per group of samples)
+    // epilogue: bias or eval-mode BatchNorm, residual addend, activation, store (+ low part), optional BatchNorm partial sums
+    // (per group of samples)
     double csum[4] = {0.0, 0.0, 0.0, 0.0}, csq[4] = {0.0, 0.0, 0.0, 0.0};   // fp64: see conv_tc.cu (variance cancellation)
     const int groups = p.bn_groups > 0 ? p.bn_groups : 1;
     const int rows_per_group = (p.B / groups) * p.Ho * p.Wo;
@@ -185,6 +186,8 @@ conv_fwd_simt_kernel(ScsfmConv p) {
             float x = acc[i][j];
             if (n < N) {
                 if (p.bias) x += __ldg(p.bias + n);
+                if (p.bn_scale) x = fmaf(x, __ldg(p.bn_scale + n), __ldg(p.bn_shift + n));
+                if (p.addend) x += __ldg(p.addend + (size_t)m * N + n);
                 x = apply_act(x, p.act);
                 if (p.act & ROUND_TF32) x = tf32_round(x);
                 if (want_stats) {
@@ -204,6 +207,10 @@ conv_fwd_simt_kernel(ScsfmConv p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j)
                 if (n0 + tx * 4 + j < N) o[j] = v[j];
+        if (p.out_lo)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (n0 + tx * 4 + j < N) p.out_lo[(size_t)m * N + n0 + tx * 4 + j] = tf32_lo(v[j]);
     }
     if (want_stats && uniform_group) {
         if (tid < BN) { s_stat[0][tid] = 0.0; s_stat[1][tid] = 0.0; }
@@ -503,6 +510,9 @@ extern "C" int scsfm_conv2d_fwd_simt(const ScsfmConv* p, void* stream) {
     SCSFM_CHECK_ARG(p->Ho == (p->Hi + 2 * p->pad - p->kh) / p->stride + 1 && p->Wo == (p->Wi + 2 * p->pad - p->kw) / p->stride + 1,
                     "conv2d_fwd: output size does not match geometry");
     SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || (p->pad < p->Hi && p->pad < p->Wi && p->pad <= 1), "conv2d_fwd: reflect pad must be 1");
+    SCSFM_CHECK_ARG((p->bn_scale == nullptr) == (p->bn_shift == nullptr), "conv2d_fwd: bn_scale and bn_shift go together");
+    SCSFM_CHECK_ARG(p->bn_scale == nullptr || (p->bias == nullptr && p->bn_sums == nullptr),
+                    "conv2d_fwd: the eval-mode BatchNorm epilogue excludes bias and bn_sums");
     cudaStream_t st = (cudaStream_t)stream;
     const int M = p->B * p->Ho * p->Wo, N = p->Cout;
     if (N <= 16) conv_fwd_simt_kernel<256, 16><<<dim3((M + 255) / 256, (N + 15) / 16), CT, 0, st>>>(*p);

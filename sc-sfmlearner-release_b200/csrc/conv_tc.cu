@@ -250,6 +250,7 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
                 float x = r[j];
                 if (row_ok && n < N) {
                     if (p.bias) x += __ldg(p.bias + n);
+                    if (p.bn_scale) x = fmaf(x, __ldg(p.bn_scale + n), __ldg(p.bn_shift + n));    // eval-mode BatchNorm
                     if (p.addend) x += __ldg(p.addend + out_row * N + n);
                     x = tc_act(x, p.act);
                     if (p.act & ROUND_TF32) x = tf32_round(x);
@@ -268,6 +269,13 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
 #pragma unroll
                     for (int j = 0; j < CW; ++j)
                         if (n0 + cc * CW + j < N) o[j] = v[j];
+                }
+                if (p.out_lo != nullptr) {                        // low part of the split-accumulate operand (N % 4 == 0)
+                    float* ol = p.out_lo + out_row * N + n0 + cc * CW;
+#pragma unroll
+                    for (int j = 0; j < CW; j += 4)
+                        if (n0 + cc * CW + j < N)
+                            *reinterpret_cast<float4*>(ol + j) = make_float4(tf32_lo(v[j]), tf32_lo(v[j + 1]), tf32_lo(v[j + 2]), tf32_lo(v[j + 3]));
                 }
             }
             if (p.bn_sums != nullptr) {
@@ -643,6 +651,13 @@ static int check_tc(const ScsfmConv* p, const char* who) {
         const int g = p->bn_groups > 0 ? p->bn_groups : 1;
         SCSFM_CHECK_ARG(p->B % g == 0, "%s: batch not divisible by the number of BatchNorm groups", who);
     }
+    SCSFM_CHECK_ARG((p->bn_scale == nullptr) == (p->bn_shift == nullptr), "%s: bn_scale and bn_shift go together", who);
+    SCSFM_CHECK_ARG(p->bn_scale == nullptr || (p->bias == nullptr && p->bn_sums == nullptr),
+                    "%s: the eval-mode BatchNorm epilogue excludes bias and bn_sums", who);
+    SCSFM_CHECK_ARG(p->out_lo == nullptr || ((p->Cout & 3) == 0 && (reinterpret_cast<uintptr_t>(p->out_lo) & 15) == 0),
+                    "%s: out_lo needs Cout %% 4 == 0 and 16-byte alignment", who);
+    SCSFM_CHECK_ARG(((reinterpret_cast<uintptr_t>(p->bn_scale) | reinterpret_cast<uintptr_t>(p->bn_shift)) & 7) == 0,
+                    "%s: bn_scale / bn_shift must be 8-byte aligned", who);
     return SCSFM_OK;
 }
 
@@ -743,6 +758,7 @@ extern "C" int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     ScsfmConv q = *p;
     q.in = p->dout; q.in_lo = p->dout_lo; q.out = p->din; q.bias = nullptr; q.bn_sums = nullptr; q.act = SCSFM_ACT_NONE;
+    q.bn_scale = nullptr; q.bn_shift = nullptr; q.out_lo = nullptr;
     q.dout_lo = nullptr;                       // (w_lo: the flipped low-part weights, laid out like w)
     q.Hi = p->Ho; q.Wi = p->Wo; q.Cin = p->Cout;
     q.Cout = p->Cin; q.pad_mode = SCSFM_PADMODE_ZERO;

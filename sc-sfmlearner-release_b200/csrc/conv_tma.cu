@@ -14,7 +14,8 @@
 //  * one CTA per SM walks the (tile, Cout tile) work list; the shared-memory stage ring and the mbarrier phases run
 //    across tiles, so the producer prefetches the next tile's patches while the current one is multiplied and stored;
 //  * the accumulator comes out pixel-major (a thread holds 2 consecutive channels of a pixel per fragment), so the
-//    epilogue writes NHWC straight from registers: bias / residual addend / activation / TF32 rounding / BatchNorm sums.
+//    epilogue writes NHWC straight from registers: bias or eval-mode BatchNorm / residual addend / activation / TF32
+//    rounding / low part / BatchNorm sums.
 //
 //   warps 0-7   two consumer warpgroups; warpgroup g owns the pixels [64 MT g, 64 MT (g + 1)) of the tile
 //   warp 8      lane 0: TMA producer (1 activation box + kh weight boxes per stage, mbarrier expect_tx)
@@ -222,20 +223,28 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
             for (int i = 0; i < BNW / 4; ++i) { bs1[i] = 0.f; bs2[i] = 0.f; }
             const long long tile_off = (long long)b * img_step + (long long)(y0 * v.out_sy + v.out_oy) * (v.out_W * N) +
                                        (long long)(x0 * v.out_sx + v.out_ox) * N + n0;
+            // channel pair outermost: its bias / BatchNorm coefficients are loaded once and stay live for 2 * MT pixels only
 #pragma unroll
-            for (int mb = 0; mb < MT; ++mb) {
+            for (int i = 0; i < BNW / 8; ++i) {
+                const int c = 8 * i + fc;
+                if (c >= cv) continue;
+                float2 bb = make_float2(0.f, 0.f), sc = make_float2(0.f, 0.f), sh = make_float2(0.f, 0.f);
+                if (p.bias != nullptr) bb = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
+                if (p.bn_scale != nullptr) {
+                    sc = __ldg(reinterpret_cast<const float2*>(p.bn_scale + n0 + c));
+                    sh = __ldg(reinterpret_cast<const float2*>(p.bn_shift + n0 + c));
+                }
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int l = 64 * (wg * MT + mb) + fr + 8 * h;       // pixel index inside the tile
-                    const int row = l >> g.tw_log2, col = l & (TW - 1);
-                    if (y0 + row >= p.Ho || x0 + col >= p.Wo) continue;
-                    const long long off = tile_off + (long long)row * row_step + (long long)col * px_step;
+                for (int mb = 0; mb < MT; ++mb) {
 #pragma unroll
-                    for (int i = 0; i < BNW / 8; ++i) {
-                        const int c = 8 * i + fc;
-                        if (c >= cv) continue;
+                    for (int h = 0; h < 2; ++h) {
+                        const int l = 64 * (wg * MT + mb) + fr + 8 * h;       // pixel index inside the tile
+                        const int row = l >> g.tw_log2, col = l & (TW - 1);
+                        if (y0 + row >= p.Ho || x0 + col >= p.Wo) continue;
+                        const long long off = tile_off + (long long)row * row_step + (long long)col * px_step;
                         float2 x = make_float2(acc[mb][4 * i + 2 * h], acc[mb][4 * i + 2 * h + 1]);
-                        if (p.bias != nullptr) { const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)); x.x += bb.x; x.y += bb.y; }
+                        if (p.bias != nullptr) { x.x += bb.x; x.y += bb.y; }
+                        if (p.bn_scale != nullptr) { x.x = fmaf(x.x, sc.x, sh.x); x.y = fmaf(x.y, sc.y, sh.y); }   // eval-mode BatchNorm (bn_apply's arithmetic)
                         if (p.addend != nullptr) {
                             const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + off + c));
                             x.x += a.x; x.y += a.y;
@@ -243,6 +252,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
                         if (act != ACT_NONE) { x.x = tc_act(x.x, act); x.y = tc_act(x.y, act); }
                         if (round) { x.x = tf32_round(x.x); x.y = tf32_round(x.y); }
                         *reinterpret_cast<float2*>(p.out + off + c) = x;
+                        if (p.out_lo != nullptr) *reinterpret_cast<float2*>(p.out_lo + off + c) = make_float2(tf32_lo(x.x), tf32_lo(x.y));
                         bs1[2 * i] += x.x; bs1[2 * i + 1] += x.y;
                         bs2[2 * i] += x.x * x.x; bs2[2 * i + 1] += x.y * x.y;
                     }

@@ -126,6 +126,33 @@ __global__ void bn_prepare_kernel(const double* __restrict__ sums, int G, int C,
     }
 }
 
+// Per-channel affine of BatchNorm: shared by bn_apply_kernel (both modes) and the eval-mode prepare of the fused convolution
+// epilogue, so that the two cannot diverge (the fused eval forward is bitwise the conv followed by bn_apply).
+__device__ __forceinline__ float bn_eval_invstd(float running_var, float eps) { return 1.0f / sqrtf(running_var + eps); }
+__device__ __forceinline__ void bn_affine(float gamma, float beta, float mean, float invstd, float& scale, float& shift) {
+    scale = gamma * invstd;
+    shift = beta - mean * scale;
+}
+
+// table rows {gamma, beta, running_mean, running_var, scale, shift, C, eps bits}; one CTA per layer
+__global__ void __launch_bounds__(NT) bn_eval_prepare_batched_kernel(const long long* __restrict__ table) {
+    const long long* e = table + (size_t)blockIdx.x * 8;
+    const float* gamma = reinterpret_cast<const float*>(e[0]);
+    const float* beta = reinterpret_cast<const float*>(e[1]);
+    const float* rmean = reinterpret_cast<const float*>(e[2]);
+    const float* rvar = reinterpret_cast<const float*>(e[3]);
+    float* scale = reinterpret_cast<float*>(e[4]);
+    float* shift = reinterpret_cast<float*>(e[5]);
+    const int C = (int)e[6];
+    const float eps = __int_as_float((int)e[7]);
+    for (int c = threadIdx.x; c < C; c += NT) {
+        float sc, sh;
+        bn_affine(gamma[c], beta[c], rmean[c], bn_eval_invstd(rvar[c], eps), sc, sh);
+        scale[c] = sc;
+        shift[c] = sh;
+    }
+}
+
 // z = relu?(y*scale + shift + residual), with scale/shift derived IN the kernel from the fused batch sums (training) or
 // taken from `saved` (eval).  Grid (row chunks, groups, channel slabs); a thread owns 4 consecutive channels and walks
 // rows, so there is no per-element index arithmetic: pure float4 streaming.  The first row-chunk CTA of every
@@ -161,9 +188,10 @@ bn_apply_kernel(const float* __restrict__ y, const double* __restrict__ sums, co
             invstd = (float)(1.0 / sqrt(var + (double)eps));
         } else {
             mean = rmean[ch];
-            invstd = 1.0f / sqrtf(rvar[ch] + eps);
+            invstd = bn_eval_invstd(rvar[ch], eps);
         }
-        const float scale = gamma[ch] * invstd, shift = beta[ch] - mean * scale;
+        float scale, shift;
+        bn_affine(gamma[ch], beta[ch], mean, invstd, scale, shift);
         s_sc[cc] = scale;
         s_sh[cc] = shift;
         if (blockIdx.x == 0) {
@@ -670,6 +698,13 @@ extern "C" int scsfm_bn_apply(const float* y, const double* sums, const float* g
     bn_grid(rows / groups, C, groups, grid, rpc);
     bn_apply_kernel<<<grid, NT, 0, ST>>>(y, sums, gamma, beta, running_mean, running_var, momentum, eps, sums != nullptr, saved, residual, z, z_lo,
                                          rows / groups, C, groups, flags, rpc);
+    SCSFM_CHECK_LAUNCH();
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_bn_eval_prepare_batched(const long long* table, int n_layers, void* stream) {
+    SCSFM_CHECK_ARG(table != nullptr && n_layers > 0, "bn_eval_prepare_batched: bad arguments");
+    bn_eval_prepare_batched_kernel<<<n_layers, NT, 0, ST>>>(table);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }

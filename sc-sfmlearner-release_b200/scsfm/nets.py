@@ -314,6 +314,21 @@ class ArenaNet(nn.Module):
             # flipped / transposed copies for the data gradients: all of them in one launch, in place
             cx.refresh_flips(self._flat.device)
 
+    def _fused_eval(self):
+        """Eval mode with autograd off: the forward runs without recording (every activation is freed once dead) and with
+        BatchNorm fused into the convolution epilogues (see encoder_forward_eval)."""
+        return not self.training and not torch.is_grad_enabled()
+
+    def bn_eval_coeffs(self):
+        """Eval-mode {scale, shift} of every BatchNorm layer, recomputed from the current parameters and running statistics
+        by one launch; returns {id(BNParams): (scale, shift)}.  The job table is rebuilt when a buffer address changes."""
+        bns = [m for m in self.modules() if isinstance(m, BNParams)]
+        tab = getattr(self, "_bn_eval", None)
+        if tab is None or tab.key != O.BnEvalTable.key_of(bns):
+            tab = self._bn_eval = O.BnEvalTable(bns, BN_EPS)
+        tab.prepare()
+        return {id(bn): c for bn, c in zip(bns, tab.coeffs)}
+
     def _attach_grads(self):
         """Called at the start of every backward: if an optimizer dropped the gradients
         (zero_grad(set_to_none=True)) the arena is stale -> zero it and re-attach the views."""
@@ -513,6 +528,53 @@ def encoder_forward(cx, enc, imgs, training, G=1):
     return rec, feats
 
 
+def _conv_bn_eval(cx, x, conv, bn, coeffs, stride, pad, relu, residual=None, with_lo=False):
+    """relu?(bn(conv(x)) [+ residual]) in eval mode as ONE convolution: BatchNorm, residual, ReLU and TF32 rounding in its
+    epilogue (bitwise conv_fwd followed by bn_apply).  with_lo: the output feeds a tensor-core convolution (tf32x3: write its
+    low part too)."""
+    sc, sh = coeffs[id(bn)]
+    return cx.conv_fwd(x, conv.w_op(cx), None, stride, pad, O.PAD_ZERO, (O.ACT_RELU if relu else O.ACT_NONE) | cx.rnd(), None, 1,
+                       conv.w_lo(cx), bn_scale=sc, bn_shift=sh, addend=residual, with_lo=with_lo and cx.split)
+
+
+def block_forward_eval(cx, blk, x, coeffs):
+    if blk.bottleneck:
+        h1 = _conv_bn_eval(cx, x, blk.conv1, blk.bn1, coeffs, 1, 0, True, None, True)
+        h2 = _conv_bn_eval(cx, h1, blk.conv2, blk.bn2, coeffs, blk.stride, 1, True, None, True)
+        del h1
+        last_in, last_conv, last_bn, ls, lp = h2, blk.conv3, blk.bn3, 1, 0
+    else:
+        h1 = _conv_bn_eval(cx, x, blk.conv1, blk.bn1, coeffs, blk.stride, 1, True, None, True)
+        last_in, last_conv, last_bn, ls, lp = h1, blk.conv2, blk.bn2, 1, 1
+    sc = x
+    if blk.downsample is not None:
+        sc = _conv_bn_eval(cx, x, blk.downsample[0], blk.downsample[1], coeffs, blk.stride, 0, False)
+    return _conv_bn_eval(cx, last_in, last_conv, last_bn, coeffs, ls, lp, True, sc, True)
+
+
+def encoder_forward_eval(cx, enc, imgs, coeffs):
+    """encoder_forward's eval-mode features without the record: imgs as there, coeffs from ArenaNet.bn_eval_coeffs()."""
+    t = enc.encoder
+    if cx.tc:
+        cpad = 4 * len(imgs)
+        x_nhwc = O.nchw_to_nhwc_pad(imgs[0], imgs[1] if len(imgs) > 1 else None, cpad, cx.operand)
+        w0 = O.pad_channels(t.conv1.w_khwc(), cpad, cx.operand)
+        w0_lo = O.pad_channels(t.conv1.w_khwc(), cpad, O.OPERAND_LO) if cx.split else None
+        sc, sh = coeffs[id(t.bn1)]
+        f0 = cx.conv_fwd(x_nhwc, w0, None, 2, 3, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, w0_lo, bn_scale=sc, bn_shift=sh)
+    else:
+        x_nhwc = O.nchw_to_nhwc(imgs[0], imgs[1] if len(imgs) > 1 else None)
+        f0 = _conv_bn_eval(cx, x_nhwc, t.conv1, t.bn1, coeffs, 2, 3, True)
+    del x_nhwc
+    x, _ = O.maxpool_fwd(f0)
+    feats = [f0]
+    for li in range(1, 5):
+        for blk in getattr(t, "layer%d" % li):
+            x = block_forward_eval(cx, blk, x, coeffs)
+        feats.append(x)
+    return feats
+
+
 def encoder_backward(cx, enc, rec, d_feats):
     """d_feats[i]: gradient w.r.t. feature i coming from the decoder (None if unused).  d_feats[4] is required."""
     t = enc.encoder
@@ -566,6 +628,8 @@ class DispResNet(ArenaNet):
 
     def forward(self, x):
         self.ensure_arena()
+        if self._fused_eval():
+            return self._forward_impl(1, x, fused=True)[1][0]
         if torch.is_grad_enabled():
             self._pending += 1
         outs = _NetCall.apply(self, self._hook, 1, x)
@@ -580,39 +644,52 @@ class DispResNet(ArenaNet):
         if torch.is_grad_enabled():
             self._pending += 1
         G, B = len(images), images[0].shape[0]
+        if self._fused_eval():
+            out = self._forward_impl(G, torch.cat(list(images), 0), fused=True)[1][0]
+            return [out[g * B:(g + 1) * B] for g in range(G)]
         outs = _NetCall.apply(self, self._hook, G, torch.cat(list(images), 0))
         per = [[o[g * B:(g + 1) * B] for o in outs] for g in range(G)]
         return per if self.training else [p[0] for p in per]
 
     # -- forward ------------------------------------------------------------------------------
-    def _forward_impl(self, groups, x):
+    def _forward_impl(self, groups, x, fused=False):
+        """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs)."""
         from . import lib as L
         x = L.dev_f32(x, "DispResNet input")
         self.refresh_operand_weights()
         training = self.training
         cx = self.ctx
-        enc_rec, feats = encoder_forward(cx, self.encoder, (x,), training, groups)
+        if fused:
+            enc_rec, feats = None, encoder_forward_eval(cx, self.encoder, (x,), self.bn_eval_coeffs())
+        else:
+            enc_rec, feats = encoder_forward(cx, self.encoder, (x,), training, groups)
         dec = self.decoder
         rec = {"enc": enc_rec, "stages": {}}
         cur = feats[4]
         disps = {}
         for i in range(4, -1, -1):
-            st = {"in0": cur}
             c0 = dec.up(i, 0)
-            st["a"] = cx.conv_fwd(cur, c0.w_op(cx), c0.bias, 1, 1, O.PAD_REFLECT, O.ACT_ELU | cx.rnd(), None, 1, c0.w_lo(cx))
-            st["cat"] = O.upcat_fwd(st["a"], feats[i - 1] if i > 0 else None)
+            a = cx.conv_fwd(cur, c0.w_op(cx), c0.bias, 1, 1, O.PAD_REFLECT, O.ACT_ELU | cx.rnd(), None, 1, c0.w_lo(cx))
+            cat = O.upcat_fwd(a, feats[i - 1] if i > 0 else None)
             c1 = dec.up(i, 1)
-            st["b"] = cx.conv_fwd(st["cat"], c1.w_op(cx), c1.bias, 1, 1, O.PAD_REFLECT, O.ACT_ELU | cx.rnd(), None, 1, c1.w_lo(cx))
-            cur = st["b"]
+            # (fused: b feeds the next stage's first convolution directly, so its low part is written with it)
+            b = cx.conv_fwd(cat, c1.w_op(cx), c1.bias, 1, 1, O.PAD_REFLECT, O.ACT_ELU | cx.rnd(), None, 1, c1.w_lo(cx),
+                            with_lo=fused and cx.split and i > 0)
+            if fused:
+                if i > 0:
+                    feats[i - 1] = None          # the skip feature is dead once concatenated
+            else:
+                rec["stages"][i] = {"in0": cur, "a": a, "cat": cat, "b": b}
+            del a, cat
+            cur = b
             if i < 4 and (training or i == 0):
                 dc = dec.disp(i)
                 disps[i] = O.head_fwd(cur, dc.w_khwc(), dc.bias, O.ACT_DISP)
-            rec["stages"][i] = st
         rec["disps"] = disps
         order = [0, 1, 2, 3] if training else [0]
         rec["order"] = order
         # [B,H,W,1] NHWC is bit-identical to [B,1,H,W] NCHW
-        return rec, [disps[s].view(disps[s].shape[0], 1, disps[s].shape[1], disps[s].shape[2]) for s in order]
+        return None if fused else rec, [disps[s].view(disps[s].shape[0], 1, disps[s].shape[1], disps[s].shape[2]) for s in order]
 
     # -- backward -----------------------------------------------------------------------------
     def _backward_impl(self, rec, grads):
@@ -674,6 +751,8 @@ class PoseResNet(ArenaNet):
 
     def forward(self, img1, img2):
         self.ensure_arena()
+        if self._fused_eval():
+            return self._forward_impl(1, img1, img2, fused=True)[1][0]
         if torch.is_grad_enabled():
             self._pending += 1
         return _NetCall.apply(self, self._hook, 1, img1, img2)[0]
@@ -685,16 +764,31 @@ class PoseResNet(ArenaNet):
         if torch.is_grad_enabled():
             self._pending += 1
         G, B = len(pairs), pairs[0][0].shape[0]
+        if self._fused_eval():
+            out = self._forward_impl(G, torch.cat([a for a, _ in pairs], 0), torch.cat([b for _, b in pairs], 0), fused=True)[1][0]
+            return [out[g * B:(g + 1) * B] for g in range(G)]
         out = _NetCall.apply(self, self._hook, G, torch.cat([a for a, _ in pairs], 0), torch.cat([b for _, b in pairs], 0))[0]
         return [out[g * B:(g + 1) * B] for g in range(G)]
 
-    def _forward_impl(self, groups, img1, img2):
+    def _forward_impl(self, groups, img1, img2, fused=False):
+        """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs)."""
         from . import lib as L
         img1, img2 = L.dev_f32(img1, "PoseResNet input"), L.dev_f32(img2, "PoseResNet input")
         self.refresh_operand_weights()
         cx = self.ctx
-        enc_rec, feats = encoder_forward(cx, self.encoder, (img1, img2), self.training, groups)
         n = self.decoder.net
+        if fused:
+            f4 = encoder_forward_eval(cx, self.encoder, (img1, img2), self.bn_eval_coeffs())[4]
+            lo = cx.split
+            s = cx.conv_fwd(f4, n[0].w_op(cx), n[0].bias, 1, 0, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[0].w_lo(cx), with_lo=lo)
+            del f4
+            p0 = cx.conv_fwd(s, n[1].w_op(cx), n[1].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[1].w_lo(cx), with_lo=lo)
+            del s
+            p1 = cx.conv_fwd(p0, n[2].w_op(cx), n[2].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[2].w_lo(cx))
+            del p0
+            p2 = cx.conv_fwd(p1, n[3].w_op(cx), n[3].bias, 1, 0, O.PAD_ZERO, O.ACT_NONE, None, 1, n[3].w_lo(cx))
+            return None, [O.spatial_mean_fwd(p2, 0.01)]
+        enc_rec, feats = encoder_forward(cx, self.encoder, (img1, img2), self.training, groups)
         rec = {"enc": enc_rec, "f4": feats[4]}
         rec["s"] = cx.conv_fwd(feats[4], n[0].w_op(cx), n[0].bias, 1, 0, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[0].w_lo(cx))
         rec["p0"] = cx.conv_fwd(rec["s"], n[1].w_op(cx), n[1].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[1].w_lo(cx))

@@ -39,7 +39,8 @@ class Conv(ctypes.Structure):
                 [(n, ctypes.c_int) for n in ("bn_groups", "B", "Hi", "Wi", "Cin", "Ho", "Wo", "Cout", "kh", "kw",
                                              "stride", "pad", "pad_mode", "act")] +
                 [(n, ctypes.c_void_p) for n in ("in_lo", "w_lo", "dout_lo")] +
-                [("tune", ctypes.c_uint), ("debug", ctypes.c_void_p)])
+                [("tune", ctypes.c_uint), ("debug", ctypes.c_void_p)] +
+                [(n, ctypes.c_void_p) for n in ("bn_scale", "bn_shift", "out_lo")])
 
 
 _bound = False
@@ -69,6 +70,7 @@ def _lib():
         lib.scsfm_unpad_add.argtypes = [P, LL, I, I, P, P]
         lib.scsfm_bn_prepare.argtypes = [P, I, I, LL, P, P, P, P, F, F, I, P, P]
         lib.scsfm_bn_apply.argtypes = [P, P, P, P, P, P, F, F, P, P, P, P, LL, I, I, I, P]
+        lib.scsfm_bn_eval_prepare_batched.argtypes = [P, I, P]
         lib.scsfm_bn_backward.argtypes = [P, P, P, P, P, P, P, P, P, P, LL, I, I, I, P, P]
         lib.scsfm_maxpool_fwd.argtypes = [P, I, I, I, I, P, P, P]
         lib.scsfm_maxpool_bwd.argtypes = [P, P, I, I, I, I, P, I, P]
@@ -162,7 +164,7 @@ def conv_desc(x_shape, w, stride, pad, pad_mode, act):
     Ho = (Hi + 2 * pad - kh) // stride + 1
     Wo = (Wi + 2 * pad - kw) // stride + 1
     return Conv(None, L.ptr(w), None, None, None, None, None, None, None, None, 1, B, Hi, Wi, Cin, Ho, Wo, Cout, kh, kw,
-                stride, pad, pad_mode, act, None, None, None, 0, None)
+                stride, pad, pad_mode, act, None, None, None, 0, None, None, None, None)
 
 
 def _tag(d):
@@ -255,14 +257,25 @@ class ConvCtx:
         self._table = None
 
     # -- convolutions ---------------------------------------------------------------------------------------
-    def conv_fwd(self, x, w, bias=None, stride=1, pad=0, pad_mode=PAD_ZERO, act=ACT_NONE, bn_sums=None, bn_groups=1, w_lo=None):
+    def conv_fwd(self, x, w, bias=None, stride=1, pad=0, pad_mode=PAD_ZERO, act=ACT_NONE, bn_sums=None, bn_groups=1, w_lo=None,
+                 bn_scale=None, bn_shift=None, addend=None, with_lo=False):
         """y = act(conv(x, w) + bias); optionally accumulates per-(group, channel) sum / sum-of-squares of y.
-        w_lo: low part of the weights (tf32x3 mode)."""
+        w_lo: low part of the weights (tf32x3 mode).
+        Eval-mode BatchNorm fused into the epilogue: y = act(fmaf(conv(x, w), bn_scale, bn_shift) + addend) with the
+        per-channel coefficients of bn_eval_prepare() (no bias, no bn_sums).  with_lo: also write the low part of y
+        (attached to y like lo_of() would), for a following tf32x3 convolution."""
         lib = _lib()
         d = conv_desc(x.shape, w, stride, pad, pad_mode, act)
         y = empty((d.B, d.Ho, d.Wo, d.Cout), x)
         d.inp, d.bias, d.out, d.bn_sums, d.bn_groups = x.data_ptr(), bias.data_ptr() if bias is not None else None, \
             y.data_ptr(), bn_sums.data_ptr() if bn_sums is not None else None, bn_groups
+        if bn_scale is not None:
+            d.bn_scale, d.bn_shift = bn_scale.data_ptr(), bn_shift.data_ptr()
+        if addend is not None:
+            d.addend = addend.data_ptr()
+        if with_lo:
+            y._scsfm_lo = empty(y.shape, y)
+            d.out_lo = y._scsfm_lo.data_ptr()
         tc = self._use_tc("fwd", d.Cin, d.Cout, d.kh, stride)
         if tc and self.split:
             if w_lo is None:
@@ -426,6 +439,43 @@ def bn_apply(y, sums, gamma, beta, rmean, rvar, momentum, eps, residual, flags, 
     if with_lo:
         z._scsfm_lo = z_lo
     return z, saved
+
+
+class BnEvalTable:
+    """Device job table of scsfm_bn_eval_prepare_batched for a list of BatchNorm layers (objects with weight, bias,
+    running_mean, running_var), and the [Cout] scale / shift arrays it fills: coeffs[i] = (scale, shift) of layer i.  The
+    table bakes in every buffer address; `key` lists them so that a caller can tell when it is stale."""
+
+    def __init__(self, bns, eps):
+        import struct
+        dev = bns[0].weight.device
+        total = sum(2 * _aligned64(bn.weight.numel()) for bn in bns)
+        self.buf = torch.empty(total, device=dev, dtype=torch.float32)
+        eps_bits = struct.unpack("<i", struct.pack("<f", eps))[0]
+        rows, self.coeffs, off = [], [], 0
+        for bn in bns:
+            C = bn.weight.numel()
+            sc, sh = self.buf[off:off + C], self.buf[off + _aligned64(C):off + _aligned64(C) + C]
+            off += 2 * _aligned64(C)
+            self.coeffs.append((sc, sh))
+            rows.append([bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                         sc.data_ptr(), sh.data_ptr(), C, eps_bits])
+        self.key = BnEvalTable.key_of(bns)
+        self.table = torch.tensor(rows, dtype=torch.int64).to(dev)
+        self.n, self.bytes = len(rows), 24.0 * sum(bn.weight.numel() for bn in bns)
+
+    @staticmethod
+    def key_of(bns):
+        return tuple((bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr()) for bn in bns)
+
+    def prepare(self):
+        """(Re)compute every layer's scale / shift from the current parameters and running statistics: one launch."""
+        L.launch(_lib().scsfm_bn_eval_prepare_batched, "scsfm_bn_eval_prepare_batched", "bn_prepare", 1, self.bytes,
+                 L.ptr(self.table), self.n, L.stream())
+
+
+def _aligned64(n):
+    return (n + 63) // 64 * 64
 
 
 def bn_backward(dz, z, y, saved, dgamma, dbeta, relu, want_dres, groups=1, with_lo=False):
