@@ -203,7 +203,7 @@ typedef struct ScsfmConv {
 #define SCSFM_TUNE_NO_TMA 0x1u                          /* fwd/dgrad: cp.async gather kernel only */
 #define SCSFM_TUNE_MT(mt) (((unsigned)(mt) & 3u) << 4)       /* TMA kernel: 1|2 stacked 128-pixel sub-tiles (0 = auto) */
 #define SCSFM_TUNE_TW(l2) (((unsigned)((l2) ? (l2) - 2 : 0) & 3u) << 6)   /* TMA kernel: tile width log2 3|4 (0 = auto) */
-#define SCSFM_TUNE_BN(bn) (((bn) == 16 ? 1u : (bn) == 32 ? 2u : (bn) == 64 ? 3u : (bn) == 128 ? 4u : 0u) << 8)  /* weight rows in smem */
+#define SCSFM_TUNE_BN(bn) (((bn) == 16 ? 1u : (bn) == 32 ? 2u : (bn) == 64 ? 3u : (bn) == 128 ? 4u : 0u) << 8)  /* weight rows in smem; TMA wgrad: Cout tile 32|64 */
 #define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 gather kernel, 2 TMA kernel, 3 thin-layer fp32 kernel */
 
 /* Exact-fp32 implicit-GEMM convolution on CUDA cores (every shape). */
@@ -217,7 +217,8 @@ int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream);
 /* Stride-1 (sub-)convolutions with kh, kw <= 3 run the TMA halo-patch kernel (conv_tma.cu: one 4-D tiled TMA load
  * per (channel chunk, dx) brings the input patch of a 2-D output tile, the kh vertical taps reuse it); reflection-
  * padded layers run it zero-padded and recompute the border ring with the gather kernel.  Other shapes (stride-2
- * forward, 7x7 stems) use the cp.async gather kernel. */
+ * forward, 7x7 stems) use the cp.async gather kernel.  wgrad_tc: stride-1 and zero-padded stride-2 layers with
+ * kh, kw <= 3 and the 7x7 stride-2 stems (4 or 8 channels) run the TMA weight-gradient kernel (conv_wgrad_tma.cu). */
 int scsfm_conv2d_fwd_tc(const ScsfmConv* p, void* stream);
 int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream);
 int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream);

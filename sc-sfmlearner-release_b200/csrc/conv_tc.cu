@@ -812,7 +812,8 @@ extern "C" int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream) {
     return SCSFM_OK;
 }
 
-// cp.async gather weight-gradient kernel: any stride / padding mode; border = 1: the image-border ring pixels only
+// cp.async gather weight-gradient kernel: any stride / padding mode (whatever the TMA kernel does not take); border = 1:
+// the image-border ring pixels only
 static int wgrad_gather(const ScsfmConv& p, int border, cudaStream_t st) {
     const bool split = p.in_lo != nullptr && p.dout_lo != nullptr;
     if (split && p.Cout <= 16) return launch_wgrad_tc<32, true>(p, border, st);

@@ -77,8 +77,9 @@ bool conv_tma_eligible(const ScsfmConv& p, const TcView& v);
 bool conv_tma_forced(const ScsfmConv& p);      // a tile configuration is being forced through ScsfmConv.tune (tests / experiments)
 int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st);
 
-// conv_wgrad_tma.cu: weight gradient of stride-1 layers with kh, kw <= 3 (TMA halo patch, register A operand); with
-// reflection padding it covers the interior pixels only (the ring goes through the gather kernel's border view)
+// conv_wgrad_tma.cu: weight gradient of stride-1 and zero-padded stride-2 layers with kh, kw <= 3 and of the 7x7
+// stride-2 stems with 4 or 8 channels (TMA halo patch, register A operand); with reflection padding it covers the
+// interior pixels only (the ring goes through the gather kernel's border view)
 bool conv_wgrad_tma_eligible(const ScsfmConv& p);
 int launch_conv_wgrad_tma(const ScsfmConv& p, cudaStream_t st);
 

@@ -25,13 +25,16 @@ torch.backends.cuda.matmul.allow_tf32 = False
 # name, B, H, W, Cin, Cout, k, stride, pad, reflect, launches per step in DispResNet18 (B=12) + PoseResNet18 (B=16)
 LAYERS = [
     ("stem 7x7 s2", 12, 256, 832, 4, 64, 7, 2, 3, 0),
+    ("pose stem 7x7 s2", 16, 256, 832, 8, 64, 7, 2, 3, 0),
     ("enc L1", 12, 64, 208, 64, 64, 3, 1, 1, 0),
     ("enc L2 s2", 12, 64, 208, 64, 128, 3, 2, 1, 0),
     ("down2 1x1 s2", 12, 64, 208, 64, 128, 1, 2, 0, 0),
     ("enc L2", 12, 32, 104, 128, 128, 3, 1, 1, 0),
     ("enc L3 s2", 12, 32, 104, 128, 256, 3, 2, 1, 0),
+    ("down3 1x1 s2", 12, 32, 104, 128, 256, 1, 2, 0, 0),
     ("enc L3", 12, 16, 52, 256, 256, 3, 1, 1, 0),
     ("enc L4 s2", 12, 16, 52, 256, 512, 3, 2, 1, 0),
+    ("down4 1x1 s2", 12, 16, 52, 256, 512, 1, 2, 0, 0),
     ("enc L4", 12, 8, 26, 512, 512, 3, 1, 1, 0),
     ("dec 4_0", 12, 8, 26, 512, 256, 3, 1, 1, 1),
     ("dec 4_1", 12, 16, 52, 512, 256, 3, 1, 1, 1),
