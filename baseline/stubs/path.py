@@ -18,8 +18,10 @@ class Path(str):
         out = [Path(os.path.join(self, f)) for f in sorted(os.listdir(self)) if os.path.isfile(os.path.join(self, f))]
         return [f for f in out if pattern is None or fnmatch.fnmatch(os.path.basename(f), pattern)]
 
-    def dirs(self):
-        return [Path(os.path.join(self, f)) for f in sorted(os.listdir(self)) if os.path.isdir(os.path.join(self, f))]
+    def dirs(self, pattern=None):
+        import fnmatch
+        out = [Path(os.path.join(self, f)) for f in sorted(os.listdir(self)) if os.path.isdir(os.path.join(self, f))]
+        return [d for d in out if pattern is None or fnmatch.fnmatch(os.path.basename(d), pattern)]
 
     @property
     def name(self):

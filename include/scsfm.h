@@ -308,6 +308,35 @@ int scsfm_spatial_mean_bwd(const float* dout, int B, int HW, int C, float scale,
 int scsfm_compute_errors(const float* gt, const float* pred, int B, int H, int W, int y1, int y2, int x1, int x2,
                          float max_depth, void* work, float* out, void* stream);
 
+/* Offline depth evaluation of a chunk of images (reference eval_depth.py:32-56,159-227, DepthEvalEigen.evaluate_depth with
+ * median scaling and compute_depth_errors), at the precision numpy uses.  Per image:
+ *   - prediction pred[i] [h,w] float64 (test_disp.py's predictions.npy); its inverse 1 / (p + 1e-6) is resized to the ground
+ *     truth's H x W as cv2.resize INTER_LINEAR does (half-pixel centres, edge clamp, fp64 weights; horizontal pass, then vertical,
+ *     every operation rounded, no FMA) at the masked pixels only, then inverted again: 1 / (x + 1e-6);
+ *   - mask: min_depth < gt < max_depth compared in the ground truth's dtype (float32 ground truth compares with float32(min_depth)),
+ *     and the pixel inside the crop rows [y1,y2) x columns [x1,x2) (the whole image for NYU);
+ *   - numpy medians (ranks (n-1)/2 and n/2 averaged; the ground truth's in its dtype, the prediction's in fp64), exact radix
+ *     select; ratio = median(gt) / median(pred) in fp64; prediction * ratio clamped to [min_depth, max_depth];
+ *   - out[i][SCSFM_EVAL_OUT] = {n, median(gt), median(pred), ratio, abs_rel, sq_rel, rmse, rmse_log, log10, a1, a2, a3}, fp64;
+ *     log(gt) and log10(gt) are taken in the ground truth's dtype.  An empty mask (n = 0) gives NaN for everything but n, as
+ *     np.median of an empty array does.
+ * gt: packed ground truths, gt_elems elements of gt_dtype; images_host: HOST array of n_img descriptors.  Predictions are
+ * depths (positive).  workspace: scsfm_eval_depth_workspace_bytes(images_host, n_img) bytes, 16-byte aligned (the descriptors
+ * and 16 bytes per crop pixel).  The descriptors are copied from pageable host memory, which waits for the stream's earlier work.
+ * Per-image results do not depend on the other images of the chunk. */
+#define SCSFM_EVAL_GT_F32 0
+#define SCSFM_EVAL_GT_F64 1
+#define SCSFM_EVAL_OUT 12
+typedef struct ScsfmEvalDepthImage {
+    long long gt_offset;   /* element offset of the image's [H,W] ground truth in `gt` */
+    int H, W;
+    int y1, y2, x1, x2;    /* crop */
+} ScsfmEvalDepthImage;
+size_t scsfm_eval_depth_workspace_bytes(const ScsfmEvalDepthImage* images_host, int n_img);
+int scsfm_eval_depth(const double* pred, int n_img, int h, int w, const void* gt, int gt_dtype, long long gt_elems,
+                     const ScsfmEvalDepthImage* images_host, double min_depth, double max_depth, void* workspace,
+                     size_t workspace_bytes, double* out, void* stream);
+
 /* Training-time image transforms of one batch on the device (reference: custom_transforms.py:21-89 -- RandomHorizontalFlip,
  * RandomScaleCrop, ArrayToTensor, Normalize -- applied per sample by datasets/sequence_folders.py:59-62; the zoom is Pillow's
  * 8-bit BICUBIC Image.resize, restated bit for bit).  images [n_img][B][H][W][3] uint8 (decoded frames, image slot major);

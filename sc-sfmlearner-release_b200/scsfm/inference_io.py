@@ -109,3 +109,46 @@ def integrate(pose_mats):
 
 def batches(n, batch_size):
     return [(i, min(n, i + batch_size)) for i in range(0, n, batch_size)]
+
+
+# --- pose evaluation (test_pose.py) ------------------------------------------------------------------------------------
+def kitti_sequences(dataset_dir, patterns):
+    """Names of the directories under <dataset_dir>/sequences matching any of the fnmatch patterns, SORTED (the reference
+    visits a set, whose order changes from process to process)."""
+    import fnmatch
+    root = os.path.join(dataset_dir, "sequences")
+    return sorted({d for d in os.listdir(root) if os.path.isdir(os.path.join(root, d)) and any(fnmatch.fnmatch(d, p) for p in patterns)})
+
+
+def read_poses(path):
+    """KITTI odometry ground truth: one 3x4 matrix per line, 12 numbers -> float64 [N,3,4]."""
+    return np.genfromtxt(path).astype(np.float64).reshape(-1, 3, 4)
+
+
+def snippet_indices(n_imgs, seq_length=5):
+    """[n_snippets, seq_length] frame indices: every target frame with (seq_length - 1) // 2 frames on each side."""
+    demi = (seq_length - 1) // 2
+    return np.arange(-demi, demi + 1).reshape(1, -1) + np.arange(demi, n_imgs - demi).reshape(-1, 1)
+
+
+def compensated_poses(poses, idx):
+    """Ground-truth poses [len(idx),3,4] of a snippet relative to its first frame: translations minus the first one, then
+    inv(R_first) @ pose."""
+    p = np.stack([poses[i] for i in idx])
+    t0 = p[0, :, -1].copy()
+    p[:, :, -1] -= t0
+    return np.linalg.inv(p[0, :, :3]) @ p
+
+
+def pose_error(gt, pred):
+    """(ATE, RE) of one snippet [L,3,4]: ATE = |t_gt - s t_pred| / L with the least-squares scale s of the translations;
+    RE = mean angle of gt_R @ inv(pred_R) (arctan2 of twice its sine and cosine)."""
+    t_gt, t_pred = gt[:, :, -1], pred[:, :, -1]
+    scale = np.sum(t_gt * t_pred) / np.sum(t_pred ** 2)
+    ate = np.linalg.norm((t_gt - scale * t_pred).reshape(-1))
+    re = 0
+    for g, p in zip(gt, pred):
+        R = g[:, :3] @ np.linalg.inv(p[:, :3])
+        s = np.linalg.norm([R[0, 1] - R[1, 0], R[1, 2] - R[2, 1], R[0, 2] - R[2, 0]])
+        re += np.arctan2(s, np.trace(R) - 1)
+    return ate / gt.shape[0], re / gt.shape[0]

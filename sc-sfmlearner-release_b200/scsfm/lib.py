@@ -34,6 +34,11 @@ class SmoothJob(ctypes.Structure):
     _fields_ = [("depth", ctypes.c_void_p), ("img", ctypes.c_void_p), ("grad_depth", ctypes.c_void_p)]
 
 
+class EvalDepthImage(ctypes.Structure):
+    _fields_ = [("gt_offset", ctypes.c_longlong), ("H", ctypes.c_int), ("W", ctypes.c_int), ("y1", ctypes.c_int), ("y2", ctypes.c_int),
+                ("x1", ctypes.c_int), ("x2", ctypes.c_int)]
+
+
 _lib = None
 
 
@@ -61,6 +66,10 @@ def load():
     lib.scsfm_pose_vec2mat.argtypes = [P, I, I, P, P]
     lib.scsfm_smooth_fwd.argtypes = [ctypes.POINTER(SmoothJob), I, I, I, I, P, P, P]
     lib.scsfm_smooth_bwd.argtypes = [ctypes.POINTER(SmoothJob), I, I, I, I, P, P, P]
+    lib.scsfm_eval_depth_workspace_bytes.restype = ctypes.c_size_t
+    lib.scsfm_eval_depth_workspace_bytes.argtypes = [ctypes.POINTER(EvalDepthImage), I]
+    lib.scsfm_eval_depth.argtypes = [P, I, I, I, P, I, ctypes.c_longlong, ctypes.POINTER(EvalDepthImage), ctypes.c_double,
+                                     ctypes.c_double, P, ctypes.c_size_t, P, P]
     _lib = lib
     return lib
 

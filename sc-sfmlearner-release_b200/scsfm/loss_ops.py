@@ -304,3 +304,92 @@ def compute_errors(gt, pred, y1, y2, x1, x2, max_depth):
     L.launch(lib.scsfm_compute_errors, "scsfm_compute_errors", "eval", 2, 5 * 8.0 * gt.numel(), L.ptr(gt), L.ptr(pred), B, H, W, y1, y2, x1, x2,
              max_depth, L.ptr(work), L.ptr(out), L.stream())
     return out
+
+
+# --- offline evaluation (reference eval_depth.py) ------------------------------------------------------------------------
+EVAL_COLUMNS = ("n", "med_gt", "med_pred", "ratio", "abs_rel", "sq_rel", "rmse", "rmse_log", "log10", "a1", "a2", "a3")
+EVAL_MIN_DEPTH = 1e-3
+EVAL_MAX_DEPTH = {"kitti": 80.0, "nyu": 10.0}
+EVAL_CHUNK = 64          # images per launch: bounds the device memory of a call (KITTI-sized, float32 ground truth: ~0.5 GB)
+
+
+def eigen_crop(H, W):
+    """The reference's KITTI crop of an H x W ground truth (eval_depth.py:186-187): rows [y1,y2) x columns [x1,x2)."""
+    import numpy as np
+    return tuple(int(v) for v in np.array([0.40810811 * H, 0.99189189 * H, 0.03594771 * W, 0.96405229 * W]).astype(np.int32))
+
+
+class _Staging:
+    """Pinned host buffers reused from chunk to chunk (grown when a chunk needs more)."""
+
+    def __init__(self):
+        self.bufs = {}
+
+    def get(self, name, n, dtype):
+        b = self.bufs.get(name)
+        if b is None or b.numel() < n or b.dtype != dtype:
+            b = self.bufs[name] = torch.empty(max(n, 1), dtype=dtype, pin_memory=True)
+        return b[:n]
+
+
+def eval_depth(pred, gt_list, dataset, indices=None, chunk=EVAL_CHUNK):
+    """Per-image results of the reference's median-scaled depth evaluation (eval_depth.py:159-227) on the device
+    (scsfm_eval_depth): float64 numpy [len(indices), 12] with the columns EVAL_COLUMNS.
+
+    pred: float64 [N,h,w] (test_disp.py's predictions.npy; a memory map is fine); gt_list: N or more float32 or float64
+    [H,W] ground truths, of any sizes (a sequence or an array; ground truths past the N-th are ignored); dataset 'kitti'
+    (depth range (1e-3, 80), Eigen crop) or 'nyu' ((1e-3, 10), whole image); indices: the images to evaluate (default all).
+    The images go to the device `chunk` at a time; the results do not depend on the chunk size."""
+    import numpy as np
+    if dataset not in EVAL_MAX_DEPTH:
+        raise ValueError("dataset must be 'kitti' or 'nyu', got %r" % (dataset,))
+    if getattr(pred, "ndim", None) != 3 or pred.dtype != np.float64:
+        raise TypeError("predictions must be a float64 array [N,h,w] (test_disp.py's predictions.npy), got %s %s" %
+                        (getattr(pred, "dtype", type(pred)), getattr(pred, "shape", "")))
+    N, h, w = pred.shape
+    if len(gt_list) < N:
+        raise ValueError("%d predictions but only %d ground-truth depth maps" % (N, len(gt_list)))
+    idx = list(range(N)) if indices is None else [int(i) for i in indices]
+    if any(i < 0 or i >= N for i in idx):
+        raise IndexError("image index outside the %d predictions" % N)
+    if chunk < 1:
+        raise ValueError("chunk must be positive")
+    lib = L.load()
+    dev = torch.device("cuda")
+    stage = _Staging()
+    max_depth = EVAL_MAX_DEPTH[dataset]
+    out = np.empty((len(idx), len(EVAL_COLUMNS)), np.float64)
+    for c0 in range(0, len(idx), chunk):
+        sel = idx[c0:c0 + chunk]
+        gts = [np.asarray(gt_list[i]) for i in sel]
+        dtypes = {g.dtype for g in gts}
+        if not dtypes <= {np.dtype(np.float32), np.dtype(np.float64)} or len(dtypes) != 1 or any(g.ndim != 2 for g in gts):
+            raise TypeError("ground-truth depth maps must be 2-D and all float32 or all float64, got %s" %
+                            sorted({(str(g.dtype), g.ndim) for g in gts}))
+        f64 = gts[0].dtype == np.float64
+        descs = (L.EvalDepthImage * len(sel))()
+        off = 0
+        for k, g in enumerate(gts):
+            H, W = g.shape
+            y1, y2, x1, x2 = eigen_crop(H, W) if dataset == "kitti" else (0, H, 0, W)
+            descs[k] = L.EvalDepthImage(off, H, W, y1, y2, x1, x2)
+            off += g.size
+        host_gt = stage.get("gt", off, torch.float64 if f64 else torch.float32)
+        flat = host_gt.numpy()
+        o = 0
+        for g in gts:
+            flat[o:o + g.size] = g.reshape(-1)
+            o += g.size
+        host_pred = stage.get("pred", len(sel) * h * w, torch.float64)
+        hp = host_pred.numpy().reshape(len(sel), h, w)
+        for k, i in enumerate(sel):
+            hp[k] = pred[i]
+        d_gt = host_gt.to(dev, non_blocking=True)
+        d_pred = host_pred.to(dev, non_blocking=True)
+        ws_bytes = lib.scsfm_eval_depth_workspace_bytes(descs, len(sel))
+        ws = torch.empty((ws_bytes + 15) // 16, 2, dtype=torch.float64, device=dev)
+        res = torch.empty(len(sel), len(EVAL_COLUMNS), dtype=torch.float64, device=dev)
+        L.launch(lib.scsfm_eval_depth, "scsfm_eval_depth", "eval", 1, 4.0 * off + 8.0 * len(sel) * h * w, L.ptr(d_pred), len(sel), h, w,
+                 L.ptr(d_gt), 1 if f64 else 0, off, descs, EVAL_MIN_DEPTH, max_depth, L.ptr(ws), ws.numel() * 8, L.ptr(res), L.stream())
+        out[c0:c0 + len(sel)] = res.cpu().numpy()         # also the point after which the pinned buffers may be refilled
+    return out
