@@ -255,6 +255,12 @@ int scsfm_pad_channels(const float* src, long long rows, int C, int Cpad, float*
 int scsfm_unpad_add(const float* src, long long rows, int C, int Cpad, float* dst, void* stream);
 /* NHWC [B,H,W,C] -> NCHW */
 int scsfm_nhwc_to_nchw(const float* in, int B, int C, int H, int W, float* out, void* stream);
+/* Gradient of the network's input images through the 7x7 stride-2 pad-3 stem (resnet_encoder.py:93): the transposed convolution
+ * of dy [N,Ho,Wo,64] (the stem's pre-BatchNorm gradient, 16-byte aligned; Ho = (H-1)/2+1, Wo = (W-1)/2+1) with the fp32 stem
+ * weights w [64,7,7,Cin], Cin = 3 (DispResNet) or 6 (PoseResNet, the two images concatenated on channels), written (overwritten)
+ * in NCHW: channels 0-2 to dimg1 [N,3,H,W], channels 3-5 to dimg2; a NULL image is skipped.  Exact fp32 FMAs, no atomics:
+ * the result is deterministic. */
+int scsfm_stem_dgrad(const float* dy, const float* w, int N, int H, int W, int Cin, float* dimg1, float* dimg2, void* stream);
 
 /* BatchNorm2d (torchvision resnet.py blocks): prepare per-channel scale/shift from the fused batch sums
  * (sums[SCSFM_BN_SLOTS][groups][C][2], see ScsfmConv.bn_sums)
@@ -275,7 +281,11 @@ int scsfm_bn_apply(const float* y, const double* sums, const float* gamma, const
  * scale (out), shift (out), C, eps as the bits of a float}; one CTA per layer.  scale / shift 8-byte aligned (the convolution epilogues read them as float2). */
 int scsfm_bn_eval_prepare_batched(const long long* table, int n_layers, void* stream);
 /* backward: given dz (gradient of z), z, y -> dy (overwrites `dy`), dres (= dz masked by relu; may be NULL or
- * alias dz), dgamma/dbeta accumulated into. `work` holds groups*C*2 doubles. */
+ * alias dz), dgamma/dbeta accumulated into. `work` holds groups*C*2 doubles.
+ * relu: bit 0 = ReLU gate, SCSFM_ROUND_TF32 = round dy, SCSFM_BN_FROZEN = the statistics in `saved` are frozen (eval mode,
+ * running statistics): dy = scale * dz' instead of the batch-statistics formula, one pass; dgamma / dbeta (both may be NULL,
+ * then no sums are formed) get sum dz' * xhat and sum dz' with xhat from the running mean and invstd. */
+#define SCSFM_BN_FROZEN 0x200
 int scsfm_bn_backward(const float* dz, const float* z, const float* y, const float* saved, const float* gamma,
                       float* dy, float* dy_lo, float* dres, float* dgamma, float* dbeta, long long rows, int C, int groups,
                       int relu, double* work, void* stream);   /* dy_lo (optional): low part of dy (see ScsfmConv.dout_lo) */

@@ -361,6 +361,82 @@ bn_bwd_apply_kernel(const float* __restrict__ dz, const float* __restrict__ z, c
     }
 }
 
+// Frozen statistics (eval mode: `saved` holds the running-statistics {scale, shift, mean, invstd}): dy = scale*dz' and dres = dz'
+// need no batch reduction, so one pass does the apply and, when `work` is given, the parameter-gradient sums
+// work[g][c] = { sum dz', sum dz' * xhat } (xhat from the running mean / invstd).  Grid / thread layout of bn_bwd_reduce_kernel.
+__global__ void __launch_bounds__(NT)
+bn_bwd_frozen_kernel(const float* __restrict__ dz, const float* __restrict__ z, const float* __restrict__ y,
+                     const float* __restrict__ saved, float* __restrict__ dy, float* __restrict__ dy_lo, float* __restrict__ dres,
+                     long long rows_per_group, int C, int relu, int rows_per_cta, double* __restrict__ work) {
+    const int g = blockIdx.y;
+    const int slab4 = min(C >> 2, NT);
+    const int col4 = blockIdx.z * slab4 + (threadIdx.x % slab4);
+    const int row_lanes = NT / slab4, rl = threadIdx.x / slab4;
+    const int c = col4 * 4;
+    const long long r0 = (long long)g * rows_per_group + (long long)blockIdx.x * rows_per_cta;
+    const long long r1 = min((long long)(g + 1) * rows_per_group, r0 + rows_per_cta);
+    float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
+    const bool active = c < C && rl < row_lanes;
+    if (active) {
+        float sc[4], mean[4], invstd[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float* sv = saved + ((size_t)g * C + c + j) * 4;
+            sc[j] = sv[0]; mean[j] = sv[2]; invstd[j] = sv[3];
+        }
+        const bool gate = relu & 1, rnd = relu & ROUND_TF32;
+        for (long long r = r0 + rl; r < r1; r += row_lanes) {
+            const float4 d4 = __ldg(reinterpret_cast<const float4*>(dz + r * C + c));
+            float d[4] = {d4.x, d4.y, d4.z, d4.w};
+            if (gate) {
+                const float4 z4 = __ldg(reinterpret_cast<const float4*>(z + r * C + c));
+                if (!(z4.x > 0.f)) d[0] = 0.f;
+                if (!(z4.y > 0.f)) d[1] = 0.f;
+                if (!(z4.z > 0.f)) d[2] = 0.f;
+                if (!(z4.w > 0.f)) d[3] = 0.f;
+            }
+            float o[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                o[j] = sc[j] * d[j];
+                if (rnd) o[j] = tf32_round(o[j]);
+            }
+            if (dres) *reinterpret_cast<float4*>(dres + r * C + c) = make_float4(d[0], d[1], d[2], d[3]);
+            *reinterpret_cast<float4*>(dy + r * C + c) = make_float4(o[0], o[1], o[2], o[3]);
+            if (dy_lo) *reinterpret_cast<float4*>(dy_lo + r * C + c) = make_float4(tf32_lo(o[0]), tf32_lo(o[1]), tf32_lo(o[2]), tf32_lo(o[3]));
+            if (work) {
+                const float4 y4 = __ldg(reinterpret_cast<const float4*>(y + r * C + c));
+                const float yy[4] = {y4.x, y4.y, y4.z, y4.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    s0[j] += d[j];
+                    s1[j] += d[j] * ((yy[j] - mean[j]) * invstd[j]);
+                }
+            }
+        }
+    }
+    if (!work) return;
+    __shared__ float sh[8][NT];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        sh[j][threadIdx.x] = s0[j];
+        sh[4 + j][threadIdx.x] = s1[j];
+    }
+    __syncthreads();
+    if (threadIdx.x < slab4 && c < C) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            float a = 0.f, b = 0.f;
+            for (int l = 0; l < row_lanes; ++l) {
+                a += sh[j][l * slab4 + threadIdx.x];
+                b += sh[4 + j][l * slab4 + threadIdx.x];
+            }
+            atomicAdd(work + ((size_t)g * C + c + j) * 2, (double)a);
+            atomicAdd(work + ((size_t)g * C + c + j) * 2 + 1, (double)b);
+        }
+    }
+}
+
 __global__ void bn_param_grad_kernel(const double* __restrict__ work, int G, int C, float* __restrict__ dgamma,
                                      float* __restrict__ dbeta) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -717,7 +793,7 @@ extern "C" int scsfm_bn_backward(const float* dz, const float* z, const float* y
                     "bn_backward: bad arguments");
     SCSFM_CHECK_ARG(!(relu & 1) || z, "bn_backward: relu gate needs z");
     const long long rpg = rows / groups;
-    SCSFM_CHECK_CUDA(cudaMemsetAsync(work, 0, (size_t)groups * C * 2 * sizeof(double), ST));
+    const bool param_grads = dgamma || dbeta;
     const int slab4 = (C / 4) < NT ? (C / 4) : NT;
     const int slabs = (C / 4 + slab4 - 1) / slab4;
     const int row_lanes = NT / slab4;
@@ -727,6 +803,19 @@ extern "C" int scsfm_bn_backward(const float* dz, const float* z, const float* y
     if (want > max_chunks) want = max_chunks;
     if (want < 1) want = 1;
     const int rpc = (int)((rpg + want - 1) / want);
+    if (relu & SCSFM_BN_FROZEN) {
+        // running statistics: one pass, and the sums only when a parameter gradient is wanted
+        if (param_grads) SCSFM_CHECK_CUDA(cudaMemsetAsync(work, 0, (size_t)groups * C * 2 * sizeof(double), ST));
+        bn_bwd_frozen_kernel<<<dim3((unsigned)((rpg + rpc - 1) / rpc), groups, slabs), NT, 0, ST>>>(dz, z, y, saved, dy, dy_lo, dres, rpg, C,
+                                                                                                  relu, rpc, param_grads ? work : nullptr);
+        SCSFM_CHECK_LAUNCH();
+        if (param_grads) {
+            bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, ST>>>(work, groups, C, dgamma, dbeta);
+            SCSFM_CHECK_LAUNCH();
+        }
+        return SCSFM_OK;
+    }
+    SCSFM_CHECK_CUDA(cudaMemsetAsync(work, 0, (size_t)groups * C * 2 * sizeof(double), ST));
     bn_bwd_reduce_kernel<<<dim3((unsigned)((rpg + rpc - 1) / rpc), groups, slabs), NT, 0, ST>>>(dz, z, y, saved, rpg, C, relu, rpc, work);
     SCSFM_CHECK_LAUNCH();
     {

@@ -360,6 +360,23 @@ class ArenaNet(nn.Module):
         return p.grad.permute(0, 2, 3, 1) if p.dim() == 4 else p.grad
 
 
+class BackwardPlan:
+    """What one network backward computes.
+      bn:     flags OR-ed into every BatchNorm backward: O.BN_FROZEN when the forward ran in eval mode (it normalised with the
+              running statistics, so the batch-statistics terms of the gradient are absent);
+      params: parameter gradients at all -- False when no parameter of the network requires grad: then no weight-gradient,
+              head-gradient or BatchNorm parameter-gradient work is issued and the gradient arena is left alone;
+      dimg:   one flag per input image (DispResNet 1, PoseResNet 2): its gradient is wanted (the stem's data gradient)."""
+
+    def __init__(self, training=True, params=True, dimg=(False, False)):
+        self.bn = 0 if training else O.BN_FROZEN
+        self.params = params
+        self.dimg = tuple(bool(n) for n in dimg)
+
+
+TRAIN_PLAN = BackwardPlan()
+
+
 class _NetCall(torch.autograd.Function):
     @staticmethod
     def forward(ctx, net, hook, groups, *inputs):
@@ -371,14 +388,20 @@ class _NetCall(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         net = ctx.net
-        net._attach_grads()
-        net._backward_impl(ctx.rec, [None if g is None else g.contiguous() for g in grads])
-        net.ctx.join_wgrad()           # weight gradients enqueued on the side stream (if any) are part of this backward
+        need = ctx.needs_input_grad[3:]
+        # the BatchNorm formula follows the mode the FORWARD ran in (recorded), not net.training now
+        plan = BackwardPlan(ctx.rec["training"], any(p.requires_grad for p, _ in net._views), need)
+        dimgs = [None] * len(need)
+        if plan.params or any(need):
+            if plan.params:
+                net._attach_grads()
+            dimgs = net._backward_impl(ctx.rec, [None if g is None else g.contiguous() for g in grads], plan)
+            net.ctx.join_wgrad()       # weight gradients enqueued on the side stream (if any) are part of this backward
         ctx.rec = None
         net._pending -= 1
         if net._pending == 0 and net.grads_ready_callback is not None:
             net.grads_ready_callback(net)
-        return (None, None, None) + (None,) * (len(ctx.needs_input_grad) - 3)
+        return (None, None, None) + tuple(dimgs)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -435,10 +458,16 @@ def _conv_bn(cx, x, conv, bn, stride, pad, training, relu, residual=None, groups
     return y, z, saved
 
 
-def _conv_bn_bwd(cx, dz, z, y, saved, x, conv, bn, stride, pad, relu, want_dres, need_dx, addend=None, groups=1):
+def _bn_param_grads(bn, plan):
+    return (bn.weight.grad, bn.bias.grad) if plan.params else (None, None)
+
+
+def _conv_bn_bwd(cx, dz, z, y, saved, x, conv, bn, stride, pad, relu, want_dres, need_dx, addend=None, groups=1, plan=TRAIN_PLAN):
     """Backward through relu?(bn(conv(x)) [+res]).  Returns (dx or None, dres or None)."""
-    dy, dres = O.bn_backward(dz, z, y, saved, bn.weight.grad, bn.bias.grad, (1 if relu else 0) | cx.rnd(), want_dres, groups, cx.split)
-    cx.conv_wgrad(x, dy, ArenaNet.g(conv.weight), None, stride, pad, O.PAD_ZERO)
+    dy, dres = O.bn_backward(dz, z, y, saved, *_bn_param_grads(bn, plan), (1 if relu else 0) | cx.rnd() | plan.bn, want_dres, groups,
+                             cx.split)
+    if plan.params:
+        cx.conv_wgrad(x, dy, ArenaNet.g(conv.weight), None, stride, pad, O.PAD_ZERO)
     dx = cx.conv_dgrad(dy, conv.w_op(cx), x.shape, stride, pad, addend) if need_dx else None
     return dx, dres
 
@@ -465,27 +494,28 @@ def block_forward(cx, blk, x, training, G=1):
     return r, out
 
 
-def block_backward(cx, blk, r, d_out, extra_addend=None):
+def block_backward(cx, blk, r, d_out, extra_addend=None, plan=TRAIN_PLAN):
     """d_out: gradient w.r.t. the block output (consumed / overwritten).  extra_addend: gradient that reaches
     the block INPUT from elsewhere (decoder skip connection) -- folded into the dgrad epilogue chain.
     Returns gradient w.r.t. the block input."""
     x, G = r["x"], r["G"]
     if blk.bottleneck:
-        dh2, dres = _conv_bn_bwd(cx, d_out, r["out"], r["y3"], r["s3"], r["h2"], blk.conv3, blk.bn3, 1, 0, True, True, True, None, G)
-        dh1, _ = _conv_bn_bwd(cx, dh2, r["h2"], r["y2"], r["s2"], r["h1"], blk.conv2, blk.bn2, blk.stride, 1, True, False, True, None, G)
+        dh2, dres = _conv_bn_bwd(cx, d_out, r["out"], r["y3"], r["s3"], r["h2"], blk.conv3, blk.bn3, 1, 0, True, True, True, None, G, plan)
+        dh1, _ = _conv_bn_bwd(cx, dh2, r["h2"], r["y2"], r["s2"], r["h1"], blk.conv2, blk.bn2, blk.stride, 1, True, False, True, None, G,
+                              plan)
         first = (dh1, r["h1"], r["y1"], r["s1"], blk.conv1, blk.bn1, 1, 0)
     else:
-        dh1, dres = _conv_bn_bwd(cx, d_out, r["out"], r["y2"], r["s2"], r["h1"], blk.conv2, blk.bn2, 1, 1, True, True, True, None, G)
+        dh1, dres = _conv_bn_bwd(cx, d_out, r["out"], r["y2"], r["s2"], r["h1"], blk.conv2, blk.bn2, 1, 1, True, True, True, None, G, plan)
         first = (dh1, r["h1"], r["y1"], r["s1"], blk.conv1, blk.bn1, blk.stride, 1)
     if blk.downsample is not None:
         d_sc, _ = _conv_bn_bwd(cx, dres, None, r["yd"], r["sd"], x, blk.downsample[0], blk.downsample[1], blk.stride, 0, False,
-                               False, True, extra_addend, G)
+                               False, True, extra_addend, G, plan)
     else:
         d_sc = dres
         if extra_addend is not None:
             d_sc = d_sc + extra_addend          # not reached by ResNet-18/50 (skips feed downsample blocks)
     dz, z, y, s, conv, bn, st, pd = first
-    dx, _ = _conv_bn_bwd(cx, dz, z, y, s, x, conv, bn, st, pd, True, False, True, d_sc, G)
+    dx, _ = _conv_bn_bwd(cx, dz, z, y, s, x, conv, bn, st, pd, True, False, True, d_sc, G, plan)
     return dx
 
 
@@ -575,8 +605,9 @@ def encoder_forward_eval(cx, enc, imgs, coeffs):
     return feats
 
 
-def encoder_backward(cx, enc, rec, d_feats):
-    """d_feats[i]: gradient w.r.t. feature i coming from the decoder (None if unused).  d_feats[4] is required."""
+def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
+    """d_feats[i]: gradient w.r.t. feature i coming from the decoder (None if unused).  d_feats[4] is required.
+    Returns the gradients of the input images (NCHW, one per image of the forward; None where plan.dimg does not ask)."""
     t = enc.encoder
     blocks = rec["blocks"]
     # index of the last block of each layer -> the feature it produces
@@ -591,7 +622,7 @@ def encoder_backward(cx, enc, rec, d_feats):
         extra = None
         if bi - 1 in ends and d_feats[ends[bi - 1]] is not None:
             extra = d_feats[ends[bi - 1]]
-        d = block_backward(cx, blk, r, d, extra)
+        d = block_backward(cx, blk, r, d, extra, plan)
     # d is now the gradient w.r.t. the max-pool output
     f0 = rec["f0"]
     if d_feats[0] is not None:
@@ -601,15 +632,24 @@ def encoder_backward(cx, enc, rec, d_feats):
         d_f0 = torch.empty_like(f0)
         O.maxpool_bwd(d, rec["pool_idx"], f0.shape, d_f0, False)
     x = rec["x"]
+    relu = 1 | cx.rnd() | plan.bn
     if x.shape[-1] != t.conv1.weight.shape[1]:
-        # padded-channel stem (tf32 mode): weight gradient in the padded layout, then folded into the gradient arena
-        dy, _ = O.bn_backward(d_f0, f0, rec["y0"], rec["s0"], t.bn1.weight.grad, t.bn1.bias.grad, 1 | cx.rnd(), False, rec["G"], cx.split)
-        dw = torch.zeros(t.conv1.weight.shape[0], t.conv1.k, t.conv1.k, x.shape[-1], device=x.device, dtype=torch.float32)
-        cx.conv_wgrad(x, dy, dw, None, 2, 3, O.PAD_ZERO)
-        with cx.on_wgrad_stream([dw]):
-            O.unpad_add_(ArenaNet.g(t.conv1.weight), dw)
+        # padded-channel stem (tensor-core modes): weight gradient in the padded layout, then folded into the gradient arena
+        # (the low part of dy is only read by that weight gradient)
+        dy, _ = O.bn_backward(d_f0, f0, rec["y0"], rec["s0"], *_bn_param_grads(t.bn1, plan), relu, False, rec["G"], cx.split and plan.params)
+        if plan.params:
+            dw = torch.zeros(t.conv1.weight.shape[0], t.conv1.k, t.conv1.k, x.shape[-1], device=x.device, dtype=torch.float32)
+            cx.conv_wgrad(x, dy, dw, None, 2, 3, O.PAD_ZERO)
+            with cx.on_wgrad_stream([dw]):
+                O.unpad_add_(ArenaNet.g(t.conv1.weight), dw)
     else:
-        _conv_bn_bwd(cx, d_f0, f0, rec["y0"], rec["s0"], x, t.conv1, t.bn1, 2, 3, True, False, False, None, rec["G"])
+        dy, _ = O.bn_backward(d_f0, f0, rec["y0"], rec["s0"], *_bn_param_grads(t.bn1, plan), relu, False, rec["G"], cx.split)
+        if plan.params:
+            cx.conv_wgrad(x, dy, ArenaNet.g(t.conv1.weight), None, 2, 3, O.PAD_ZERO)
+    if not any(plan.dimg):
+        return [None] * len(plan.dimg)
+    # input images: the transposed stem convolution with the fp32 weights (not the padded / TF32 operand copies)
+    return O.stem_dgrad(dy, t.conv1.w_khwc(), x.shape[1], x.shape[2], plan.dimg)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -664,7 +704,7 @@ class DispResNet(ArenaNet):
         else:
             enc_rec, feats = encoder_forward(cx, self.encoder, (x,), training, groups)
         dec = self.decoder
-        rec = {"enc": enc_rec, "stages": {}}
+        rec = {"enc": enc_rec, "stages": {}, "training": training}
         cur = feats[4]
         disps = {}
         for i in range(4, -1, -1):
@@ -692,7 +732,8 @@ class DispResNet(ArenaNet):
         return None if fused else rec, [disps[s].view(disps[s].shape[0], 1, disps[s].shape[1], disps[s].shape[2]) for s in order]
 
     # -- backward -----------------------------------------------------------------------------
-    def _backward_impl(self, rec, grads):
+    def _backward_impl(self, rec, grads, plan=TRAIN_PLAN):
+        """Returns [gradient of the input images or None] (see encoder_backward)."""
         dec = self.decoder
         g = ArenaNet.g
         cx = self.ctx
@@ -709,7 +750,8 @@ class DispResNet(ArenaNet):
                 dc = dec.disp(i)
                 disp = rec["disps"][i]
                 dpre = O.act_bwd_(d_disp[i].reshape(disp.shape).clone(), disp, O.ACT_DISP)
-                O.head_wgrad(b, dpre, g(dc.weight), dc.bias.grad)
+                if plan.params:
+                    O.head_wgrad(b, dpre, g(dc.weight), dc.bias.grad)
                 dpad = O.head_dgrad(dpre, dc.w_khwc(), b.shape)
                 if not have:
                     d_b = torch.empty_like(b)
@@ -720,14 +762,16 @@ class DispResNet(ArenaNet):
                 continue            # nothing reaches this stage (cannot happen: stage 0 always has scale 0)
             # up(i,1): b = ELU(conv(reflect_pad(cat)))
             c1 = dec.up(i, 1)
-            cx.conv_wgrad(st["cat"], d_b, g(c1.weight), c1.bias.grad, 1, 1, O.PAD_REFLECT)
+            if plan.params:
+                cx.conv_wgrad(st["cat"], d_b, g(c1.weight), c1.bias.grad, 1, 1, O.PAD_REFLECT)
             dpad = cx.conv_dgrad(d_b, c1.w_op(cx), st["cat"].shape, 1, 1, None, padded_input=True)
             d_a, d_skip = O.fold_upcat(dpad, st["a"].shape[-1], st["a"], O.ACT_ELU | cx.rnd())
             if i > 0:
                 d_feats[i - 1] = d_skip
             # up(i,0): a = ELU(conv(reflect_pad(in0)))
             c0 = dec.up(i, 0)
-            cx.conv_wgrad(st["in0"], d_a, g(c0.weight), c0.bias.grad, 1, 1, O.PAD_REFLECT)
+            if plan.params:
+                cx.conv_wgrad(st["in0"], d_a, g(c0.weight), c0.bias.grad, 1, 1, O.PAD_REFLECT)
             dpad = cx.conv_dgrad(d_a, c0.w_op(cx), st["in0"].shape, 1, 1, None, padded_input=True)
             d_in = torch.empty_like(st["in0"])
             O.fold_plain(dpad, d_in, None, O.ACT_NONE, accumulate=False)
@@ -735,7 +779,7 @@ class DispResNet(ArenaNet):
                 pending = d_in          # = raw gradient of b_{i+1}; ELU' applied once all consumers are in
             else:
                 d_feats[4] = d_in
-        encoder_backward(cx, self.encoder, rec["enc"], d_feats)
+        return encoder_backward(cx, self.encoder, rec["enc"], d_feats, plan)
 
 
 class PoseResNet(ArenaNet):
@@ -789,25 +833,27 @@ class PoseResNet(ArenaNet):
             p2 = cx.conv_fwd(p1, n[3].w_op(cx), n[3].bias, 1, 0, O.PAD_ZERO, O.ACT_NONE, None, 1, n[3].w_lo(cx))
             return None, [O.spatial_mean_fwd(p2, 0.01)]
         enc_rec, feats = encoder_forward(cx, self.encoder, (img1, img2), self.training, groups)
-        rec = {"enc": enc_rec, "f4": feats[4]}
+        rec = {"enc": enc_rec, "f4": feats[4], "training": self.training}
         rec["s"] = cx.conv_fwd(feats[4], n[0].w_op(cx), n[0].bias, 1, 0, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[0].w_lo(cx))
         rec["p0"] = cx.conv_fwd(rec["s"], n[1].w_op(cx), n[1].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[1].w_lo(cx))
         rec["p1"] = cx.conv_fwd(rec["p0"], n[2].w_op(cx), n[2].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[2].w_lo(cx))
         rec["p2"] = cx.conv_fwd(rec["p1"], n[3].w_op(cx), n[3].bias, 1, 0, O.PAD_ZERO, O.ACT_NONE, None, 1, n[3].w_lo(cx))
         return rec, [O.spatial_mean_fwd(rec["p2"], 0.01)]
 
-    def _backward_impl(self, rec, grads):
+    def _backward_impl(self, rec, grads, plan=TRAIN_PLAN):
+        """Returns [gradient of img1 or None, gradient of img2 or None] (see encoder_backward)."""
         n = self.decoder.net
         g = ArenaNet.g
         cx = self.ctx
         d = O.spatial_mean_bwd(grads[0], rec["p2"].shape, 0.01)
         chain = [(n[3], rec["p1"], 0), (n[2], rec["p0"], 1), (n[1], rec["s"], 1), (n[0], rec["f4"], 0)]
         for k, (conv, inp, pad) in enumerate(chain):
-            cx.conv_wgrad(inp, d, g(conv.weight), conv.bias.grad, 1, pad, O.PAD_ZERO)
+            if plan.params:
+                cx.conv_wgrad(inp, d, g(conv.weight), conv.bias.grad, 1, pad, O.PAD_ZERO)
             d = cx.conv_dgrad(d, conv.w_op(cx), inp.shape, 1, pad)
             if k < 3:
                 O.act_bwd_(d, inp, O.ACT_RELU | cx.rnd())       # inp is the ReLU output of the previous conv
-        encoder_backward(cx, self.encoder, rec["enc"], [None, None, None, None, d])
+        return encoder_backward(cx, self.encoder, rec["enc"], [None, None, None, None, d], plan)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -13,6 +13,7 @@ PAD_ZERO, PAD_REFLECT = 0, 1
 ACT_NONE, ACT_RELU, ACT_ELU, ACT_DISP = 0, 1, 2, 3
 BN_SLOTS = 16      # SCSFM_BN_SLOTS: replicas of the fused BatchNorm sums
 ROUND_TF32 = 0x100  # SCSFM_ROUND_TF32: store the result rounded to TF32 (operand of a tensor-core conv)
+BN_FROZEN = 0x200   # SCSFM_BN_FROZEN: bn_backward with the running statistics held fixed (eval mode)
 OPERAND_TF32, OPERAND_RAW, OPERAND_LO = 0, 1, 2      # SCSFM_OPERAND_*
 
 # Arithmetic of the convolutions (a property of each network, see ConvCtx -- there is no process-global mode):
@@ -62,6 +63,7 @@ def _lib():
         lib.scsfm_weight_flip_batched.argtypes = [P, I, I, P]
         lib.scsfm_nchw_to_nhwc.argtypes = [P, P, I, I, I, I, P, P]
         lib.scsfm_nhwc_to_nchw.argtypes = [P, I, I, I, I, P, P]
+        lib.scsfm_stem_dgrad.argtypes = [P, P, I, I, I, I, P, P, P]
         lib.scsfm_head_conv_fwd.argtypes = [P, P, P, P, I, I, I, I, I, P]
         lib.scsfm_head_conv_wgrad.argtypes = [P, P, P, P, I, I, I, I, P]
         lib.scsfm_head_conv_dgrad.argtypes = [P, P, P, I, I, I, I, P]
@@ -416,6 +418,18 @@ def nhwc_to_nchw(x):
     return out
 
 
+def stem_dgrad(dy, w, H, W, need):
+    """Gradient of the input images of a 7x7 stride-2 pad-3 stem: dy [N,Ho,Wo,64] (pre-BatchNorm gradient), w [64,7,7,Cin] the fp32
+    stem weights (Cin 3: one image, 6: two images concatenated on channels), `need` one flag per image.  Returns one NCHW
+    [N,3,H,W] tensor per image (None where not needed)."""
+    N, Cin = dy.shape[0], w.shape[-1]
+    outs = [empty((N, 3, H, W), dy) if n else None for n in need]
+    outs += [None] * (2 - len(outs))
+    L.launch(_lib().scsfm_stem_dgrad, "scsfm_stem_dgrad", "stem_dgrad", 1, 2.0 * N * H * W * Cin * 64 * 49 / 4, L.ptr(dy), L.ptr(w),
+             N, H, W, Cin, L.ptr(outs[0]), L.ptr(outs[1]), L.stream())
+    return outs[:len(need)]
+
+
 def bn_prepare(sums, groups, count, gamma, beta, rmean, rvar, momentum, eps, training):
     C = gamma.numel()
     saved = empty((groups, C, 4), gamma)
@@ -480,14 +494,16 @@ def _aligned64(n):
 
 def bn_backward(dz, z, y, saved, dgamma, dbeta, relu, want_dres, groups=1, with_lo=False):
     """Returns (dy, dres).  dres (= dz gated by the ReLU) is written in place over dz when requested.  with_lo: also
-    produce lo(dy) (attached to dy like lo_of() would)."""
+    produce lo(dy) (attached to dy like lo_of() would).  relu | BN_FROZEN: frozen statistics (eval mode), one pass; dgamma and
+    dbeta may then be None (no parameter gradient, no sums)."""
     C = y.shape[-1]
     rows = y.numel() // C
     dy = torch.empty_like(y)
     dy_lo = torch.empty_like(y) if with_lo else None
     work = torch.empty(groups * C * 2, device=y.device, dtype=torch.float64)
     dres = dz if want_dres else None
-    L.launch(_lib().scsfm_bn_backward, "scsfm_bn_backward", "bn_bwd", 4, 28.0 * y.numel(), L.ptr(dz), L.ptr(z), L.ptr(y), L.ptr(saved), None, L.ptr(dy),
+    frozen = int(relu) & BN_FROZEN
+    L.launch(_lib().scsfm_bn_backward, "scsfm_bn_backward", "bn_bwd", 2 if frozen else 4, (20.0 if frozen else 28.0) * y.numel(), L.ptr(dz), L.ptr(z), L.ptr(y), L.ptr(saved), None, L.ptr(dy),
              L.ptr(dy_lo), L.ptr(dres), L.ptr(dgamma), L.ptr(dbeta), rows, C, groups, int(relu), L.ptr(work), L.stream())
     if with_lo:
         dy._scsfm_lo = dy_lo
