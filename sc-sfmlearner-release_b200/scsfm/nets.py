@@ -14,6 +14,7 @@ section 2.2).  Differences from a stock nn.Module network:
 
 There is no CPU path: calling a network on CPU tensors raises.
 """
+import collections
 import math
 
 import torch
@@ -99,6 +100,17 @@ class Block(nn.Module):
         if stride != 1 or cin != cout:
             self.downsample = nn.Sequential(ConvParams(cin, cout, 1, False, "kaiming_fan_out"), BNParams(cout))
         self.cout = cout
+
+    def units(self):
+        """The block's convolutions as (conv, bn, stride, pad) units: the main path in forward order (every unit followed by a
+        ReLU, the last one after the residual add), and the downsample unit of the shortcut or None.  Plain tuples of the
+        registered submodules: nothing here is registered again."""
+        if self.bottleneck:
+            main = [(self.conv1, self.bn1, 1, 0), (self.conv2, self.bn2, self.stride, 1), (self.conv3, self.bn3, 1, 0)]
+        else:
+            main = [(self.conv1, self.bn1, self.stride, 1), (self.conv2, self.bn2, 1, 1)]
+        ds = None if self.downsample is None else (self.downsample[0], self.downsample[1], self.stride, 0)
+        return main, ds
 
 
 class Trunk(nn.Module):
@@ -191,13 +203,19 @@ class PoseDecoder(nn.Module):
                                   ConvParams(256, 6, 1, True, "default")])
 
 
+# PoseDecoder.net[k] in forward order as (pad, activation); all four convolutions have stride 1 and a bias.
+POSE_HEAD = ((0, O.ACT_RELU), (1, O.ACT_RELU), (1, O.ACT_RELU), (0, O.ACT_NONE))
+
+
+def _pose_act(cx, k):
+    """Activation flags of pose-head convolution k: the output of every one but the last feeds the next convolution."""
+    act = POSE_HEAD[k][1]
+    return act | cx.rnd() if k + 1 < len(POSE_HEAD) else act
+
+
 # ------------------------------------------------------------------------------------------------
 # flat parameter / gradient arenas
 # ------------------------------------------------------------------------------------------------
-def _aligned(n, quantum=64):
-    return (n + quantum - 1) // quantum * quantum
-
-
 class ArenaNet(nn.Module):
     """Base class: owns the flat arenas and the single-autograd-node plumbing."""
 
@@ -235,7 +253,7 @@ class ArenaNet(nn.Module):
         for p in self.parameters():
             if p.data_ptr() != self._flat.data_ptr() + 4 * off:
                 return False
-            off += _aligned(p.numel())
+            off += O.aligned64(p.numel())
         return True
 
     def ensure_arena(self):
@@ -247,9 +265,13 @@ class ArenaNet(nn.Module):
         dev = params[0].device
         if dev.type != "cuda":
             raise RuntimeError("the networks run on CUDA only (no CPU fallback): move the module with .to('cuda')")
-        n = sum(_aligned(p.numel()) for p in params)      # every tensor starts on a 256-byte boundary (float4 loads)
+        n = sum(O.aligned64(p.numel()) for p in params)      # every tensor starts on a 256-byte boundary (float4 loads)
         flat = torch.zeros(n, device=dev, dtype=torch.float32)
         gflat = torch.zeros(n, device=dev, dtype=torch.float32)
+        # operand mirror of the parameter arena for the tensor-core kernels: the TF32-rounded parameters in tf32 mode, their
+        # low parts in tf32x3 mode (refreshed at the start of a network call when stale; ArenaAdam writes it with the update)
+        self._flat_tf32 = torch.zeros_like(flat)
+        convs = {id(m.weight): m for m in self.modules() if isinstance(m, ConvParams)}
         views, off = [], 0
         for p in params:
             cnt = p.numel()
@@ -257,6 +279,7 @@ class ArenaNet(nn.Module):
                 O_, I_, kh, kw = p.shape
                 dst = flat[off:off + cnt].view(O_, kh, kw, I_).permute(0, 3, 1, 2)
                 gv = gflat[off:off + cnt].view(O_, kh, kw, I_).permute(0, 3, 1, 2)
+                convs[id(p)]._tc_view = self._flat_tf32[off:off + cnt].view(O_, kh, kw, I_)
             else:
                 dst = flat[off:off + cnt].view(p.shape)
                 gv = gflat[off:off + cnt].view(p.shape)
@@ -264,7 +287,7 @@ class ArenaNet(nn.Module):
             p.data = dst
             p.grad = gv
             views.append((p, gv))
-            off += _aligned(cnt)
+            off += O.aligned64(cnt)
         self._flat, self._flat_grad, self._views = flat, gflat, views
         self._hook = torch.zeros(1, device=dev, requires_grad=True)
         # num_batches_tracked of all BatchNorm layers as views of one int64 tensor (one add per network call)
@@ -276,19 +299,8 @@ class ArenaNet(nn.Module):
             for m in self.modules():
                 if isinstance(m, ResnetEncoder):
                     m._nbt = nbt
-        # operand mirror of the parameter arena for the tensor-core kernels: the TF32-rounded parameters in tf32 mode, their
-        # low parts in tf32x3 mode (refreshed at the start of a network call when stale; ArenaAdam writes it with the update)
-        self._flat_tf32 = torch.zeros_like(flat)
         self._tf32_version = None
         self.ctx.invalidate()              # cached flips referred to the previous arena
-        off = 0
-        mods = {id(m.weight): m for m in self.modules() if isinstance(m, ConvParams)}
-        for p in params:
-            cnt = p.numel()
-            if p.dim() == 4 and id(p) in mods:
-                O_, I_, kh, kw = p.shape
-                mods[id(p)]._tc_view = self._flat_tf32[off:off + cnt].view(O_, kh, kw, I_)
-            off += _aligned(cnt)
 
     trust_adam_mirror = False      # see refresh_operand_weights
     _tf32_version = None
@@ -316,8 +328,25 @@ class ArenaNet(nn.Module):
 
     def _fused_eval(self):
         """Eval mode with autograd off: the forward runs without recording (every activation is freed once dead) and with
-        BatchNorm fused into the convolution epilogues (see encoder_forward_eval)."""
+        BatchNorm fused into the convolution epilogues (see _conv_bn)."""
         return not self.training and not torch.is_grad_enabled()
+
+    def _call(self, inputs, groups=None):
+        """One network call on `inputs`: the fused eval forward, or one autograd node.  groups=None returns the call's
+        outputs; otherwise the inputs stack `groups` equal sample groups on the batch axis (BatchNorm statistics stay per
+        group) and the result is one output list per group."""
+        G = groups or 1
+        self.ensure_arena()
+        if self._fused_eval():
+            outs = self._forward_impl(G, *inputs, fused=True)[1]
+        else:
+            if torch.is_grad_enabled():
+                self._pending += 1
+            outs = _NetCall.apply(self, self._hook, G, *inputs)
+        if groups is None:
+            return outs
+        B = inputs[0].shape[0] // G
+        return [[o[g * B:(g + 1) * B] for o in outs] for g in range(G)]
 
     def bn_eval_coeffs(self):
         """Eval-mode {scale, shift} of every BatchNorm layer, recomputed from the current parameters and running statistics
@@ -442,89 +471,117 @@ def _pool(cx):
     return cx.sums_pool
 
 
-def _bn_fwd(cx, y, sums, bn, training, relu, residual, groups):
-    """BatchNorm over `groups` independent sample groups (one per batched network call: statistics, and the
-    running-stat updates, stay per call exactly as in train.py:427-442).  num_batches_tracked of every layer is bumped
-    by one add per network call (ArenaNet._nbt, see encoder_forward)."""
-    return O.bn_apply(y, sums if training else None, bn.weight, bn.bias, bn.running_mean, bn.running_var, BN_MOMENTUM, BN_EPS,
-                      residual, (1 if relu else 0) | cx.rnd(), groups, cx.split)
+class _Forward:
+    """What differs between the forwards of one network call.  Recording (coeffs None): BatchNorm with batch statistics
+    (training) or the running ones over `groups` independent sample groups, and every unit returns its record for the
+    backward.  Fused (coeffs = ArenaNet.bn_eval_coeffs()): eval-mode BatchNorm in the convolution epilogues, no record."""
+
+    def __init__(self, net, groups, fused):
+        self.cx, self.training, self.groups = net.ctx, net.training, groups
+        self.coeffs = net.bn_eval_coeffs() if fused else None
+
+    @property
+    def fused(self):
+        return self.coeffs is not None
 
 
-def _conv_bn(cx, x, conv, bn, stride, pad, training, relu, residual=None, groups=1):
-    C = conv.weight.shape[0]
-    sums = _pool(cx).take(O.BN_SLOTS * groups * C * 2, x.device) if training else None
-    y = cx.conv_fwd(x, conv.w_op(cx), None, stride, pad, O.PAD_ZERO, O.ACT_NONE, sums, groups, conv.w_lo(cx))
-    z, saved = _bn_fwd(cx, y, sums, bn, training, relu, residual, groups)
-    return y, z, saved
+# One conv+BatchNorm unit of the recording forward: its input x, the convolution output y, the unit output z and the
+# BatchNorm's saved statistics.  z is kept only where a ReLU follows (the backward reads it for the ReLU's gate), so that
+# the record does not hold the downsample's output until the backward.
+_Unit = collections.namedtuple("_Unit", "x y z saved")
+
+
+def _conv_bn(f, x, unit, relu, residual=None, with_lo=False, w=None):
+    """z = relu?(bn(conv(x)) [+ residual]) for unit (conv, bn, stride, pad); returns (z, its _Unit record or None).
+    w: (operand weights, their low part) in place of the unit's own (the padded stem).
+    Fused: ONE convolution with BatchNorm, residual, ReLU and TF32 rounding in its epilogue (bitwise conv_fwd followed by
+    bn_apply); with_lo: z feeds a tensor-core convolution (tf32x3: write its low part too).
+    Recording: BatchNorm statistics, and the running-stat updates, stay per sample group (one per batched network call,
+    exactly as in train.py:427-442); bn_apply writes lo(z) in every tf32x3 call."""
+    conv, bn, stride, pad = unit
+    cx = f.cx
+    w, w_lo = (conv.w_op(cx), conv.w_lo(cx)) if w is None else w
+    if f.fused:
+        sc, sh = f.coeffs[id(bn)]
+        z = cx.conv_fwd(x, w, None, stride, pad, O.PAD_ZERO, (O.ACT_RELU if relu else O.ACT_NONE) | cx.rnd(), None, 1, w_lo,
+                        bn_scale=sc, bn_shift=sh, addend=residual, with_lo=with_lo and cx.split)
+        return z, None
+    G = f.groups
+    sums = _pool(cx).take(O.BN_SLOTS * G * conv.weight.shape[0] * 2, x.device) if f.training else None
+    y = cx.conv_fwd(x, w, None, stride, pad, O.PAD_ZERO, O.ACT_NONE, sums, G, w_lo)
+    z, saved = O.bn_apply(y, sums, bn.weight, bn.bias, bn.running_mean, bn.running_var, BN_MOMENTUM, BN_EPS, residual,
+                          (1 if relu else 0) | cx.rnd(), G, cx.split)
+    return z, _Unit(x, y, z if relu else None, saved)
 
 
 def _bn_param_grads(bn, plan):
     return (bn.weight.grad, bn.bias.grad) if plan.params else (None, None)
 
 
-def _conv_bn_bwd(cx, dz, z, y, saved, x, conv, bn, stride, pad, relu, want_dres, need_dx, addend=None, groups=1, plan=TRAIN_PLAN):
-    """Backward through relu?(bn(conv(x)) [+res]).  Returns (dx or None, dres or None)."""
-    dy, dres = O.bn_backward(dz, z, y, saved, *_bn_param_grads(bn, plan), (1 if relu else 0) | cx.rnd() | plan.bn, want_dres, groups,
-                             cx.split)
+def _conv_bn_bwd(cx, dz, unit, r, relu, want_dres, addend, groups, plan):
+    """Backward through relu?(bn(conv(x)) [+res]) of `unit` with record `r`; `addend` is added to dx in the data gradient's
+    epilogue.  Returns (dx, dres or None)."""
+    conv, bn, stride, pad = unit
+    dy, dres = O.bn_backward(dz, r.z, r.y, r.saved, *_bn_param_grads(bn, plan), (1 if relu else 0) | cx.rnd() | plan.bn, want_dres,
+                             groups, cx.split)
     if plan.params:
-        cx.conv_wgrad(x, dy, ArenaNet.g(conv.weight), None, stride, pad, O.PAD_ZERO)
-    dx = cx.conv_dgrad(dy, conv.w_op(cx), x.shape, stride, pad, addend) if need_dx else None
-    return dx, dres
+        cx.conv_wgrad(r.x, dy, ArenaNet.g(conv.weight), None, stride, pad, O.PAD_ZERO)
+    return cx.conv_dgrad(dy, conv.w_op(cx), r.x.shape, stride, pad, addend), dres
 
 
-def block_forward(cx, blk, x, training, G=1):
-    r = {"x": x, "G": G}
-    if blk.bottleneck:
-        r["y1"], r["h1"], r["s1"] = _conv_bn(cx, x, blk.conv1, blk.bn1, 1, 0, training, True, None, G)
-        r["y2"], r["h2"], r["s2"] = _conv_bn(cx, r["h1"], blk.conv2, blk.bn2, blk.stride, 1, training, True, None, G)
-        last_in, last_conv, last_bn, key = r["h2"], blk.conv3, blk.bn3, "3"
-        ls, lp = 1, 0
+def block_forward(f, blk, x):
+    """Returns (block output, record: (main-path unit records, downsample record or None); None in the fused forward)."""
+    main, ds = blk.units()
+    h, recs = x, []
+    for unit in main[:-1]:
+        h, r = _conv_bn(f, h, unit, True, with_lo=True)
+        recs.append(r)
+    # the shortcut runs between the main path's first convolution(s) and its last one
+    sc, ds_rec = (x, None) if ds is None else _conv_bn(f, x, ds, False)
+    out, r = _conv_bn(f, h, main[-1], True, sc, with_lo=True)
+    return out, None if f.fused else (recs + [r], ds_rec)
+
+
+def block_backward(cx, blk, rec, d_out, d_skip, groups, plan):
+    """d_out: gradient w.r.t. the block output (consumed / overwritten).  d_skip: gradient that reaches the block INPUT from
+    the decoder (skip connection) or None -- folded into the shortcut's dgrad epilogue.  Returns gradient w.r.t. the block
+    input."""
+    main, ds = blk.units()
+    recs, ds_rec = rec
+    d, dres = _conv_bn_bwd(cx, d_out, main[-1], recs[-1], True, True, None, groups, plan)
+    for k in range(len(main) - 2, 0, -1):
+        d, _ = _conv_bn_bwd(cx, d, main[k], recs[k], True, False, None, groups, plan)
+    if ds is not None:
+        d_sc, _ = _conv_bn_bwd(cx, dres, ds, ds_rec, False, False, d_skip, groups, plan)
     else:
-        r["y1"], r["h1"], r["s1"] = _conv_bn(cx, x, blk.conv1, blk.bn1, blk.stride, 1, training, True, None, G)
-        last_in, last_conv, last_bn, key = r["h1"], blk.conv2, blk.bn2, "2"
-        ls, lp = 1, 1
-    sc = x
-    if blk.downsample is not None:
-        r["yd"], sc, r["sd"] = _conv_bn(cx, x, blk.downsample[0], blk.downsample[1], blk.stride, 0, training, False, None, G)
-    C = last_conv.weight.shape[0]
-    sums = _pool(cx).take(O.BN_SLOTS * G * C * 2, x.device) if training else None
-    y = cx.conv_fwd(last_in, last_conv.w_op(cx), None, ls, lp, O.PAD_ZERO, O.ACT_NONE, sums, G, last_conv.w_lo(cx))
-    out, saved = _bn_fwd(cx, y, sums, last_bn, training, True, sc, G)
-    r["y" + key], r["s" + key], r["out"] = y, saved, out
-    return r, out
-
-
-def block_backward(cx, blk, r, d_out, extra_addend=None, plan=TRAIN_PLAN):
-    """d_out: gradient w.r.t. the block output (consumed / overwritten).  extra_addend: gradient that reaches
-    the block INPUT from elsewhere (decoder skip connection) -- folded into the dgrad epilogue chain.
-    Returns gradient w.r.t. the block input."""
-    x, G = r["x"], r["G"]
-    if blk.bottleneck:
-        dh2, dres = _conv_bn_bwd(cx, d_out, r["out"], r["y3"], r["s3"], r["h2"], blk.conv3, blk.bn3, 1, 0, True, True, True, None, G, plan)
-        dh1, _ = _conv_bn_bwd(cx, dh2, r["h2"], r["y2"], r["s2"], r["h1"], blk.conv2, blk.bn2, blk.stride, 1, True, False, True, None, G,
-                              plan)
-        first = (dh1, r["h1"], r["y1"], r["s1"], blk.conv1, blk.bn1, 1, 0)
-    else:
-        dh1, dres = _conv_bn_bwd(cx, d_out, r["out"], r["y2"], r["s2"], r["h1"], blk.conv2, blk.bn2, 1, 1, True, True, True, None, G, plan)
-        first = (dh1, r["h1"], r["y1"], r["s1"], blk.conv1, blk.bn1, blk.stride, 1)
-    if blk.downsample is not None:
-        d_sc, _ = _conv_bn_bwd(cx, dres, None, r["yd"], r["sd"], x, blk.downsample[0], blk.downsample[1], blk.stride, 0, False,
-                               False, True, extra_addend, G, plan)
-    else:
+        # a skip feature is the output of a layer's last block, and the block after it opens one of layers 2-4: stride 2,
+        # so it has a downsample
+        assert d_skip is None, "skip-connection gradient at a block without downsample"
         d_sc = dres
-        if extra_addend is not None:
-            d_sc = d_sc + extra_addend          # not reached by ResNet-18/50 (skips feed downsample blocks)
-    dz, z, y, s, conv, bn, st, pd = first
-    dx, _ = _conv_bn_bwd(cx, dz, z, y, s, x, conv, bn, st, pd, True, False, True, d_sc, G, plan)
+    dx, _ = _conv_bn_bwd(cx, d, main[0], recs[0], True, False, d_sc, groups, plan)
     return dx
 
 
-def encoder_forward(cx, enc, imgs, training, G=1):
-    """imgs: tuple of one (DispResNet) or two (PoseResNet, channel-concatenated) NCHW image batches."""
+def _stem_operands(cx, conv, imgs):
+    """(x_nhwc, w, w_lo) of the 7x7 stem: imgs as in encoder_forward.  On the tensor cores the input channels are
+    zero-padded 3 -> 4 / 6 -> 8 (K = 49 * Cpad) and the weights likewise; in fp32 mode the plain NHWC input and the
+    unit's own weights."""
+    if not cx.tc:
+        return O.nchw_to_nhwc(imgs[0], imgs[1] if len(imgs) > 1 else None), conv.w_op(cx), conv.w_lo(cx)
+    cpad = 4 * len(imgs)
+    x_nhwc = O.nchw_to_nhwc_pad(imgs[0], imgs[1] if len(imgs) > 1 else None, cpad, cx.operand)
+    w = O.pad_channels(conv.w_khwc(), cpad, cx.operand)
+    w_lo = O.pad_channels(conv.w_khwc(), cpad, O.OPERAND_LO) if cx.split else None
+    return x_nhwc, w, w_lo
+
+
+def encoder_forward(f, enc, imgs):
+    """imgs: tuple of one (DispResNet) or two (PoseResNet, channel-concatenated) NCHW image batches.
+    Returns (record, or None in the fused forward; the five features)."""
     t = enc.encoder
-    rec = {"G": G}
-    if training:
-        _pool(cx).begin(imgs[0].device)
+    G = f.groups
+    if f.training:
+        _pool(f.cx).begin(imgs[0].device)
         nbt = getattr(enc, "_nbt", None)
         if nbt is not None:
             nbt.add_(G)                      # every BatchNorm layer's num_batches_tracked (views of this tensor)
@@ -532,84 +589,24 @@ def encoder_forward(cx, enc, imgs, training, G=1):
             for m in enc.modules():
                 if isinstance(m, BNParams):
                     m.num_batches_tracked += G
-    if cx.tc:
-        # 7x7 stem on the tensor cores: input channels zero-padded 3 -> 4 / 6 -> 8 (K = 49 * Cpad), weights likewise
-        cpad = 4 * len(imgs)
-        x_nhwc = O.nchw_to_nhwc_pad(imgs[0], imgs[1] if len(imgs) > 1 else None, cpad, cx.operand)
-        w0 = O.pad_channels(t.conv1.w_khwc(), cpad, cx.operand)
-        w0_lo = O.pad_channels(t.conv1.w_khwc(), cpad, O.OPERAND_LO) if cx.split else None
-        C = w0.shape[0]
-        sums = _pool(cx).take(O.BN_SLOTS * G * C * 2, x_nhwc.device) if training else None
-        rec["y0"] = cx.conv_fwd(x_nhwc, w0, None, 2, 3, O.PAD_ZERO, O.ACT_NONE, sums, G, w0_lo)
-        f0, rec["s0"] = _bn_fwd(cx, rec["y0"], sums, t.bn1, training, True, None, G)
-    else:
-        x_nhwc = O.nchw_to_nhwc(imgs[0], imgs[1] if len(imgs) > 1 else None)
-        rec["y0"], f0, rec["s0"] = _conv_bn(cx, x_nhwc, t.conv1, t.bn1, 2, 3, training, True, None, G)
-    rec["x"] = x_nhwc
-    rec["f0"] = f0
-    pooled, rec["pool_idx"] = O.maxpool_fwd(f0)
-    feats, blocks, x = [f0], [], pooled
+    x_nhwc, w0, w0_lo = _stem_operands(f.cx, t.conv1, imgs)
+    f0, stem = _conv_bn(f, x_nhwc, (t.conv1, t.bn1, 2, 3), True, w=(w0, w0_lo))
+    del x_nhwc, w0, w0_lo              # dead in the fused forward (the record keeps the stem's input for the backward)
+    x, pool_idx = O.maxpool_fwd(f0)
+    feats, blocks = [f0], []
     for li in range(1, 5):
         for blk in getattr(t, "layer%d" % li):
-            r, x = block_forward(cx, blk, x, training, G)
+            x, r = block_forward(f, blk, x)
             blocks.append((blk, r))
         feats.append(x)
-    rec["blocks"], rec["feats"] = blocks, feats
-    return rec, feats
-
-
-def _conv_bn_eval(cx, x, conv, bn, coeffs, stride, pad, relu, residual=None, with_lo=False):
-    """relu?(bn(conv(x)) [+ residual]) in eval mode as ONE convolution: BatchNorm, residual, ReLU and TF32 rounding in its
-    epilogue (bitwise conv_fwd followed by bn_apply).  with_lo: the output feeds a tensor-core convolution (tf32x3: write its
-    low part too)."""
-    sc, sh = coeffs[id(bn)]
-    return cx.conv_fwd(x, conv.w_op(cx), None, stride, pad, O.PAD_ZERO, (O.ACT_RELU if relu else O.ACT_NONE) | cx.rnd(), None, 1,
-                       conv.w_lo(cx), bn_scale=sc, bn_shift=sh, addend=residual, with_lo=with_lo and cx.split)
-
-
-def block_forward_eval(cx, blk, x, coeffs):
-    if blk.bottleneck:
-        h1 = _conv_bn_eval(cx, x, blk.conv1, blk.bn1, coeffs, 1, 0, True, None, True)
-        h2 = _conv_bn_eval(cx, h1, blk.conv2, blk.bn2, coeffs, blk.stride, 1, True, None, True)
-        del h1
-        last_in, last_conv, last_bn, ls, lp = h2, blk.conv3, blk.bn3, 1, 0
-    else:
-        h1 = _conv_bn_eval(cx, x, blk.conv1, blk.bn1, coeffs, blk.stride, 1, True, None, True)
-        last_in, last_conv, last_bn, ls, lp = h1, blk.conv2, blk.bn2, 1, 1
-    sc = x
-    if blk.downsample is not None:
-        sc = _conv_bn_eval(cx, x, blk.downsample[0], blk.downsample[1], coeffs, blk.stride, 0, False)
-    return _conv_bn_eval(cx, last_in, last_conv, last_bn, coeffs, ls, lp, True, sc, True)
-
-
-def encoder_forward_eval(cx, enc, imgs, coeffs):
-    """encoder_forward's eval-mode features without the record: imgs as there, coeffs from ArenaNet.bn_eval_coeffs()."""
-    t = enc.encoder
-    if cx.tc:
-        cpad = 4 * len(imgs)
-        x_nhwc = O.nchw_to_nhwc_pad(imgs[0], imgs[1] if len(imgs) > 1 else None, cpad, cx.operand)
-        w0 = O.pad_channels(t.conv1.w_khwc(), cpad, cx.operand)
-        w0_lo = O.pad_channels(t.conv1.w_khwc(), cpad, O.OPERAND_LO) if cx.split else None
-        sc, sh = coeffs[id(t.bn1)]
-        f0 = cx.conv_fwd(x_nhwc, w0, None, 2, 3, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, w0_lo, bn_scale=sc, bn_shift=sh)
-    else:
-        x_nhwc = O.nchw_to_nhwc(imgs[0], imgs[1] if len(imgs) > 1 else None)
-        f0 = _conv_bn_eval(cx, x_nhwc, t.conv1, t.bn1, coeffs, 2, 3, True)
-    del x_nhwc
-    x, _ = O.maxpool_fwd(f0)
-    feats = [f0]
-    for li in range(1, 5):
-        for blk in getattr(t, "layer%d" % li):
-            x = block_forward_eval(cx, blk, x, coeffs)
-        feats.append(x)
-    return feats
+    return None if f.fused else {"G": G, "stem": stem, "pool_idx": pool_idx, "blocks": blocks}, feats
 
 
 def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
     """d_feats[i]: gradient w.r.t. feature i coming from the decoder (None if unused).  d_feats[4] is required.
     Returns the gradients of the input images (NCHW, one per image of the forward; None where plan.dimg does not ask)."""
     t = enc.encoder
-    blocks = rec["blocks"]
+    blocks, G = rec["blocks"], rec["G"]
     # index of the last block of each layer -> the feature it produces
     ends, k = {}, 0
     for li in range(1, 5):
@@ -622,29 +619,27 @@ def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
         extra = None
         if bi - 1 in ends and d_feats[ends[bi - 1]] is not None:
             extra = d_feats[ends[bi - 1]]
-        d = block_backward(cx, blk, r, d, extra, plan)
+        d = block_backward(cx, blk, r, d, extra, G, plan)
     # d is now the gradient w.r.t. the max-pool output
-    f0 = rec["f0"]
+    stem = rec["stem"]
+    f0, x = stem.z, stem.x
     if d_feats[0] is not None:
         d_f0 = d_feats[0]
         O.maxpool_bwd(d, rec["pool_idx"], f0.shape, d_f0, True)
     else:
         d_f0 = torch.empty_like(f0)
         O.maxpool_bwd(d, rec["pool_idx"], f0.shape, d_f0, False)
-    x = rec["x"]
-    relu = 1 | cx.rnd() | plan.bn
-    if x.shape[-1] != t.conv1.weight.shape[1]:
-        # padded-channel stem (tensor-core modes): weight gradient in the padded layout, then folded into the gradient arena
-        # (the low part of dy is only read by that weight gradient)
-        dy, _ = O.bn_backward(d_f0, f0, rec["y0"], rec["s0"], *_bn_param_grads(t.bn1, plan), relu, False, rec["G"], cx.split and plan.params)
-        if plan.params:
+    # the low part of dy is read only by the tensor-core weight gradient (the plain stem runs in fp32 mode, without one)
+    dy, _ = O.bn_backward(d_f0, f0, stem.y, stem.saved, *_bn_param_grads(t.bn1, plan), 1 | cx.rnd() | plan.bn, False, G,
+                          cx.split and plan.params)
+    if plan.params:
+        if x.shape[-1] != t.conv1.weight.shape[1]:
+            # padded-channel stem (tensor-core modes): weight gradient in the padded layout, then folded into the gradient arena
             dw = torch.zeros(t.conv1.weight.shape[0], t.conv1.k, t.conv1.k, x.shape[-1], device=x.device, dtype=torch.float32)
             cx.conv_wgrad(x, dy, dw, None, 2, 3, O.PAD_ZERO)
             with cx.on_wgrad_stream([dw]):
                 O.unpad_add_(ArenaNet.g(t.conv1.weight), dw)
-    else:
-        dy, _ = O.bn_backward(d_f0, f0, rec["y0"], rec["s0"], *_bn_param_grads(t.bn1, plan), relu, False, rec["G"], cx.split)
-        if plan.params:
+        else:
             cx.conv_wgrad(x, dy, ArenaNet.g(t.conv1.weight), None, 2, 3, O.PAD_ZERO)
     if not any(plan.dimg):
         return [None] * len(plan.dimg)
@@ -667,12 +662,7 @@ class DispResNet(ArenaNet):
         pass
 
     def forward(self, x):
-        self.ensure_arena()
-        if self._fused_eval():
-            return self._forward_impl(1, x, fused=True)[1][0]
-        if torch.is_grad_enabled():
-            self._pending += 1
-        outs = _NetCall.apply(self, self._hook, 1, x)
+        outs = self._call((x,))
         return list(outs) if self.training else outs[0]
 
     def forward_multi(self, images):
@@ -680,15 +670,7 @@ class DispResNet(ArenaNet):
         returns one output per image, each exactly what `self(image)` would return.  The calls are stacked on
         the batch axis (more rows per GEMM, 1/len(images) of the kernel launches) while BatchNorm statistics
         and running-stat updates stay per call, in list order (train.py:427-434 semantics)."""
-        self.ensure_arena()
-        if torch.is_grad_enabled():
-            self._pending += 1
-        G, B = len(images), images[0].shape[0]
-        if self._fused_eval():
-            out = self._forward_impl(G, torch.cat(list(images), 0), fused=True)[1][0]
-            return [out[g * B:(g + 1) * B] for g in range(G)]
-        outs = _NetCall.apply(self, self._hook, G, torch.cat(list(images), 0))
-        per = [[o[g * B:(g + 1) * B] for o in outs] for g in range(G)]
+        per = self._call((torch.cat(list(images), 0),), len(images))
         return per if self.training else [p[0] for p in per]
 
     # -- forward ------------------------------------------------------------------------------
@@ -699,10 +681,7 @@ class DispResNet(ArenaNet):
         self.refresh_operand_weights()
         training = self.training
         cx = self.ctx
-        if fused:
-            enc_rec, feats = None, encoder_forward_eval(cx, self.encoder, (x,), self.bn_eval_coeffs())
-        else:
-            enc_rec, feats = encoder_forward(cx, self.encoder, (x,), training, groups)
+        enc_rec, feats = encoder_forward(_Forward(self, groups, fused), self.encoder, (x,))
         dec = self.decoder
         rec = {"enc": enc_rec, "stages": {}, "training": training}
         cur = feats[4]
@@ -794,25 +773,13 @@ class PoseResNet(ArenaNet):
         pass
 
     def forward(self, img1, img2):
-        self.ensure_arena()
-        if self._fused_eval():
-            return self._forward_impl(1, img1, img2, fused=True)[1][0]
-        if torch.is_grad_enabled():
-            self._pending += 1
-        return _NetCall.apply(self, self._hook, 1, img1, img2)[0]
+        return self._call((img1, img2))[0]
 
     def forward_multi(self, pairs):
         """`pairs` = list of (img1, img2); one stacked launch sequence, BatchNorm per call (see DispResNet.forward_multi).
         Returns the list of [B,6] poses."""
-        self.ensure_arena()
-        if torch.is_grad_enabled():
-            self._pending += 1
-        G, B = len(pairs), pairs[0][0].shape[0]
-        if self._fused_eval():
-            out = self._forward_impl(G, torch.cat([a for a, _ in pairs], 0), torch.cat([b for _, b in pairs], 0), fused=True)[1][0]
-            return [out[g * B:(g + 1) * B] for g in range(G)]
-        out = _NetCall.apply(self, self._hook, G, torch.cat([a for a, _ in pairs], 0), torch.cat([b for _, b in pairs], 0))[0]
-        return [out[g * B:(g + 1) * B] for g in range(G)]
+        per = self._call((torch.cat([a for a, _ in pairs], 0), torch.cat([b for _, b in pairs], 0)), len(pairs))
+        return [p[0] for p in per]
 
     def _forward_impl(self, groups, img1, img2, fused=False):
         """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs)."""
@@ -820,39 +787,33 @@ class PoseResNet(ArenaNet):
         img1, img2 = L.dev_f32(img1, "PoseResNet input"), L.dev_f32(img2, "PoseResNet input")
         self.refresh_operand_weights()
         cx = self.ctx
-        n = self.decoder.net
-        if fused:
-            f4 = encoder_forward_eval(cx, self.encoder, (img1, img2), self.bn_eval_coeffs())[4]
-            lo = cx.split
-            s = cx.conv_fwd(f4, n[0].w_op(cx), n[0].bias, 1, 0, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[0].w_lo(cx), with_lo=lo)
-            del f4
-            p0 = cx.conv_fwd(s, n[1].w_op(cx), n[1].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[1].w_lo(cx), with_lo=lo)
-            del s
-            p1 = cx.conv_fwd(p0, n[2].w_op(cx), n[2].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[2].w_lo(cx))
-            del p0
-            p2 = cx.conv_fwd(p1, n[3].w_op(cx), n[3].bias, 1, 0, O.PAD_ZERO, O.ACT_NONE, None, 1, n[3].w_lo(cx))
-            return None, [O.spatial_mean_fwd(p2, 0.01)]
-        enc_rec, feats = encoder_forward(cx, self.encoder, (img1, img2), self.training, groups)
-        rec = {"enc": enc_rec, "f4": feats[4], "training": self.training}
-        rec["s"] = cx.conv_fwd(feats[4], n[0].w_op(cx), n[0].bias, 1, 0, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[0].w_lo(cx))
-        rec["p0"] = cx.conv_fwd(rec["s"], n[1].w_op(cx), n[1].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[1].w_lo(cx))
-        rec["p1"] = cx.conv_fwd(rec["p0"], n[2].w_op(cx), n[2].bias, 1, 1, O.PAD_ZERO, O.ACT_RELU | cx.rnd(), None, 1, n[2].w_lo(cx))
-        rec["p2"] = cx.conv_fwd(rec["p1"], n[3].w_op(cx), n[3].bias, 1, 0, O.PAD_ZERO, O.ACT_NONE, None, 1, n[3].w_lo(cx))
-        return rec, [O.spatial_mean_fwd(rec["p2"], 0.01)]
+        enc_rec, feats = encoder_forward(_Forward(self, groups, fused), self.encoder, (img1, img2))
+        x = feats[4]
+        del feats                       # the fused forward frees f0-f3 here
+        head = None if fused else [x]   # recording: the input of every head convolution, then the head's output
+        for k, (pad, _) in enumerate(POSE_HEAD):
+            conv = self.decoder.net[k]
+            # (fused, tf32x3: the inputs of the two 3x3 convolutions are written with their low part; the last convolution,
+            # 256 -> 6 channels, runs on the CUDA cores and reads none)
+            x = cx.conv_fwd(x, conv.w_op(cx), conv.bias, 1, pad, O.PAD_ZERO, _pose_act(cx, k), None, 1, conv.w_lo(cx),
+                            with_lo=fused and cx.split and k < 2)
+            if head is not None:
+                head.append(x)
+        rec = None if fused else {"enc": enc_rec, "head": head, "training": self.training}
+        return rec, [O.spatial_mean_fwd(x, 0.01)]
 
     def _backward_impl(self, rec, grads, plan=TRAIN_PLAN):
         """Returns [gradient of img1 or None, gradient of img2 or None] (see encoder_backward)."""
-        n = self.decoder.net
-        g = ArenaNet.g
         cx = self.ctx
-        d = O.spatial_mean_bwd(grads[0], rec["p2"].shape, 0.01)
-        chain = [(n[3], rec["p1"], 0), (n[2], rec["p0"], 1), (n[1], rec["s"], 1), (n[0], rec["f4"], 0)]
-        for k, (conv, inp, pad) in enumerate(chain):
+        head = rec["head"]
+        d = O.spatial_mean_bwd(grads[0], head[-1].shape, 0.01)
+        for k in range(len(POSE_HEAD) - 1, -1, -1):
+            conv, pad, inp = self.decoder.net[k], POSE_HEAD[k][0], head[k]
             if plan.params:
-                cx.conv_wgrad(inp, d, g(conv.weight), conv.bias.grad, 1, pad, O.PAD_ZERO)
+                cx.conv_wgrad(inp, d, ArenaNet.g(conv.weight), conv.bias.grad, 1, pad, O.PAD_ZERO)
             d = cx.conv_dgrad(d, conv.w_op(cx), inp.shape, 1, pad)
-            if k < 3:
-                O.act_bwd_(d, inp, O.ACT_RELU | cx.rnd())       # inp is the ReLU output of the previous conv
+            if k > 0:
+                O.act_bwd_(d, inp, _pose_act(cx, k - 1))       # inp is the output of convolution k - 1
         return encoder_backward(cx, self.encoder, rec["enc"], [None, None, None, None, d], plan)
 
 

@@ -112,6 +112,12 @@ def empty(shape, like):
     return torch.empty(shape, device=like.device, dtype=torch.float32)
 
 
+def aligned64(n):
+    """n rounded up to a multiple of 64 elements: slices of a packed fp32 buffer at such offsets start on a 256-byte
+    boundary (float4 loads)."""
+    return (n + 63) // 64 * 64
+
+
 def tc_supported(kind, Cin, Cout, kh, stride):
     """Shapes the tensor-core kernels take; everything else runs the CUDA-core kernel."""
     if kind == "fwd":
@@ -463,14 +469,14 @@ class BnEvalTable:
     def __init__(self, bns, eps):
         import struct
         dev = bns[0].weight.device
-        total = sum(2 * _aligned64(bn.weight.numel()) for bn in bns)
+        total = sum(2 * aligned64(bn.weight.numel()) for bn in bns)
         self.buf = torch.empty(total, device=dev, dtype=torch.float32)
         eps_bits = struct.unpack("<i", struct.pack("<f", eps))[0]
         rows, self.coeffs, off = [], [], 0
         for bn in bns:
             C = bn.weight.numel()
-            sc, sh = self.buf[off:off + C], self.buf[off + _aligned64(C):off + _aligned64(C) + C]
-            off += 2 * _aligned64(C)
+            sc, sh = self.buf[off:off + C], self.buf[off + aligned64(C):off + aligned64(C) + C]
+            off += 2 * aligned64(C)
             self.coeffs.append((sc, sh))
             rows.append([bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
                          sc.data_ptr(), sh.data_ptr(), C, eps_bits])
@@ -486,10 +492,6 @@ class BnEvalTable:
         """(Re)compute every layer's scale / shift from the current parameters and running statistics: one launch."""
         L.launch(_lib().scsfm_bn_eval_prepare_batched, "scsfm_bn_eval_prepare_batched", "bn_prepare", 1, self.bytes,
                  L.ptr(self.table), self.n, L.stream())
-
-
-def _aligned64(n):
-    return (n + 63) // 64 * 64
 
 
 def bn_backward(dz, z, y, saved, dgamma, dbeta, relu, want_dres, groups=1, with_lo=False):
