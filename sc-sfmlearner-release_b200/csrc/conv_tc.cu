@@ -621,14 +621,24 @@ static int tc_dispatch_gather(const ScsfmConv& p, const TcView& v, cudaStream_t 
     return launch_fwd_tc<128>(p, v, st);
 }
 
+// Stride-2 forwards the gather kernel runs faster than the TMA kernel (tools/conv_layers.py --only s2 --tune mt=1
+// --compare no_tma=1, H100): in split mode, Cin >= 512 into output planes of at most 8 x 26 pixels (the ResNet-50 layer4
+// 3x3 512 -> 512 and 1x1 1024 -> 2048).  Two 128-pixel tiles per image leave most SMs idle through a long K loop, where
+// the gather kernel's 64-pixel tiles give twice the CTAs.  The ResNet-18 layer4 (Cin 256) and every tf32 shape are at
+// least as fast on the TMA kernel.
+static bool s2_prefers_gather(const ScsfmConv& p, const TcView& v) {
+    return v.in_stride == 2 && p.in_lo != nullptr && p.Cin >= 512 && p.Ho * p.Wo <= 8 * 26 && !conv_tma_forced(p);
+}
+
 static int tc_dispatch(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
-    if (p.pad_mode == PADMODE_ZERO && conv_tma_eligible(p, v)) return launch_conv_tma(p, v, st);
-    if (p.pad_mode == PADMODE_REFLECT && p.bn_sums == nullptr && p.Ho >= 3 && p.Wo >= 3 &&
+    if (p.pad_mode == PADMODE_ZERO && conv_tma_eligible(p, v) && !s2_prefers_gather(p, v)) return launch_conv_tma(p, v, st);
+    if (p.pad_mode == PADMODE_REFLECT && v.in_stride == 1 && p.bn_sums == nullptr && p.Ho >= 3 && p.Wo >= 3 &&
         (p.Ho * p.Wo >= 64 * 208 || conv_tma_forced(p)) && conv_tma_eligible(p, v)) {
         // reflection padding only changes the outermost ring of output pixels: run the TMA kernel with zero padding
         // (interior exact), then recompute the 2*(Ho+Wo)-4 border pixels per image with the reflecting gather kernel.
-        // Measured (tools/check_conv_tma.py): pays off from 64x208 upwards; below that the ring is too large a share
-        // of the image and the gather kernel alone is faster.
+        // Measured on H100 (tools/conv_layers.py --only dec --compare mt=1, tf32x3): pays off from 64x208 upwards; below
+        // that the ring is too large a share of the image and the gather kernel alone is as fast or faster (8x26:
+        // x0.63, 16x52: x0.95; at 32x104 the split was x1.14, not yet taken: tf32 unmeasured).
         ScsfmConv q = p;
         q.pad_mode = PADMODE_ZERO;
         if (int rc = launch_conv_tma(q, v, st)) return rc;

@@ -72,7 +72,8 @@ CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, cuuint32_t ra
                       const cuuint64_t* gstride, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapInterleave il,
                       CUtensorMapSwizzle sw, CUtensorMapL2promotion l2, CUtensorMapFloatOOBfill oob);
 
-// conv_tma.cu: stride-1 zero-padded (sub-)convolutions with kh, kw <= 3 through the TMA halo-patch kernel
+// conv_tma.cu: zero-padded stride-1 (sub-)convolutions and stride-2 convolutions with kh, kw <= 3 through the TMA
+// halo-patch kernel (stride 2: parity views of the input)
 bool conv_tma_eligible(const ScsfmConv& p, const TcView& v);
 bool conv_tma_forced(const ScsfmConv& p);      // a tile configuration is being forced through ScsfmConv.tune (tests / experiments)
 int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st);

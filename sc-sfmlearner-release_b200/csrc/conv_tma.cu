@@ -1,5 +1,5 @@
-// Stride-1 convolution on the tensor cores: persistent CTAs, TMA halo-patch producer, two consumer warpgroups
-// (wgmma, tf32 operands, fp32 accumulation in registers).
+// Stride-1 and stride-2 convolution on the tensor cores: persistent CTAs, TMA halo-patch producer, two consumer
+// warpgroups (wgmma, tf32 operands, fp32 accumulation in registers).
 //
 //   D[pixels (M = 64 per wgmma), Cout tile (N = BNW)] = im2col(x)[pixels, K] x W[Cout, K]^T
 //
@@ -11,6 +11,10 @@
 //    shifted by dy*TW rows = dy*TW*128 bytes (a multiple of the 1024-byte swizzle atom): the kh vertical taps reuse one
 //    load.  Zero padding is the TMA's out-of-bounds fill; channels beyond Cin in the last 32-wide chunk are zero-filled
 //    the same way (the matching weight columns then multiply zeros) and all-zero K8 slices are not issued at all;
+//  * stride 2: the input is read through (row parity, column parity) views (row and column strides doubled, base on
+//    the even or odd row / column), where a tap is again a plain shift.  Taps of the same row parity share one box
+//    (3x3 pad 1: dy = 0 and 2 the odd rows, MT*TH + 1 of them; dy = 1 the MT*TH even rows), so a stage is one
+//    (channel chunk, dx, row parity) box with its taps' weights, sized for the larger box (TmaGeom);
 //  * one CTA per SM walks the (tile, Cout tile) work list; the shared-memory stage ring and the mbarrier phases run
 //    across tiles, so the producer prefetches the next tile's patches while the current one is multiplied and stored;
 //  * the accumulator comes out pixel-major (a thread holds 2 consecutive channels of a pixel per fragment), so the
@@ -18,19 +22,25 @@
 //    rounding / low part / BatchNorm sums.
 //
 //   warps 0-7   two consumer warpgroups; warpgroup g owns the pixels [64 MT g, 64 MT (g + 1)) of the tile
-//   warp 8      lane 0: TMA producer (1 activation box + kh weight boxes per stage, mbarrier expect_tx)
+//   warp 8      lane 0: TMA producer (1 activation box + its taps' weight boxes per stage, mbarrier expect_tx); warps
+//               9-11 only complete the producer warpgroup, whose registers setmaxnreg hands to the consumers
 //
-// Used for: forward of every stride-1 layer with kh, kw <= 3 (reflection-padded layers run it with zero padding and
-// the cp.async kernel then recomputes the 2*(H+W)-4 border pixels per image, see tc_dispatch in conv_tc.cu), stride-1
-// data gradients, and the four parity-class sub-convolutions of stride-2 data gradients.
+// Used for: forward of every stride-1 layer and of the zero-padded stride-2 layers with kh, kw <= 3 (s2_prefers_gather in
+// conv_tc.cu keeps the shapes measured faster on the gather kernel there; reflection-padded stride-1 layers run it with zero padding and the cp.async kernel then recomputes the 2*(H+W)-4 border pixels per
+// image, see tc_dispatch in conv_tc.cu), stride-1 data gradients, and the four parity-class sub-convolutions of
+// stride-2 data gradients.
 #include <stdlib.h>
+#include <string.h>
 
 #include "conv_tc.cuh"
 
 namespace scsfm {
 
 constexpr int TMA_CWARPS = 8;
-constexpr int TMA_THREADS = (TMA_CWARPS + 1) * 32;
+// a whole producer warpgroup (warp 8 issues, 9-11 idle): registers are handed out per warpgroup, so with 9 warps the
+// consumers would get 65536 / 384 = 168 each anyway; setmaxnreg moves the producer group's share to the consumers
+constexpr int TMA_THREADS = (TMA_CWARPS + 4) * 32;
+constexpr int TMA_PRODUCER_REGS = 40, TMA_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int TMA_MAX_KH = 3;
 constexpr int TMA_MAX_STAGES = 8;
 constexpr int TMA_SMEM_MAX = 232448;                         // 227 KB: the most one CTA may opt into on sm_90
@@ -41,6 +51,15 @@ struct TmaGeom {
     int n_tiles, num_work;   // Cout tiles; work items = B * tiles_y * tiles_x * n_tiles (Cout tile fastest)
     int stages;              // shared-memory ring depth
     int a_bytes, stage_bytes;
+    // Activation boxes: one stage = one (channel chunk, dx, box).  Box i reads the row-parity view box_py[i] (stride 1:
+    // the input itself) from view row y0 + box_y[i], box_rows[i] rows, and serves the kernel rows tap_dy[box_tap0[i] + j]
+    // (j < box_ntap[i]), tap j shifted by tap_shift[...] * TW pixels; stage weight slot j holds that tap.  Column tap dx
+    // reads the column-parity view col_px[dx] from view column x0 + col_x[dx].  Stride 1: one box of MT*TH + kh - 1
+    // rows; stride 2 (3x3 pad 1): the odd rows (dy = 0, 2: MT*TH + 1 rows) and the even rows (dy = 1: MT*TH rows).
+    int nbox;
+    int box_py[2], box_y[2], box_rows[2], box_tap0[2], box_ntap[2];
+    int tap_dy[TMA_MAX_KH], tap_shift[TMA_MAX_KH];
+    int col_px[TMA_MAX_KH], col_x[TMA_MAX_KH];
     // split-accumulate passes per (channel chunk, dx): pass i multiplies (activations: lo if a_lo bit i else raw) by
     // (weights: lo if w_lo bit i else raw); plain TF32 = one pass with both masks 0
     int npass, a_lo, w_lo;
@@ -51,12 +70,17 @@ struct TmaGeom {
     unsigned long long* dbg; // optional per-CTA cycle counters (ScsfmConv.debug), 8 per CTA; NULL = off
 };
 
+// a[py * 2 + px]: the activations seen through the (row parity py, column parity px) view (stride 2; stride 1 uses a[0]
+// only), a_lo the same for the low part; w, w_lo the weight matrix [Cout][K]
+struct TmaMaps {
+    CUtensorMap a[4], a_lo[4], w, w_lo;
+};
+
 // BNW: Cout tile = weight rows kept in shared memory = N of the wgmma (16/32/64/128).
 // MT: 128-pixel sub-tiles stacked vertically; each consumer warpgroup runs MT wgmma of M = 64 per K8 slice.
 template <int BNW, int MT>
 __global__ void __launch_bounds__(TMA_THREADS, 1)
-conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap wmap,
-                const __grid_constant__ CUtensorMap amap_lo, const __grid_constant__ CUtensorMap wmap_lo) {
+conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMaps maps) {
     constexpr int W_TILE = BNW * 128;                        // one tap: BNW rows x 32 floats
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -68,7 +92,6 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
     const int TW = 1 << g.tw_log2, TH = TBM >> g.tw_log2;
     const int N = p.Cout;
     const int chunks = (p.Cin + TBK - 1) / TBK;
-    const int patch_rows = MT * TH + v.kh - 1;
 
     if (tid == 0) {
         for (int s = 0; s < g.stages; ++s) {
@@ -80,14 +103,18 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
     __syncthreads();
     const uint32_t ring_base = tc::smem_u32(ring);
 
-    if (warp == TMA_CWARPS) {
+    if (warp >= TMA_CWARPS) {
         // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
-            tc::tma_prefetch_desc(&amap);
-            tc::tma_prefetch_desc(&wmap);
-            if (g.a_lo) tc::tma_prefetch_desc(&amap_lo);
-            if (g.w_lo) tc::tma_prefetch_desc(&wmap_lo);
-            const uint32_t tx_bytes = (uint32_t)(patch_rows * TW * 128 + v.kh * W_TILE);
+        tc::setmaxnreg_dec<TMA_PRODUCER_REGS>();
+        if (warp == TMA_CWARPS && lane == 0) {
+            for (int i = 0; i < g.nbox; ++i)
+                for (int dx = 0; dx < v.kw; ++dx) {
+                    const int mi = g.box_py[i] * 2 + g.col_px[dx];
+                    tc::tma_prefetch_desc(&maps.a[mi]);
+                    if (g.a_lo) tc::tma_prefetch_desc(&maps.a_lo[mi]);
+                }
+            tc::tma_prefetch_desc(&maps.w);
+            if (g.w_lo) tc::tma_prefetch_desc(&maps.w_lo);
             int s = 0;
             uint32_t ph = 0;
             long long t_wait = 0;
@@ -98,26 +125,32 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
                 const int tx = t % g.tiles_x; t /= g.tiles_x;
                 const int ty = t % g.tiles_y;
                 const int b = t / g.tiles_y;
-                const int y0 = ty * (MT * TH) + v.oy0, x0 = tx * TW + v.ox0;
+                const int y0 = ty * (MT * TH), x0 = tx * TW;
                 // one accumulation chain = cpg channel chunks; inside a chain the low-part passes run FIRST (their sums are
                 // 2^-11 of the main term: added while the accumulator is still small they lose nothing to its truncation),
                 // the raw x raw pass last
                 for (int ck0 = 0; ck0 < chunks; ck0 += g.cpg)
                 for (int q = 0; q < g.npass; ++q) {
                     const int ps = (q + 1) % g.npass;
-                    const CUtensorMap* am = ((g.a_lo >> ps) & 1) ? &amap_lo : &amap;
-                    const CUtensorMap* wm = ((g.w_lo >> ps) & 1) ? &wmap_lo : &wmap;
+                    const CUtensorMap* am = ((g.a_lo >> ps) & 1) ? maps.a_lo : maps.a;
+                    const CUtensorMap* wm = ((g.w_lo >> ps) & 1) ? &maps.w_lo : &maps.w;
                     for (int ck = ck0; ck < min(chunks, ck0 + g.cpg); ++ck) {
                         for (int dx = 0; dx < v.kw; ++dx) {
-                            const long long t0 = g.dbg ? clock64() : 0;
-                            tc::mbar_wait(bar_empty + s, ph ^ 1);
-                            if (g.dbg) t_wait += clock64() - t0;
-                            const uint32_t st = ring_base + (uint32_t)(s * g.stage_bytes);
-                            tc::mbar_arrive_expect_tx(bar_full + s, tx_bytes);
-                            tc::tma_load_4d(st, am, ck * TBK, x0 + dx, y0, b, bar_full + s);
-                            for (int dy = 0; dy < v.kh; ++dy)
-                                tc::tma_load_2d(st + (uint32_t)(g.a_bytes + dy * W_TILE), wm, (dy * v.kw + dx) * p.Cin + ck * TBK, n0, bar_full + s);
-                            if (++s == g.stages) { s = 0; ph ^= 1; }
+                            for (int bx = 0; bx < g.nbox; ++bx) {
+                                const long long t0 = g.dbg ? clock64() : 0;
+                                tc::mbar_wait(bar_empty + s, ph ^ 1);
+                                if (g.dbg) t_wait += clock64() - t0;
+                                const uint32_t st = ring_base + (uint32_t)(s * g.stage_bytes);
+                                const int nt = g.box_ntap[bx];
+                                tc::mbar_arrive_expect_tx(bar_full + s, (uint32_t)(g.box_rows[bx] * TW * 128 + nt * W_TILE));
+                                tc::tma_load_4d(st, am + g.box_py[bx] * 2 + g.col_px[dx], ck * TBK, x0 + g.col_x[dx], y0 + g.box_y[bx], b,
+                                                bar_full + s);
+                                for (int j = 0; j < nt; ++j) {
+                                    const int dy = g.tap_dy[g.box_tap0[bx] + j];
+                                    tc::tma_load_2d(st + (uint32_t)(g.a_bytes + j * W_TILE), wm, (dy * v.kw + dx) * p.Cin + ck * TBK, n0, bar_full + s);
+                                }
+                                if (++s == g.stages) { s = 0; ph ^= 1; }
+                            }
                         }
                     }
                 }
@@ -130,6 +163,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
         __syncwarp();
     } else {
         // ------------------------------------------------------------------ consumer warpgroups (warps 0-7)
+        tc::setmaxnreg_inc<TMA_CONSUMER_REGS>();
         const int wg = warp >> 2, t = tid & 127;
         const int fr = 16 * (t >> 5) + ((t & 31) >> 2), fc = 2 * (t & 3);   // fragment row / column of d[0]
         const int groups = p.bn_groups > 0 ? p.bn_groups : 1;
@@ -142,10 +176,10 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
         int s = 0;
         uint32_t ph = 0;
         int pend = -1;
-        int j = 0;
+        int items = 0;                                   // work items of this CTA (debug slot 7)
         long long t_full = 0;
         const long long t_begin = clock64();
-        for (int w = blockIdx.x; w < g.num_work; w += gridDim.x, ++j) {
+        for (int w = blockIdx.x; w < g.num_work; w += gridDim.x, ++items) {
             int tt = w / g.n_tiles;
             const int n0 = (w - tt * g.n_tiles) * BNW;
             const int tx = tt % g.tiles_x; tt /= g.tiles_x;
@@ -162,7 +196,8 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
                     for (int ck = ck0; ck < min(chunks, ck0 + g.cpg); ++ck) {
                         const int rem = p.Cin - ck * TBK;
                         const int k8 = rem >= TBK ? TBK / 8 : (rem + 7) / 8;           // K8 slices holding real channels
-                        for (int dx = 0; dx < v.kw; ++dx) {
+                        for (int dxb = 0; dxb < v.kw * g.nbox; ++dxb) {
+                            const int bx = dxb % g.nbox;
                             const long long t0 = g.dbg ? clock64() : 0;
                             tc::mbar_wait(bar_full + s, ph);
                             if (g.dbg) t_full += clock64() - t0;
@@ -171,12 +206,13 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
 #pragma unroll
                             for (int mb = 0; mb < MT; ++mb) tc::reg_fence(part[mb]);
                             tc::wgmma_fence();
-                            for (int dy = 0; dy < v.kh; ++dy) {
+                            for (int j = 0; j < g.box_ntap[bx]; ++j) {
+                                const int shift = g.tap_shift[g.box_tap0[bx] + j];
                                 for (int q8 = 0; q8 < k8; ++q8) {
-                                    const uint64_t dw = tc::make_desc_sw128(w_addr + (uint32_t)(dy * W_TILE + q8 * 32));
+                                    const uint64_t dw = tc::make_desc_sw128(w_addr + (uint32_t)(j * W_TILE + q8 * 32));
 #pragma unroll
                                     for (int mb = 0; mb < MT; ++mb) {
-                                        const uint32_t a = x_addr + (uint32_t)((dy * TW + 64 * (wg * MT + mb)) * 128 + q8 * 32);
+                                        const uint32_t a = x_addr + (uint32_t)((shift * TW + 64 * (wg * MT + mb)) * 128 + q8 * 32);
                                         tc::wgmma_tf32<BNW>(part[mb], tc::make_desc_sw128(a), dw, first ? 0u : 1u);
                                     }
                                     first = false;
@@ -289,7 +325,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ CUtens
         if (g.dbg && tid == 0) {
             g.dbg[blockIdx.x * 8 + 2] = (unsigned long long)t_full;
             g.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(clock64() - t_begin);
-            g.dbg[blockIdx.x * 8 + 7] = (unsigned long long)j;
+            g.dbg[blockIdx.x * 8 + 7] = (unsigned long long)items;
         }
     }
 }
@@ -304,7 +340,8 @@ static int tune_bn(const ScsfmConv& p) { const int t = (int)((p.tune >> 8) & 15u
 
 bool conv_tma_eligible(const ScsfmConv& p, const TcView& v) {
     if ((p.tune & SCSFM_TUNE_NO_TMA) || v.border) return false;
-    if (v.in_stride != 1 || v.kh > TMA_MAX_KH || v.kw > TMA_MAX_KH || v.kh < 1 || v.kw < 1) return false;
+    if (v.kh > TMA_MAX_KH || v.kw > TMA_MAX_KH || v.kh < 1 || v.kw < 1) return false;
+    if (v.in_stride != 1 && (v.in_stride != 2 || p.Hi < 2 || p.Wi < 2)) return false;   // stride 2: every parity view non-empty
     if ((p.Cin & 3) != 0 || (p.Cout & 3) != 0) return false;      // 16-byte TMA rows / float4 epilogue
     if (p.bn_sums && p.B % (p.bn_groups > 0 ? p.bn_groups : 1) != 0) return false;
     return true;
@@ -333,8 +370,40 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
     g.tiles_y = (p.Ho + MT * TH - 1) / (MT * TH);
     g.n_tiles = (p.Cout + BNW - 1) / BNW;
     g.num_work = g.tiles_x * g.tiles_y * p.B * g.n_tiles;
-    g.a_bytes = ((MT * TH + v.kh - 1) * TW * 128 + 1023) / 1024 * 1024;
-    g.stage_bytes = g.a_bytes + v.kh * BNW * 128;
+    // input row of output row ho and tap dy: S ho + oy0 + dy = S (ho + off) + par, par = (oy0 + dy) mod S; the taps of one
+    // row parity share one box, starting at the smallest off, and lie (off - that) rows further into it
+    const int S = v.in_stride;
+    g.nbox = 0;
+    for (int dy = 0; dy < v.kh; ++dy) {
+        const int par = (v.oy0 + dy) & (S - 1), off = (v.oy0 + dy - par) / S;
+        int i = 0;
+        while (i < g.nbox && g.box_py[i] != par) ++i;
+        if (i == g.nbox) { g.box_py[i] = par; g.box_y[i] = off; g.box_ntap[i] = 0; ++g.nbox; }
+        ++g.box_ntap[i];
+    }
+    for (int i = 0, t = 0; i < g.nbox; ++i) {
+        g.box_tap0[i] = t;
+        int last = g.box_y[i];
+        for (int dy = 0; dy < v.kh; ++dy) {
+            const int par = (v.oy0 + dy) & (S - 1), off = (v.oy0 + dy - par) / S;
+            if (par != g.box_py[i]) continue;
+            g.tap_dy[t] = dy;
+            g.tap_shift[t++] = off - g.box_y[i];
+            last = off;
+        }
+        g.box_rows[i] = MT * TH + last - g.box_y[i];
+    }
+    for (int dx = 0; dx < v.kw; ++dx) {
+        g.col_px[dx] = (v.ox0 + dx) & (S - 1);
+        g.col_x[dx] = (v.ox0 + dx - g.col_px[dx]) / S;
+    }
+    int max_rows = 0, max_taps = 0;
+    for (int i = 0; i < g.nbox; ++i) {
+        max_rows = g.box_rows[i] > max_rows ? g.box_rows[i] : max_rows;
+        max_taps = g.box_ntap[i] > max_taps ? g.box_ntap[i] : max_taps;
+    }
+    g.a_bytes = (max_rows * TW * 128 + 1023) / 1024 * 1024;
+    g.stage_bytes = g.a_bytes + max_taps * BNW * 128;
     const int fixed = 1024 + 1024;                          // 1024 alignment slack + 1024 barrier block
     g.stages = (TMA_SMEM_MAX - fixed) / g.stage_bytes;
     if (g.stages > TMA_MAX_STAGES) g.stages = TMA_MAX_STAGES;
@@ -355,28 +424,36 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
         if (g.cpg < 1) g.cpg = 1;
     }
     const size_t smem = (size_t)fixed + (size_t)g.stages * g.stage_bytes;
-    CUtensorMap amap, wmap, amap_lo, wmap_lo;
+    TmaMaps maps;
+    memset(&maps, 0, sizeof(maps));
     for (int lo = 0; lo < 2; ++lo) {
         const float* base = lo ? p.in_lo : p.in;
-        CUtensorMap& amap_ = lo ? amap_lo : amap;
-        if (base == nullptr) { amap_lo = amap; continue; }
-        // activations [B][Hi][Wi][Cin] (Cin contiguous); box = 32 channels x TW x (MT*TH + kh - 1) x 1, 128B swizzle
-        const cuuint64_t gdim[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Wi, (cuuint64_t)p.Hi, (cuuint64_t)p.B};
-        const cuuint64_t gstride[3] = {(cuuint64_t)p.Cin * 4, (cuuint64_t)p.Wi * p.Cin * 4, (cuuint64_t)p.Hi * p.Wi * p.Cin * 4};
-        const cuuint32_t box[4] = {(cuuint32_t)TBK, (cuuint32_t)TW, (cuuint32_t)(MT * TH + v.kh - 1), 1};
-        const cuuint32_t estr[4] = {1, 1, 1, 1};
-        const CUresult r = encode_tiled(&amap_, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstride, box, estr,
-                                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            set_error("cuTensorMapEncodeTiled(activations %d x %d x %d x %d) failed with CUresult %d", p.B, p.Hi, p.Wi, p.Cin, (int)r);
-            return SCSFM_ERR_CUDA;
-        }
+        if (base == nullptr) continue;
+        for (int i = 0; i < g.nbox; ++i)
+            for (int dx = 0; dx < v.kw; ++dx) {
+                // activations [B][Hi][Wi][Cin] (Cin contiguous), seen through the (py, px) parity view at stride 2: every
+                // S-th row and column from row py, column px; box = 32 channels x TW x box_rows x 1, 128B swizzle
+                const int py = g.box_py[i], px = g.col_px[dx];
+                CUtensorMap& m = (lo ? maps.a_lo : maps.a)[py * 2 + px];
+                const cuuint64_t gdim[4] = {(cuuint64_t)p.Cin, (cuuint64_t)((p.Wi - px + S - 1) / S), (cuuint64_t)((p.Hi - py + S - 1) / S),
+                                            (cuuint64_t)p.B};
+                const cuuint64_t gstride[3] = {(cuuint64_t)S * p.Cin * 4, (cuuint64_t)S * p.Wi * p.Cin * 4, (cuuint64_t)p.Hi * p.Wi * p.Cin * 4};
+                const cuuint32_t box[4] = {(cuuint32_t)TBK, (cuuint32_t)TW, (cuuint32_t)g.box_rows[i], 1};
+                const cuuint32_t estr[4] = {1, 1, 1, 1};
+                const CUresult r = encode_tiled(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base + ((size_t)py * p.Wi + px) * p.Cin),
+                                                gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                if (r != CUDA_SUCCESS) {
+                    set_error("cuTensorMapEncodeTiled(activations %d x %d x %d x %d, view %d/%d) failed with CUresult %d", p.B, p.Hi, p.Wi,
+                              p.Cin, py, px, (int)r);
+                    return SCSFM_ERR_CUDA;
+                }
+            }
     }
     for (int lo = 0; lo < 2; ++lo) {
         const float* base = lo ? p.w_lo : p.w;
-        CUtensorMap& wmap_ = lo ? wmap_lo : wmap;
-        if (base == nullptr) { wmap_lo = wmap; continue; }
+        CUtensorMap& wmap_ = lo ? maps.w_lo : maps.w;
+        if (base == nullptr) continue;
         // weights [Cout][K] (K contiguous); box = 32 columns x BNW rows (rows past Cout are zero-filled)
         const int K = v.kh * v.kw * p.Cin;
         const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)p.Cout};
@@ -393,7 +470,7 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
     }
     int ctas = sm_count();
     if (ctas > g.num_work) ctas = g.num_work;
-    conv_tma_kernel<BNW, MT><<<ctas, TMA_THREADS, smem, st>>>(p, v, g, amap, wmap, amap_lo, wmap_lo);
+    conv_tma_kernel<BNW, MT><<<ctas, TMA_THREADS, smem, st>>>(p, v, g, maps);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
@@ -420,7 +497,8 @@ int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
             const long ty = (p.Ho + th - 1) / th, tx = (p.Wo + tw - 1) / tw;
             const long work = ty * tx * p.B * nt;
             const long waves = (work + nsm - 1) / nsm;
-            const double area = (double)(ty * (th + v.kh - 1)) * (double)(tx * tw) / ((double)p.Ho * p.Wo);     // >= 1
+            const double halo = (double)(v.kh - 1) / v.in_stride;          // extra rows per tile, in output rows
+            const double area = (double)ty * (th + halo) * (double)(tx * tw) / ((double)p.Ho * p.Wo);     // >= 1
             const double cost = (double)waves + 0.05 * area + 0.01 * mt;
             if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_mt = mt; best_tw = twl; }
         }

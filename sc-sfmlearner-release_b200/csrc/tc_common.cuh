@@ -72,6 +72,12 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* tensor_map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tensor_map)) : "memory");
 }
 
+// ----- per-warpgroup register budget (setmaxnreg: every warp of the warpgroup executes it) ---------------------------
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ----- wgmma (sm_90a warpgroup MMA) -----------------------------------------------------------------
 // D[regs] (+)= A[smem] * B[smem], m64 x N x k8, tf32 operands, fp32 accumulation in the registers of the 128 threads of a
 // warpgroup.  Both operands K-major (the only layout wgmma takes for 32-bit types).  Accumulator fragment of thread t:

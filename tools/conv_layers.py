@@ -51,6 +51,12 @@ LAYERS = [
     ("r50 1x1 256->64", 6, 64, 208, 256, 64, 1, 1, 0, 0),
     ("r50 1x1 64->256", 6, 64, 208, 64, 256, 1, 1, 0, 0),
     ("r50 1x1 1024->256", 6, 16, 52, 1024, 256, 1, 1, 0, 0),
+    ("r50 L2 3x3 s2", 6, 64, 208, 128, 128, 3, 2, 1, 0),
+    ("r50 L3 3x3 s2", 6, 32, 104, 256, 256, 3, 2, 1, 0),
+    ("r50 L4 3x3 s2", 6, 16, 52, 512, 512, 3, 2, 1, 0),
+    ("r50 down2 1x1 s2", 6, 64, 208, 256, 512, 1, 2, 0, 0),
+    ("r50 down3 1x1 s2", 6, 32, 104, 512, 1024, 1, 2, 0, 0),
+    ("r50 down4 1x1 s2", 6, 16, 52, 1024, 2048, 1, 2, 0, 0),
     ("odd zero", 2, 37, 45, 20, 24, 3, 1, 1, 0),
     ("odd refl", 3, 19, 21, 36, 40, 3, 1, 1, 1),
     ("odd s2", 2, 37, 45, 24, 20, 3, 2, 1, 0),
