@@ -358,6 +358,30 @@ long long scsfm_augment_workspace_ints(int B, int H, int W);
 int scsfm_augment_batch(const unsigned char* images, const int* params, int n_img, int B, int H, int W, const float* mean3,
                         const float* std3, float* out, int* workspace, long long workspace_ints, void* stream);
 
+/* Training-set preparation (reference data/prepare_train_data.py and its loaders; data/prepare_train_data.py here).
+ *
+ * Resize of B frames of one source size: PIL.Image.fromarray(img).resize((out_w, out_h), Image.BILINEAR) bit for bit (what
+ * scipy.misc.imresize did, kitti_raw_loader.py:224): triangle filter of support max(in / out, 1), Pillow's 22-bit fixed-point
+ * taps, horizontal pass into an 8-bit intermediate, then the vertical pass; a pass whose axis keeps its size is skipped.
+ * in [B][H][W][3] uint8, out [B][out_h][out_w][3] uint8; workspace: scsfm_resize_bilinear_workspace_bytes(...) bytes,
+ * 16-byte aligned.  Downscales of more than 31x per axis are refused. */
+size_t scsfm_resize_bilinear_workspace_bytes(int B, int H, int W, int out_h, int out_w);
+int scsfm_resize_bilinear_u8(const unsigned char* in, int B, int H, int W, int out_h, int out_w, unsigned char* out,
+                             void* workspace, size_t workspace_bytes, void* stream);
+
+/* Velodyne ground-truth depth of B frames (kitti_raw_loader.py:243-300, generate_depth_map, with its quirks).
+ * points: float32 [N][4] (the .bin rows: forward, left, up, reflectance; the 4th column is ignored), frame b's points are rows
+ * offsets[b] .. offsets[b+1]-1 (offsets: int64 [B+1] on the device, and the same values in HOST memory as offsets_host);
+ * P: float64 [B][3][4] P_velo2im per frame; depth: float32 [B][Hd][Wd] (Hd = H / ratio, Wd = W / ratio; Wd >= 2).
+ * For every point with x >= 0: u = P [x y z 1] in fp64 (left to right, no FMA), px = rint(u0/u2) - 1, py = rint(u1/u2) - 1
+ * (half to even), kept if 0 <= px < Wd and 0 <= py < Hd.  Pixel value: float32(u2) of the last point on the pixel; for every
+ * key py * (Wd-1) + px - 1 with >= 2 points (pixels (y, Wd-1) and (y+1, 0) share a key), the pixel of the key's first point
+ * gets float32(min u2) of the key; negative values become 0, pixels without points 0.  Deterministic.  workspace:
+ * scsfm_velo_depth_workspace_bytes(B, Hd, Wd) bytes (16 per pixel), 16-byte aligned. */
+size_t scsfm_velo_depth_workspace_bytes(int B, int Hd, int Wd);
+int scsfm_velo_depth(const float* points, const long long* offsets, const long long* offsets_host, const double* P, int B,
+                     int Hd, int Wd, float* depth, void* workspace, size_t workspace_bytes, void* stream);
+
 /* out[i] = round-to-nearest TF32 of in[i] (weights of the tensor-core convolutions, once per optimizer step) */
 int scsfm_round_tf32(const float* in, float* out, long long n, void* stream);
 /* lo[i] = tf32(in[i] - trunc_tf32(in[i])): the low part of the split-accumulate operands (ScsfmConv.in_lo / w_lo / dout_lo) */
