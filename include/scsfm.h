@@ -197,6 +197,11 @@ typedef struct ScsfmConv {
     /* forward only (NULL = off, 16-byte aligned, Cout % 4 == 0): also write tf32_lo(out) here, the split-accumulate low part a following tf32x3
      * convolution reads as in_lo (what scsfm_split_tf32 of the output would produce) */
     float* out_lo;
+    /* 1: split-accumulate (tf32x3) arithmetic.  With it, in_lo / dout_lo may be NULL where scsfm_conv_reads_lo() says the
+     * kernel chosen for the call computes them from the operands itself (w_lo is still required in the forward); a kernel
+     * that reads a low part which was not passed makes the call fail with SCSFM_ERR_ARG.  0: split mode as implied by the
+     * low parts passed. */
+    int split;
 } ScsfmConv;
 
 /* ScsfmConv.tune */
@@ -216,12 +221,24 @@ int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream);
  * scsfm_weight_flip (the data gradient is the forward kernel run on dout). */
 /* Stride-1 (sub-)convolutions with kh, kw <= 3 run the TMA halo-patch kernel (conv_tma.cu: one 4-D tiled TMA load
  * per (channel chunk, dx) brings the input patch of a 2-D output tile, the kh vertical taps reuse it); reflection-
- * padded layers run it zero-padded and recompute the border ring with the gather kernel.  Other shapes (stride-2
- * forward, 7x7 stems) use the cp.async gather kernel.  wgrad_tc: stride-1 and zero-padded stride-2 layers with
+ * padded layers run it zero-padded and recompute the border ring with the gather kernel; so do the zero-padded stride-2
+ * forwards with kh, kw <= 3, and the 7x7 stems run conv_stem_fwd.cu (below).  Other shapes use the cp.async gather
+ * kernel.  wgrad_tc: stride-1 and zero-padded stride-2 layers with
  * kh, kw <= 3 and the 7x7 stride-2 stems (4 or 8 channels) run the TMA weight-gradient kernel (conv_wgrad_tma.cu). */
 int scsfm_conv2d_fwd_tc(const ScsfmConv* p, void* stream);
 int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream);
 int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream);
+/* The 7x7 stride-2 pad-3 zero-padded stems with Cin = 4 or 8 (padded) and Cout = 64 run a forward
+ * kernel of their own (conv_stem_fwd.cu): a TMA box of the tile's input rows, the im2col operand fed to wgmma from
+ * registers, and lo(in) computed from that operand. */
+/* Whether the kernel scsfm_conv2d_{fwd,dgrad,wgrad}_tc would pick for *p in split mode (tune knobs included) reads the
+ * low parts of its activation operands: in_lo (SCSFM_PASS_FWD), dout_lo (SCSFM_PASS_DGRAD), in_lo and dout_lo
+ * (SCSFM_PASS_WGRAD).  1 yes, 0 no (the kernel computes them itself), SCSFM_ERR_ARG for a bad descriptor or pass.  Only
+ * the geometry, padding mode, epilogue pointers and tune of *p are looked at; nothing is launched. */
+#define SCSFM_PASS_FWD 0
+#define SCSFM_PASS_DGRAD 1
+#define SCSFM_PASS_WGRAD 2
+int scsfm_conv_reads_lo(const ScsfmConv* p, int pass);
 /* Operand copies of a tensor for the tensor-core kernels: */
 #define SCSFM_OPERAND_TF32 0     /* round-to-nearest TF32 (plain TF32 mode) */
 #define SCSFM_OPERAND_RAW 1      /* bits unchanged (split mode: the MMA truncates, i.e. reads the high part) */

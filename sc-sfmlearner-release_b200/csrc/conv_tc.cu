@@ -604,6 +604,41 @@ static int launch_fwd_tc(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
 
 using namespace scsfm;
 
+// Weight-gradient kernel for *p: 1 the gather kernel, 2 the TMA kernel (and the gather kernel on the ring of a reflection-
+// padded layer), 3 the thin-layer fp32 kernel.  SCSFM_TUNE_WGRAD: 0 auto, 1 the gather kernel, 2 the TMA kernel (the
+// gather kernel where it does not apply), 3 the thin-layer kernel.
+static int wgrad_kernel(const ScsfmConv& p) {
+    const bool split = p.split || (p.in_lo != nullptr && p.dout_lo != nullptr);
+    int kernel = (int)((p.tune >> 12) & 3u);
+    if (kernel == 3 && !conv_wgrad_thin_eligible(p)) kernel = 0;
+    // the 16-output-channel decoder layers in split mode read four tensors and use 16 of the MMA's columns: the fp32 FMA
+    // kernel reads two and is exact per product (conv_wgrad_thin.cu)
+    if (kernel == 0 && (split || p.in_lo != nullptr || p.dout_lo != nullptr) && conv_wgrad_thin_eligible(p)) kernel = 3;
+    if ((kernel == 0 || kernel == 2) && conv_wgrad_tma_eligible(p) && (split || (p.in_lo == nullptr && p.dout_lo == nullptr))) return 2;
+    return kernel == 3 ? 3 : 1;
+}
+
+// split mode: does the kernel the dispatcher picks for *p read the low parts of its activation operands?  The stem forward
+// kernel and the TMA / thin weight-gradient kernels compute or do not need them; the gather kernels and the TMA forward
+// read them, as does the gather pass over the ring of a reflection-padded weight gradient.
+static bool conv_reads_lo(const ScsfmConv& p, int pass) {
+    if (pass == SCSFM_PASS_FWD) return !conv_stem_eligible(p);
+    if (pass == SCSFM_PASS_WGRAD) {
+        ScsfmConv q = p;
+        q.split = 1;
+        const int k = wgrad_kernel(q);
+        return k == 1 || (k == 2 && p.pad_mode == PADMODE_REFLECT);
+    }
+    return true;
+}
+
+extern "C" int scsfm_conv_reads_lo(const ScsfmConv* p, int pass) {
+    SCSFM_CHECK_ARG(p != nullptr && pass >= SCSFM_PASS_FWD && pass <= SCSFM_PASS_WGRAD, "conv_reads_lo: bad arguments");
+    SCSFM_CHECK_ARG(p->B > 0 && p->Hi > 0 && p->Wi > 0 && p->Cin > 0 && p->Cout > 0 && p->kh > 0 && p->kw > 0 && p->stride > 0 && p->pad >= 0,
+                    "conv_reads_lo: bad geometry");
+    return conv_reads_lo(*p, pass) ? 1 : 0;
+}
+
 // cp.async gather kernel: any stride / padding mode / border-only rows
 static int tc_dispatch_gather(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
     const int N = p.Cout;
@@ -631,6 +666,7 @@ static bool s2_prefers_gather(const ScsfmConv& p, const TcView& v) {
 }
 
 static int tc_dispatch(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
+    if (conv_stem_eligible(p)) return launch_conv_stem_fwd(p, st);      // (a data gradient's sub-convolutions have stride 1)
     if (p.pad_mode == PADMODE_ZERO && conv_tma_eligible(p, v) && !s2_prefers_gather(p, v)) return launch_conv_tma(p, v, st);
     if (p.pad_mode == PADMODE_REFLECT && v.in_stride == 1 && p.bn_sums == nullptr && p.Ho >= 3 && p.Wo >= 3 &&
         (p.Ho * p.Wo >= 64 * 208 || conv_tma_forced(p)) && conv_tma_eligible(p, v)) {
@@ -673,6 +709,11 @@ static int check_tc(const ScsfmConv* p, const char* who) {
 
 extern "C" int scsfm_conv2d_fwd_tc(const ScsfmConv* p, void* stream) {
     if (int rc = check_tc(p, "conv2d_fwd_tc")) return rc;
+    if (p->split) {
+        SCSFM_CHECK_ARG(p->w_lo != nullptr, "conv2d_fwd_tc: split mode needs w_lo");
+        SCSFM_CHECK_ARG(p->in_lo != nullptr || !conv_reads_lo(*p, SCSFM_PASS_FWD),
+                        "conv2d_fwd_tc: the kernel chosen for this call reads in_lo, which was not passed (scsfm_conv_reads_lo)");
+    }
     return tc_dispatch(*p, plain_view(*p), (cudaStream_t)stream);
 }
 
@@ -764,6 +805,7 @@ extern "C" int scsfm_weight_flip_s2(const float* w, int Cout, int kh, int kw, in
 extern "C" int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream) {
     SCSFM_CHECK_ARG(p != nullptr && p->dout && p->w && p->din, "conv2d_dgrad_tc: null tensor");
     SCSFM_CHECK_ARG(p->stride == 1 || p->stride == 2, "conv2d_dgrad_tc: stride must be 1 or 2");
+    SCSFM_CHECK_ARG(!p->split || (p->dout_lo != nullptr && p->w_lo != nullptr), "conv2d_dgrad_tc: split mode needs dout_lo and w_lo");
     SCSFM_CHECK_ARG(p->kh == p->kw && p->kh - 1 - p->pad >= 0, "conv2d_dgrad_tc: square kernels only");
     cudaStream_t st = (cudaStream_t)stream;
     ScsfmConv q = *p;
@@ -843,17 +885,12 @@ extern "C" int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream) {
     SCSFM_CHECK_ARG((p->Cin & 3) == 0 && (p->Cout & 3) == 0, "conv2d_wgrad_tc: needs Cin %% 4 == 0 and Cout %% 4 == 0");
     SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || p->pad == 1, "conv2d_wgrad_tc: reflect pad must be 1");
     SCSFM_CHECK_ARG((long long)p->B * p->Ho * p->Wo < (1LL << 31), "conv2d_wgrad_tc: too many pixels");
+    SCSFM_CHECK_ARG(!p->split || (p->in_lo != nullptr && p->dout_lo != nullptr) || !conv_reads_lo(*p, SCSFM_PASS_WGRAD),
+                    "conv2d_wgrad_tc: the kernel chosen for this call reads in_lo and dout_lo, which were not passed (scsfm_conv_reads_lo)");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    // SCSFM_TUNE_WGRAD: 0 auto, 1 the gather kernel, 2 the TMA kernel (the gather kernel where it does not apply), 3 the
-    // thin-layer fp32 kernel
-    int kernel = (int)((p->tune >> 12) & 3u);
-    if (kernel == 3 && !conv_wgrad_thin_eligible(*p)) kernel = 0;
-    // the 16-output-channel decoder layers in split mode read four tensors and use 16 of the MMA's columns: the fp32 FMA
-    // kernel reads two and is exact per product (conv_wgrad_thin.cu)
-    if (kernel == 0 && (p->in_lo != nullptr || p->dout_lo != nullptr) && conv_wgrad_thin_eligible(*p)) kernel = 3;
-    const bool split = p->in_lo != nullptr && p->dout_lo != nullptr;
-    if ((kernel == 0 || kernel == 2) && conv_wgrad_tma_eligible(*p) && (split || (p->in_lo == nullptr && p->dout_lo == nullptr))) {
+    const int kernel = wgrad_kernel(*p);
+    if (kernel == 2) {
         // reflection padding: the TMA kernel takes the interior with zero padding, the gather kernel the border ring
         if ((rc = launch_conv_wgrad_tma(*p, st))) return rc;
         rc = p->pad_mode == PADMODE_REFLECT ? wgrad_gather(*p, 1, st) : SCSFM_OK;

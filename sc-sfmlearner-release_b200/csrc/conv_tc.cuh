@@ -78,6 +78,11 @@ bool conv_tma_eligible(const ScsfmConv& p, const TcView& v);
 bool conv_tma_forced(const ScsfmConv& p);      // a tile configuration is being forced through ScsfmConv.tune (tests / experiments)
 int launch_conv_tma(const ScsfmConv& p, const TcView& v, cudaStream_t st);
 
+// conv_stem_fwd.cu: forward of the 7x7 stride-2 pad-3 zero-padded stems with Cin 4 or 8 and Cout 64
+// (TMA box of the tile's input rows, register A operand, lo(in) computed from it: in_lo is never read)
+bool conv_stem_eligible(const ScsfmConv& p);
+int launch_conv_stem_fwd(const ScsfmConv& p, cudaStream_t st);
+
 // conv_wgrad_tma.cu: weight gradient of stride-1 and zero-padded stride-2 layers with kh, kw <= 3 and of the 7x7
 // stride-2 stems with 4 or 8 channels (TMA halo patch, register A operand); with reflection padding it covers the
 // interior pixels only (the ring goes through the gather kernel's border view)

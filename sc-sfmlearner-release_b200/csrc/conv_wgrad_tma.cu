@@ -69,41 +69,6 @@ __device__ __forceinline__ uint32_t ld_shared_u32(uint32_t saddr) {
     return v;
 }
 
-// D[64 x N] (+)= A[64 x 8] (registers) * B[8 x N] (shared memory, K-major), tf32 operands, fp32 accumulation
-template <int N>
-__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate);
-template <>
-__device__ __forceinline__ void wgmma_tf32_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %21, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
-        "}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t"
-        "}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32_rs<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %37, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
-        "}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t"
-        "}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
-}
-
 // KW: taps per kernel row (1 or 3; a 2-wide kernel runs as KW = 3 with the third tap's sums discarded).  S: stride.
 // KW = 7: the 7x7 stride-2 stems with Cin = 4 or 8 (padded) channels.  A kernel row times the channels is only 28 or 56
 // rows, so the stem puts (dx, c) on M, m = dx * Cin + c, with one accumulator: the box holds the 4 x 37 x Cin patch
@@ -273,14 +238,14 @@ conv_wgrad_tma_kernel(ScsfmConv p, WtGeom g, const __grid_constant__ CUtensorMap
                     for (int j = 0; j < NS; ++j) {
                         const int sl = 4 * wg + NS * h + j;
                         const uint32_t boff = (uint32_t)((sl >> 2) * BN * 128 + (sl & 3) * 32);
-                        wgmma_tf32_rs<BN>(part, alo[j], tc::make_desc_sw128(bhi + boff), j == 0 ? 0u : 1u);
-                        wgmma_tf32_rs<BN>(part, ahi[j], tc::make_desc_sw128(blo + boff), 1u);
+                        tc::wgmma_tf32_rs<BN>(part, alo[j], tc::make_desc_sw128(bhi + boff), j == 0 ? 0u : 1u);
+                        tc::wgmma_tf32_rs<BN>(part, ahi[j], tc::make_desc_sw128(blo + boff), 1u);
                     }
 #pragma unroll
                     for (int j = 0; j < NS; ++j) {
                         const int sl = 4 * wg + NS * h + j;
                         const uint32_t boff = (uint32_t)((sl >> 2) * BN * 128 + (sl & 3) * 32);
-                        wgmma_tf32_rs<BN>(part, ahi[j], tc::make_desc_sw128(bhi + boff), 1u);
+                        tc::wgmma_tf32_rs<BN>(part, ahi[j], tc::make_desc_sw128(bhi + boff), 1u);
                     }
                     tc::wgmma_commit();
                     tc::wgmma_wait<0>();
@@ -294,7 +259,7 @@ conv_wgrad_tma_kernel(ScsfmConv p, WtGeom g, const __grid_constant__ CUtensorMap
                     for (int j = 0; j < NS; ++j) {
                         const int sl = 4 * wg + j;
                         const uint32_t boff = (uint32_t)((sl >> 2) * BN * 128 + (sl & 3) * 32);
-                        wgmma_tf32_rs<BN>(acc[dx], ahi[j], tc::make_desc_sw128(bhi + boff), 1u);
+                        tc::wgmma_tf32_rs<BN>(acc[dx], ahi[j], tc::make_desc_sw128(bhi + boff), 1u);
                     }
                     tc::wgmma_commit();
                     tc::wgmma_wait<0>();
@@ -415,10 +380,10 @@ static int launch_wgrad_tma_bn(const ScsfmConv& p, cudaStream_t st) {
 }
 
 // Zero-padded pass over every pixel (reflection padding: interior pixels only, the caller adds the ring).  Split mode is
-// taken from p.in_lo / p.dout_lo being set; the kernel recomputes the low parts rather than reading them.
+// taken from p.split or from p.in_lo / p.dout_lo being set; the kernel recomputes the low parts rather than reading them.
 // SCSFM_TUNE_BN(32 | 64) picks the Cout tile (default: 32 for Cout <= 32, else 64).
 int launch_conv_wgrad_tma(const ScsfmConv& p, cudaStream_t st) {
-    const bool split = p.in_lo != nullptr && p.dout_lo != nullptr;
+    const bool split = p.split || (p.in_lo != nullptr && p.dout_lo != nullptr);
     const unsigned bn_knob = (p.tune >> 8) & 7u;
     const bool bn32 = bn_knob == 2 || (bn_knob != 3 && p.Cout <= 32);
     if (bn32) return split ? launch_wgrad_tma_bn<32, true>(p, st) : launch_wgrad_tma_bn<32, false>(p, st);

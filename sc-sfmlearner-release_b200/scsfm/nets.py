@@ -629,9 +629,11 @@ def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
     else:
         d_f0 = torch.empty_like(f0)
         O.maxpool_bwd(d, rec["pool_idx"], f0.shape, d_f0, False)
-    # the low part of dy is read only by the tensor-core weight gradient (the plain stem runs in fp32 mode, without one)
+    # lo(dy) could only be read by the stem's weight gradient (its data gradient, stem_dgrad, is exact fp32), and the TMA
+    # weight-gradient kernel computes it itself
+    w_shape = (t.conv1.weight.shape[0], t.conv1.k, t.conv1.k, x.shape[-1])
     dy, _ = O.bn_backward(d_f0, f0, stem.y, stem.saved, *_bn_param_grads(t.bn1, plan), 1 | cx.rnd() | plan.bn, False, G,
-                          cx.split and plan.params)
+                          plan.params and cx.wgrad_reads_lo(x.shape, w_shape, 2, 3))
     if plan.params:
         if x.shape[-1] != t.conv1.weight.shape[1]:
             # padded-channel stem (tensor-core modes): weight gradient in the padded layout, then folded into the gradient arena

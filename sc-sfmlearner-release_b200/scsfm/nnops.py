@@ -41,7 +41,10 @@ class Conv(ctypes.Structure):
                                              "stride", "pad", "pad_mode", "act")] +
                 [(n, ctypes.c_void_p) for n in ("in_lo", "w_lo", "dout_lo")] +
                 [("tune", ctypes.c_uint), ("debug", ctypes.c_void_p)] +
-                [(n, ctypes.c_void_p) for n in ("bn_scale", "bn_shift", "out_lo")])
+                [(n, ctypes.c_void_p) for n in ("bn_scale", "bn_shift", "out_lo")] +
+                [("split", ctypes.c_int)])
+
+PASS_FWD, PASS_DGRAD, PASS_WGRAD = 0, 1, 2        # SCSFM_PASS_* of scsfm_conv_reads_lo
 
 
 _bound = False
@@ -56,6 +59,7 @@ def _lib():
         for name in ("scsfm_conv2d_fwd_simt", "scsfm_conv2d_dgrad_simt", "scsfm_conv2d_wgrad_simt",
                      "scsfm_conv2d_fwd_tc", "scsfm_conv2d_dgrad_tc", "scsfm_conv2d_wgrad_tc"):
             getattr(lib, name).argtypes = [CP, P]
+        lib.scsfm_conv_reads_lo.argtypes = [CP, I]
         lib.scsfm_round_tf32.argtypes = [P, P, LL, P]
         lib.scsfm_split_tf32.argtypes = [P, P, LL, P]
         lib.scsfm_weight_flip.argtypes = [P, I, I, I, I, P, I, P]
@@ -167,8 +171,10 @@ class FlipTable:
 
 
 def conv_desc(x_shape, w, stride, pad, pad_mode, act):
+    """ScsfmConv of a convolution of an input of shape x_shape with weights w (a tensor, or only their shape)."""
     B, Hi, Wi, Cin = x_shape
-    Cout, kh, kw, _ = w.shape
+    Cout, kh, kw, _ = w if isinstance(w, tuple) else w.shape
+    w = None if isinstance(w, tuple) else w
     Ho = (Hi + 2 * pad - kh) // stride + 1
     Wo = (Wi + 2 * pad - kw) // stride + 1
     return Conv(None, L.ptr(w), None, None, None, None, None, None, None, None, 1, B, Hi, Wi, Cin, Ho, Wo, Cout, kh, kw,
@@ -230,6 +236,22 @@ class ConvCtx:
         d.tune = self.tune
         d.debug = self.debug.data_ptr() if self.debug is not None else None
 
+    def _reads_lo(self, d, pass_):
+        """tf32x3: does the kernel picked for descriptor d (its tune included) read the low parts of its activation
+        operands?  The stem forward and the TMA / thin-layer weight gradients compute them themselves."""
+        rc = _lib().scsfm_conv_reads_lo(ctypes.byref(d), pass_)
+        L.check(0 if rc >= 0 else rc, "scsfm_conv_reads_lo")
+        return rc == 1
+
+    def wgrad_reads_lo(self, x_shape, w_shape, stride, pad, pad_mode=PAD_ZERO):
+        """Whether conv_wgrad of this shape will read lo(x) and lo(dout): False outside tf32x3, and where its kernel
+        computes them itself (a producer of dout can then skip writing lo(dout))."""
+        if not (self.split and self._use_tc("wgrad", x_shape[-1], w_shape[0], w_shape[1], stride)):
+            return False
+        d = conv_desc(tuple(x_shape), tuple(w_shape), stride, pad, pad_mode, ACT_NONE)
+        self._finish(d)
+        return self._reads_lo(d, PASS_WGRAD)
+
     # -- flipped weights of the data gradients -----------------------------------------------------------
     def flipped_weights(self, w, stride, pad, operand):
         """[Cout,kh,kw,Cin] -> weights of the transposed conv ([Cin,kh,kw,Cout], reversed taps; for stride 2 the four
@@ -288,8 +310,10 @@ class ConvCtx:
         if tc and self.split:
             if w_lo is None:
                 raise RuntimeError("tf32x3 convolution called without the low part of its weights")
-            d.in_lo, d.w_lo = lo_of(x).data_ptr(), w_lo.data_ptr()
+            d.w_lo, d.split = w_lo.data_ptr(), 1
         self._finish(d)
+        if tc and self.split and self._reads_lo(d, PASS_FWD):
+            d.in_lo = lo_of(x).data_ptr()
         _tag(d)
         fn = lib.scsfm_conv2d_fwd_tc if tc else lib.scsfm_conv2d_fwd_simt
         L.launch(fn, "scsfm_conv2d_fwd", "conv_fwd_tc" if tc else "conv_fwd_simt", 1, _flops(d), ctypes.byref(d), L.stream())
@@ -313,7 +337,7 @@ class ConvCtx:
                 src = w if w_src is None else w_src
                 d.w = self.flipped_weights(src, stride, pad, OPERAND_RAW).data_ptr()
                 d.w_lo = self.flipped_weights(src, stride, pad, OPERAND_LO).data_ptr()
-                d.dout_lo = lo_of(dout).data_ptr()
+                d.dout_lo, d.split = lo_of(dout).data_ptr(), 1
             else:
                 d.w = self.flipped_weights(w, stride, pad, OPERAND_TF32).data_ptr()
         self._finish(d)
@@ -332,11 +356,13 @@ class ConvCtx:
         d.w = None
         tc = self._use_tc("wgrad", d.Cin, d.Cout, d.kh, stride)
         keep = [x, dout]
-        if tc and self.split:
-            x_lo, dout_lo = lo_of(x), lo_of(dout)          # (computed on the CURRENT stream: the data gradient reads them too)
-            d.in_lo, d.dout_lo = x_lo.data_ptr(), dout_lo.data_ptr()
-            keep += [x_lo, dout_lo]
         self._finish(d)
+        if tc and self.split:
+            d.split = 1
+            if self._reads_lo(d, PASS_WGRAD):
+                x_lo, dout_lo = lo_of(x), lo_of(dout)      # (computed on the CURRENT stream: the data gradient reads them too)
+                d.in_lo, d.dout_lo = x_lo.data_ptr(), dout_lo.data_ptr()
+                keep += [x_lo, dout_lo]
         _tag(d)
         fn = lib.scsfm_conv2d_wgrad_tc if tc else lib.scsfm_conv2d_wgrad_simt
         with self.on_wgrad_stream(keep):
