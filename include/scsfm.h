@@ -316,7 +316,7 @@ int scsfm_maxpool_bwd(const float* dy, const unsigned char* idx, int B, int H, i
 int scsfm_upcat_fwd(const float* lo, const float* skip, int B, int H, int W, int C1, int C2, float* out, void* stream);
 /* Backward of ReflectionPad2d(1) (+ optional upsample/concat): dpad is the gradient w.r.t. the padded tensor
  * [B,H+2,W+2,C1+C2].  d_lo [B,H/2,W/2,C1] (overwritten; multiplied by act'(lo_act) if act != NONE),
- * d_skip [B,H,W,C2] overwritten.  With C2 == 0 and upsample == 0: plain fold into d_lo [B,H,W,C1]
+ * d_skip [B,H,W,C2] overwritten, or NULL when its gradient is not wanted (not computed).  With C2 == 0 and upsample == 0: plain fold into d_lo [B,H,W,C1]
  * (accumulate flag honoured, act applied after accumulation). */
 int scsfm_fold_bwd(const float* dpad, int B, int H, int W, int C1, int C2, int upsample, float* d_lo,
                    const float* lo_act, int act, int accumulate, float* d_skip, void* stream);
@@ -411,6 +411,13 @@ int scsfm_split_tf32(const float* in, float* lo, long long n, void* stream);
 int scsfm_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n, float lr,
                     float beta1, float beta2, float eps, float weight_decay, int step, const int* step_dev,
                     float* mirror, int mirror_operand, void* stream);
+/* scsfm_adam_step for an arena with frozen parameters: chunk_mask (device, ceil(n / 64) bytes) says per 64-float chunk whether
+ * it is trainable (nonzero).  Frozen chunks are not touched at all -- parameter, exp_avg, exp_avg_sq, weight decay, mirror --
+ * as torch.optim.Adam skips parameters whose grad is None; every parameter of an arena starts on a 64-float boundary.
+ * Trainable elements get exactly scsfm_adam_step's arithmetic (an all-ones mask gives the same bits). */
+int scsfm_adam_step_masked(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
+                           const unsigned char* chunk_mask, float lr, float beta1, float beta2, float eps, float weight_decay,
+                           int step, const int* step_dev, float* mirror, int mirror_operand, void* stream);
 
 #ifdef __cplusplus
 }

@@ -674,28 +674,52 @@ __global__ void __launch_bounds__(NT) split_tf32_kernel(const float* __restrict_
 }
 
 // ----- Adam ---------------------------------------------------------------------------------------
+// torch.optim.Adam (non-amsgrad): m = b1 m + (1-b1) g ; v = b2 v + (1-b2) g^2 ;
+// p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps).  The step count may live on the device so that a captured
+// CUDA graph of the training step stays valid across replays.
+struct AdamCoeffs {
+    float step_size, bc2_sqrt;
+};
+
+__device__ __forceinline__ AdamCoeffs adam_coeffs(float lr, float b1, float b2, int step_host, const int* __restrict__ step_dev) {
+    const int step = step_dev ? *step_dev : step_host;
+    const float bc1 = 1.0f - powf(b1, (float)step);
+    return AdamCoeffs{lr / bc1, sqrtf(1.0f - powf(b2, (float)step))};
+}
+
+// the update of element i: shared by the whole-arena and the masked kernel, so both give the same bits
+__device__ __forceinline__ void adam_update(long long i, float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                            float* __restrict__ v, float b1, float b2, float eps, float wd, AdamCoeffs c,
+                                            float* __restrict__ mirror, int mirror_operand) {
+    float gr = g[i];
+    const float pp = p[i];
+    if (wd != 0.f) gr += wd * pp;
+    const float mm = b1 * m[i] + (1.f - b1) * gr;
+    const float vv = b2 * v[i] + (1.f - b2) * gr * gr;
+    m[i] = mm;
+    v[i] = vv;
+    const float pn = pp - c.step_size * (mm / (sqrtf(vv) / c.bc2_sqrt + eps));
+    p[i] = pn;
+    if (mirror != nullptr) mirror[i] = tc_operand(pn, mirror_operand);      // operand mirror of the tensor-core convolutions
+}
+
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                             long long n, float lr, float b1, float b2, float eps, float wd, int step_host,
                             const int* __restrict__ step_dev, float* __restrict__ mirror, int mirror_operand) {
-    // torch.optim.Adam (non-amsgrad): m = b1 m + (1-b1) g ; v = b2 v + (1-b2) g^2 ;
-    // p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps).  The step count may live on the device so that a captured
-    // CUDA graph of the training step stays valid across replays.
-    const int step = step_dev ? *step_dev : step_host;
-    const float bc1 = 1.0f - powf(b1, (float)step);
-    const float bc2_sqrt = sqrtf(1.0f - powf(b2, (float)step));
-    const float step_size = lr / bc1;
-    for (long long i = blockIdx.x * (long long)NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT) {
-        float gr = g[i];
-        const float pp = p[i];
-        if (wd != 0.f) gr += wd * pp;
-        const float mm = b1 * m[i] + (1.f - b1) * gr;
-        const float vv = b2 * v[i] + (1.f - b2) * gr * gr;
-        m[i] = mm;
-        v[i] = vv;
-        const float pn = pp - step_size * (mm / (sqrtf(vv) / bc2_sqrt + eps));
-        p[i] = pn;
-        if (mirror != nullptr) mirror[i] = tc_operand(pn, mirror_operand);      // operand mirror of the tensor-core convolutions
-    }
+    const AdamCoeffs c = adam_coeffs(lr, b1, b2, step_host, step_dev);
+    for (long long i = blockIdx.x * (long long)NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT)
+        adam_update(i, p, g, m, v, b1, b2, eps, wd, c, mirror, mirror_operand);
+}
+
+// Frozen parameters (torch.optim.Adam skips `grad is None`): chunk_mask[i / 64] == 0 leaves element i's parameter, moments and
+// operand mirror untouched.  Every parameter of an arena starts on a 64-float boundary, so a chunk never straddles two of them.
+__global__ void adam_masked_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                   long long n, const unsigned char* __restrict__ chunk_mask, float lr, float b1, float b2, float eps,
+                                   float wd, int step_host, const int* __restrict__ step_dev, float* __restrict__ mirror,
+                                   int mirror_operand) {
+    const AdamCoeffs c = adam_coeffs(lr, b1, b2, step_host, step_dev);
+    for (long long i = blockIdx.x * (long long)NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT)
+        if (__ldg(chunk_mask + (i >> 6))) adam_update(i, p, g, m, v, b1, b2, eps, wd, c, mirror, mirror_operand);
 }
 
 }  // namespace scsfm
@@ -867,10 +891,10 @@ extern "C" int scsfm_fold_bwd(const float* dpad, int B, int H, int W, int C1, in
         SCSFM_CHECK_LAUNCH();
         return SCSFM_OK;
     }
-    SCSFM_CHECK_ARG((H & 1) == 0 && (W & 1) == 0 && (C2 == 0 || d_skip), "fold_bwd: bad upsample geometry");
+    SCSFM_CHECK_ARG((H & 1) == 0 && (W & 1) == 0, "fold_bwd: bad upsample geometry");
     fold_up_lo_kernel<<<grid_for((long long)B * (H / 2) * (W / 2) * (C1 / 4)), NT, 0, ST>>>(dpad, B, H, W, C1, C1 + C2, d_lo, lo_act, act);
     SCSFM_CHECK_LAUNCH();
-    if (C2 > 0) {
+    if (C2 > 0 && d_skip) {
         fold_up_skip_kernel<<<grid_for((long long)B * H * W * (C2 / 4)), NT, 0, ST>>>(dpad, B, H, W, C1, C2, d_skip);
         SCSFM_CHECK_LAUNCH();
     }
@@ -921,6 +945,19 @@ extern "C" int scsfm_adam_step(float* param, const float* grad, float* exp_avg, 
     SCSFM_CHECK_ARG(mirror_operand == SCSFM_OPERAND_TF32 || mirror_operand == SCSFM_OPERAND_LO, "adam_step: bad mirror operand kind");
     adam_kernel<<<grid_for(n), NT, 0, ST>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, step_dev, mirror,
                                             mirror_operand);
+    SCSFM_CHECK_LAUNCH();
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_adam_step_masked(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
+                                      const unsigned char* chunk_mask, float lr, float beta1, float beta2, float eps,
+                                      float weight_decay, int step, const int* step_dev, float* mirror, int mirror_operand,
+                                      void* stream) {
+    SCSFM_CHECK_ARG(param && grad && exp_avg && exp_avg_sq && chunk_mask && n > 0 && (step >= 1 || step_dev),
+                    "adam_step_masked: bad arguments");
+    SCSFM_CHECK_ARG(mirror_operand == SCSFM_OPERAND_TF32 || mirror_operand == SCSFM_OPERAND_LO, "adam_step_masked: bad mirror operand kind");
+    adam_masked_kernel<<<grid_for(n), NT, 0, ST>>>(param, grad, exp_avg, exp_avg_sq, n, chunk_mask, lr, beta1, beta2, eps, weight_decay,
+                                                   step, step_dev, mirror, mirror_operand);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }

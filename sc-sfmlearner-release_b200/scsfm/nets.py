@@ -60,14 +60,20 @@ class ConvParams(nn.Module):
         return self._tc_view if cx.split else None
 
 
-class BNParams(nn.Module):
-    def __init__(self, c):
-        super().__init__()
-        self.weight = nn.Parameter(torch.ones(c))
-        self.bias = nn.Parameter(torch.zeros(c))
-        self.register_buffer("running_mean", torch.zeros(c))
-        self.register_buffer("running_var", torch.ones(c))
-        self.register_buffer("num_batches_tracked", torch.tensor(0, dtype=torch.long))
+class BNParams(nn.BatchNorm2d):
+    """The reference's nn.BatchNorm2d(c): the same parameters, buffers, state_dict keys and initial values, found by
+    isinstance(m, nn.BatchNorm2d), and put in eval mode per module (`m.eval()`: running statistics, none updated).  The
+    network's kernels apply it, so its own forward is never called, and momentum / eps other than the reference's are refused
+    (check_supported)."""
+
+    def forward(self, x):
+        raise RuntimeError("BNParams is applied by its network's kernels; it is not callable on its own")
+
+    def check_supported(self):
+        if self.momentum != BN_MOMENTUM or self.eps != BN_EPS or not self.affine or not self.track_running_stats:
+            raise ValueError("BatchNorm with momentum=%r eps=%r affine=%r track_running_stats=%r: the network kernels implement "
+                             "only the reference's momentum=%r eps=%r with affine parameters and running statistics"
+                             % (self.momentum, self.eps, self.affine, self.track_running_stats, BN_MOMENTUM, BN_EPS))
 
 
 class LinearParams(nn.Module):
@@ -285,20 +291,21 @@ class ArenaNet(nn.Module):
                 gv = gflat[off:off + cnt].view(p.shape)
             dst.copy_(p.data)
             p.data = dst
-            p.grad = gv
+            p.grad = gv if p.requires_grad else None
+            p._arena_grad = gv             # what the kernels accumulate into, whether or not p.grad exposes it
             views.append((p, gv))
             off += O.aligned64(cnt)
         self._flat, self._flat_grad, self._views = flat, gflat, views
         self._hook = torch.zeros(1, device=dev, requires_grad=True)
         # num_batches_tracked of all BatchNorm layers as views of one int64 tensor (one add per network call)
-        bns = [m for m in self.modules() if isinstance(m, BNParams)]
+        bns = self._bns = [m for m in self.modules() if isinstance(m, BNParams)]
         if bns:
             nbt = torch.stack([m.num_batches_tracked.to(dev) for m in bns])
             for i, m in enumerate(bns):
                 m.num_batches_tracked = nbt[i]
             for m in self.modules():
                 if isinstance(m, ResnetEncoder):
-                    m._nbt = nbt
+                    m._nbt, m._nbt_bns, m._nbt_inc = nbt, bns, {}
         self._tf32_version = None
         self.ctx.invalidate()              # cached flips referred to the previous arena
 
@@ -329,7 +336,19 @@ class ArenaNet(nn.Module):
     def _fused_eval(self):
         """Eval mode with autograd off: the forward runs without recording (every activation is freed once dead) and with
         BatchNorm fused into the convolution epilogues (see _conv_bn)."""
-        return not self.training and not torch.is_grad_enabled()
+        return not self.training and not torch.is_grad_enabled() and not any(bn.training for bn in self._bns)
+
+    def _encoder_forward(self, groups, imgs, fused, plan):
+        """The encoder part of a network call: fused where the whole call is, and inside a recording call whose backward does
+        not reach the encoder (plan.feats[4] False) when all its BatchNorms are in eval mode -- bitwise the same features,
+        no record."""
+        fused = fused or (not plan.feats[4] and not any(bn.training for bn in self._bns))
+        return encoder_forward(_Forward(self, groups, fused, plan), self.encoder, imgs)
+
+    def flag_pattern(self):
+        """The module flags a network call depends on: requires_grad of every parameter, the mode of every BatchNorm and of
+        the network (a CUDA graph captured with one pattern is not valid for another).  Needs the packed arena."""
+        return (self.training, tuple(p.requires_grad for p, _ in self._views), tuple(bn.training for bn in self._bns))
 
     def _call(self, inputs, groups=None):
         """One network call on `inputs`: the fused eval forward, or one autograd node.  groups=None returns the call's
@@ -337,12 +356,16 @@ class ArenaNet(nn.Module):
         group) and the result is one output list per group."""
         G = groups or 1
         self.ensure_arena()
+        for bn in self._bns:
+            bn.check_supported()
         if self._fused_eval():
             outs = self._forward_impl(G, *inputs, fused=True)[1]
         else:
-            if torch.is_grad_enabled():
+            grad = torch.is_grad_enabled()
+            if grad:
                 self._pending += 1
-            outs = _NetCall.apply(self, self._hook, G, *inputs)
+            plan = BackwardPlan(self, [grad and x.requires_grad for x in inputs])
+            outs = _NetCall.apply(self, self._hook, G, plan, *inputs)
         if groups is None:
             return outs
         B = inputs[0].shape[0] // G
@@ -359,19 +382,28 @@ class ArenaNet(nn.Module):
         return {id(bn): c for bn, c in zip(bns, tab.coeffs)}
 
     def _attach_grads(self):
-        """Called at the start of every backward: if an optimizer dropped the gradients
-        (zero_grad(set_to_none=True)) the arena is stale -> zero it and re-attach the views."""
-        if self._views and self._views[0][0].grad is None:
+        """Called at the start of every backward that computes parameter gradients: trainable parameters get their arena view
+        as .grad, frozen ones keep None (as autograd leaves them; torch.optim then skips them).  If an optimizer dropped the
+        gradients (zero_grad(set_to_none=True)) the arena is stale -> zero it; a parameter trainable again after being frozen
+        starts from a zeroed slice."""
+        first = next((p for p, _ in self._views if p.requires_grad), None)
+        stale = first is not None and first.grad is None
+        if stale:
             self._flat_grad.zero_()
         for p, gv in self._views:
-            if p.grad is not gv:
+            if not p.requires_grad:
+                if p.grad is gv:
+                    p.grad = None
+            elif p.grad is not gv:
+                if p.grad is None and not stale:
+                    gv.zero_()
                 p.grad = gv
 
     def zero_grad(self, set_to_none=False):
         if self._flat_grad is not None:
             self._flat_grad.zero_()
             for p, gv in self._views:
-                p.grad = gv
+                p.grad = gv if p.requires_grad else None
         else:
             super().zero_grad(set_to_none=set_to_none)
 
@@ -385,31 +417,81 @@ class ArenaNet(nn.Module):
 
     @staticmethod
     def g(p):
-        """Gradient buffer of a parameter in kernel layout."""
-        return p.grad.permute(0, 2, 3, 1) if p.dim() == 4 else p.grad
+        """Gradient buffer of a parameter (its arena slice) in kernel layout."""
+        g = p._arena_grad
+        return g.permute(0, 2, 3, 1) if p.dim() == 4 else g
 
 
 class BackwardPlan:
-    """What one network backward computes.
-      bn:     flags OR-ed into every BatchNorm backward: O.BN_FROZEN when the forward ran in eval mode (it normalised with the
-              running statistics, so the batch-statistics terms of the gradient are absent);
-      params: parameter gradients at all -- False when no parameter of the network requires grad: then no weight-gradient,
-              head-gradient or BatchNorm parameter-gradient work is issued and the gradient arena is left alone;
-      dimg:   one flag per input image (DispResNet 1, PoseResNet 2): its gradient is wanted (the stem's data gradient)."""
+    """What one network backward computes, unit by unit.  A unit is a (conv, BatchNorm) pair, a decoder convolution, a
+    disparity head or a pose-head convolution, keyed by id() of its convolution module.  The plan is a pure function of module
+    flags -- requires_grad of every parameter and which input images need a gradient -- decided when the forward runs, so
+    that the forward knows what to record.
 
-    def __init__(self, training=True, params=True, dimg=(False, False)):
-        self.bn = 0 if training else O.BN_FROZEN
-        self.params = params
+    A gradient w.r.t. an activation is "live" when a trainable parameter or an image needing a gradient lies upstream of it
+    (at or below it in backward order).  Per unit:
+      runs[u]:    the gradient w.r.t. its output is live: its backward (BatchNorm backward, weight / data gradients) runs;
+      dgrad[u]:   the gradient w.r.t. its input is live: its data gradient runs;
+      trains(p):  the parameter requires grad: the unit runs the weight (BatchNorm parameter) gradient it belongs to;
+      feats[j]:   the gradient w.r.t. encoder feature j (stem output, layers 1-4) is live -- feats[4] False: the encoder has no
+                  backward and its forward keeps no record;
+      dimg:       one flag per input image (DispResNet 1, PoseResNet 2): its gradient is wanted (the stem's data gradient).
+    Which BatchNorm backward a unit uses (O.BN_FROZEN for a module in eval mode) is recorded by the forward with the unit."""
+
+    def __init__(self, net, dimg):
         self.dimg = tuple(bool(n) for n in dimg)
+        self.train = {id(p) for p in net.parameters() if p.requires_grad} if torch.is_grad_enabled() else set()
+        self.runs, self.dgrad = {}, {}
+        t = net.encoder.encoder
+        live = self._unit(t.conv1, t.bn1, any(self.dimg))
+        self.feats = [live]
+        for li in range(1, 5):
+            for blk in getattr(t, "layer%d" % li):
+                main, ds = blk.units()
+                h = live
+                for conv, bn, _, _ in main[:-1]:
+                    h = self._unit(conv, bn, h)
+                sc = live if ds is None else self._unit(ds[0], ds[1], live)
+                # the last unit's backward also gates the shortcut's gradient (dres): it runs when the block output is live
+                last = self._unit(main[-1][0], main[-1][1], h) or sc
+                self.runs[id(main[-1][0])] = last
+                live = last
+            self.feats.append(live)
+        if isinstance(net, DispResNet):
+            cur = live
+            for i in range(4, -1, -1):
+                a = self._unit(net.decoder.up(i, 0), None, cur)
+                cur = self._unit(net.decoder.up(i, 1), None, a or (i > 0 and self.feats[i - 1]))
+                if i < 4:
+                    self._unit(net.decoder.disp(i), None, cur)
+        else:
+            for conv in net.decoder.net:
+                live = self._unit(conv, None, live)
+        self.any = any(self.runs.values())       # the backward has anything to do (an image gradient makes every unit run)
 
+    def _unit(self, conv, bn, live_in):
+        """Records the unit's flags; returns whether the gradient w.r.t. its output is live."""
+        out = live_in or self.trains(conv.weight) or self.trains(conv.bias) or (
+            bn is not None and (self.trains(bn.weight) or self.trains(bn.bias)))
+        self.runs[id(conv)], self.dgrad[id(conv)] = out, live_in
+        return out
 
-TRAIN_PLAN = BackwardPlan()
+    def trains(self, p):
+        return p is not None and id(p) in self.train
+
+    def wgrad(self, conv):
+        """The unit's convolution runs its weight (and bias) gradient."""
+        return self.trains(conv.weight) or self.trains(conv.bias)
+
+    def grad_of(self, p):
+        """The arena slice that receives p's gradient when p is trainable, else None (the kernel skips it)."""
+        return ArenaNet.g(p) if self.trains(p) else None
 
 
 class _NetCall(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, net, hook, groups, *inputs):
-        rec, outs = net._forward_impl(groups, *inputs)
+    def forward(ctx, net, hook, groups, plan, *inputs):
+        rec, outs = net._forward_impl(groups, *inputs, plan=plan)
         ctx.net, ctx.rec = net, rec
         ctx.set_materialize_grads(False)     # unused outputs (scales 1-3 with --num-scales 1) arrive as None
         return tuple(outs)
@@ -417,12 +499,14 @@ class _NetCall(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         net = ctx.net
-        need = ctx.needs_input_grad[3:]
-        # the BatchNorm formula follows the mode the FORWARD ran in (recorded), not net.training now
-        plan = BackwardPlan(ctx.rec["training"], any(p.requires_grad for p, _ in net._views), need)
+        need = ctx.needs_input_grad[4:]
+        # the plan of the forward (what it recorded follows from it); the BatchNorm formula of every unit follows the mode its
+        # module had in the FORWARD (recorded with the unit), not its mode now
+        plan = ctx.rec["plan"]
+        assert plan.dimg == tuple(bool(n) for n in need)
         dimgs = [None] * len(need)
-        if plan.params or any(need):
-            if plan.params:
+        if plan.any:
+            if plan.train:
                 net._attach_grads()
             dimgs = net._backward_impl(ctx.rec, [None if g is None else g.contiguous() for g in grads], plan)
             net.ctx.join_wgrad()       # weight gradients enqueued on the side stream (if any) are part of this backward
@@ -430,7 +514,7 @@ class _NetCall(torch.autograd.Function):
         net._pending -= 1
         if net._pending == 0 and net.grads_ready_callback is not None:
             net.grads_ready_callback(net)
-        return (None, None, None) + tuple(dimgs)
+        return (None, None, None, None) + tuple(dimgs)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -472,12 +556,13 @@ def _pool(cx):
 
 
 class _Forward:
-    """What differs between the forwards of one network call.  Recording (coeffs None): BatchNorm with batch statistics
-    (training) or the running ones over `groups` independent sample groups, and every unit returns its record for the
-    backward.  Fused (coeffs = ArenaNet.bn_eval_coeffs()): eval-mode BatchNorm in the convolution epilogues, no record."""
+    """What differs between the forwards of one network call.  Recording (coeffs None): each BatchNorm with batch statistics
+    (its module in train mode) or the running ones (eval mode) over `groups` independent sample groups, and every unit whose
+    backward runs (plan.runs) returns its record.  Fused (coeffs = ArenaNet.bn_eval_coeffs()): eval-mode BatchNorm in the
+    convolution epilogues, no record."""
 
-    def __init__(self, net, groups, fused):
-        self.cx, self.training, self.groups = net.ctx, net.training, groups
+    def __init__(self, net, groups, fused, plan=None):
+        self.cx, self.groups, self.plan = net.ctx, groups, plan
         self.coeffs = net.bn_eval_coeffs() if fused else None
 
     @property
@@ -485,10 +570,11 @@ class _Forward:
         return self.coeffs is not None
 
 
-# One conv+BatchNorm unit of the recording forward: its input x, the convolution output y, the unit output z and the
-# BatchNorm's saved statistics.  z is kept only where a ReLU follows (the backward reads it for the ReLU's gate), so that
-# the record does not hold the downsample's output until the backward.
-_Unit = collections.namedtuple("_Unit", "x y z saved")
+# One conv+BatchNorm unit of the recording forward: its input x, the convolution output y, the unit output z, the
+# BatchNorm's saved statistics and the flags of its backward (O.BN_FROZEN when the module was in eval mode).  z is kept only
+# where a ReLU follows (the backward reads it for the ReLU's gate), so that the record does not hold the downsample's output
+# until the backward.
+_Unit = collections.namedtuple("_Unit", "x y z saved bn_flags")
 
 
 def _conv_bn(f, x, unit, relu, residual=None, with_lo=False, w=None):
@@ -507,30 +593,31 @@ def _conv_bn(f, x, unit, relu, residual=None, with_lo=False, w=None):
                         bn_scale=sc, bn_shift=sh, addend=residual, with_lo=with_lo and cx.split)
         return z, None
     G = f.groups
-    sums = _pool(cx).take(O.BN_SLOTS * G * conv.weight.shape[0] * 2, x.device) if f.training else None
+    sums = _pool(cx).take(O.BN_SLOTS * G * conv.weight.shape[0] * 2, x.device) if bn.training else None
     y = cx.conv_fwd(x, w, None, stride, pad, O.PAD_ZERO, O.ACT_NONE, sums, G, w_lo)
     z, saved = O.bn_apply(y, sums, bn.weight, bn.bias, bn.running_mean, bn.running_var, BN_MOMENTUM, BN_EPS, residual,
                           (1 if relu else 0) | cx.rnd(), G, cx.split)
-    return z, _Unit(x, y, z if relu else None, saved)
-
-
-def _bn_param_grads(bn, plan):
-    return (bn.weight.grad, bn.bias.grad) if plan.params else (None, None)
+    if not f.plan.runs[id(conv)]:
+        return z, None
+    return z, _Unit(x, y, z if relu else None, saved, 0 if bn.training else O.BN_FROZEN)
 
 
 def _conv_bn_bwd(cx, dz, unit, r, relu, want_dres, addend, groups, plan):
     """Backward through relu?(bn(conv(x)) [+res]) of `unit` with record `r`; `addend` is added to dx in the data gradient's
-    epilogue.  Returns (dx, dres or None)."""
+    epilogue.  Returns (dx, or None where the plan needs no data gradient; dres or None)."""
     conv, bn, stride, pad = unit
-    dy, dres = O.bn_backward(dz, r.z, r.y, r.saved, *_bn_param_grads(bn, plan), (1 if relu else 0) | cx.rnd() | plan.bn, want_dres,
-                             groups, cx.split)
-    if plan.params:
+    dy, dres = O.bn_backward(dz, r.z, r.y, r.saved, plan.grad_of(bn.weight), plan.grad_of(bn.bias),
+                             (1 if relu else 0) | cx.rnd() | r.bn_flags, want_dres, groups, cx.split)
+    if plan.wgrad(conv):
         cx.conv_wgrad(r.x, dy, ArenaNet.g(conv.weight), None, stride, pad, O.PAD_ZERO)
+    if not plan.dgrad[id(conv)]:
+        return None, dres
     return cx.conv_dgrad(dy, conv.w_op(cx), r.x.shape, stride, pad, addend), dres
 
 
 def block_forward(f, blk, x):
-    """Returns (block output, record: (main-path unit records, downsample record or None); None in the fused forward)."""
+    """Returns (block output, record: (main-path unit records, downsample record or None); None in the fused forward and
+    where the block's backward does not run)."""
     main, ds = blk.units()
     h, recs = x, []
     for unit in main[:-1]:
@@ -539,25 +626,30 @@ def block_forward(f, blk, x):
     # the shortcut runs between the main path's first convolution(s) and its last one
     sc, ds_rec = (x, None) if ds is None else _conv_bn(f, x, ds, False)
     out, r = _conv_bn(f, h, main[-1], True, sc, with_lo=True)
-    return out, None if f.fused else (recs + [r], ds_rec)
+    return out, None if f.fused or r is None else (recs + [r], ds_rec)
 
 
 def block_backward(cx, blk, rec, d_out, d_skip, groups, plan):
     """d_out: gradient w.r.t. the block output (consumed / overwritten).  d_skip: gradient that reaches the block INPUT from
     the decoder (skip connection) or None -- folded into the shortcut's dgrad epilogue.  Returns gradient w.r.t. the block
-    input."""
+    input, or None where the plan stops the backward inside this block.  Units whose backward does not run (nothing upstream of
+    them trains) are skipped: the main path from its first unit up, the shortcut."""
     main, ds = blk.units()
     recs, ds_rec = rec
     d, dres = _conv_bn_bwd(cx, d_out, main[-1], recs[-1], True, True, None, groups, plan)
     for k in range(len(main) - 2, 0, -1):
+        if d is None:                   # main[k] and the units before it do not run
+            break
         d, _ = _conv_bn_bwd(cx, d, main[k], recs[k], True, False, None, groups, plan)
     if ds is not None:
-        d_sc, _ = _conv_bn_bwd(cx, dres, ds, ds_rec, False, False, d_skip, groups, plan)
+        d_sc = _conv_bn_bwd(cx, dres, ds, ds_rec, False, False, d_skip, groups, plan)[0] if plan.runs[id(ds[0])] else None
     else:
         # a skip feature is the output of a layer's last block, and the block after it opens one of layers 2-4: stride 2,
         # so it has a downsample
         assert d_skip is None, "skip-connection gradient at a block without downsample"
         d_sc = dres
+    if d is None:
+        return None
     dx, _ = _conv_bn_bwd(cx, d, main[0], recs[0], True, False, d_sc, groups, plan)
     return dx
 
@@ -577,18 +669,11 @@ def _stem_operands(cx, conv, imgs):
 
 def encoder_forward(f, enc, imgs):
     """imgs: tuple of one (DispResNet) or two (PoseResNet, channel-concatenated) NCHW image batches.
-    Returns (record, or None in the fused forward; the five features)."""
+    Returns (record, or None in the fused forward and where the plan gives the encoder no backward; the five features)."""
     t = enc.encoder
     G = f.groups
-    if f.training:
-        _pool(f.cx).begin(imgs[0].device)
-        nbt = getattr(enc, "_nbt", None)
-        if nbt is not None:
-            nbt.add_(G)                      # every BatchNorm layer's num_batches_tracked (views of this tensor)
-        else:
-            for m in enc.modules():
-                if isinstance(m, BNParams):
-                    m.num_batches_tracked += G
+    if not f.fused:
+        _count_batches(f, enc, imgs[0].device)
     x_nhwc, w0, w0_lo = _stem_operands(f.cx, t.conv1, imgs)
     f0, stem = _conv_bn(f, x_nhwc, (t.conv1, t.bn1, 2, 3), True, w=(w0, w0_lo))
     del x_nhwc, w0, w0_lo              # dead in the fused forward (the record keeps the stem's input for the backward)
@@ -599,12 +684,35 @@ def encoder_forward(f, enc, imgs):
             x, r = block_forward(f, blk, x)
             blocks.append((blk, r))
         feats.append(x)
-    return None if f.fused else {"G": G, "stem": stem, "pool_idx": pool_idx, "blocks": blocks}, feats
+    if f.fused or not f.plan.feats[4]:
+        return None, feats
+    return {"G": G, "stem": stem, "pool_idx": pool_idx, "blocks": blocks}, feats
 
 
-def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
+def _count_batches(f, enc, device):
+    """Recording forward: readies the BatchNorm-sums pool when any module uses batch statistics, and adds the call's group
+    count to num_batches_tracked of every BatchNorm in train mode -- one add over the views of the encoder's one int64
+    tensor; with some modules in eval mode the increment is a cached per-module tensor, so the add stays capturable in a CUDA
+    graph."""
+    G, bns = f.groups, enc._nbt_bns
+    modes = tuple(bn.training for bn in bns)
+    if not any(modes):
+        return
+    _pool(f.cx).begin(device)
+    if all(modes):
+        enc._nbt.add_(G)
+        return
+    key = (modes, G)
+    inc = enc._nbt_inc.get(key)
+    if inc is None:
+        inc = enc._nbt_inc[key] = torch.tensor([G if m else 0 for m in modes], dtype=torch.long).to(enc._nbt.device)
+    enc._nbt.add_(inc)
+
+
+def encoder_backward(cx, enc, rec, d_feats, plan):
     """d_feats[i]: gradient w.r.t. feature i coming from the decoder (None if unused).  d_feats[4] is required.
-    Returns the gradients of the input images (NCHW, one per image of the forward; None where plan.dimg does not ask)."""
+    Returns the gradients of the input images (NCHW, one per image of the forward; None where plan.dimg does not ask).
+    The backward stops where nothing upstream trains (plan.runs): the blocks before that point, and the stem, do not run."""
     t = enc.encoder
     blocks, G = rec["blocks"], rec["G"]
     # index of the last block of each layer -> the feature it produces
@@ -615,11 +723,15 @@ def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
     d = d_feats[4]
     for bi in range(len(blocks) - 1, -1, -1):
         blk, r = blocks[bi]
+        if d is None:
+            return [None] * len(plan.dimg)
         # the INPUT of block bi is the output of block bi-1; if that is a skip feature, add the decoder's gradient
         extra = None
         if bi - 1 in ends and d_feats[ends[bi - 1]] is not None:
             extra = d_feats[ends[bi - 1]]
         d = block_backward(cx, blk, r, d, extra, G, plan)
+    if d is None:
+        return [None] * len(plan.dimg)
     # d is now the gradient w.r.t. the max-pool output
     stem = rec["stem"]
     f0, x = stem.z, stem.x
@@ -632,9 +744,10 @@ def encoder_backward(cx, enc, rec, d_feats, plan=TRAIN_PLAN):
     # lo(dy) could only be read by the stem's weight gradient (its data gradient, stem_dgrad, is exact fp32), and the TMA
     # weight-gradient kernel computes it itself
     w_shape = (t.conv1.weight.shape[0], t.conv1.k, t.conv1.k, x.shape[-1])
-    dy, _ = O.bn_backward(d_f0, f0, stem.y, stem.saved, *_bn_param_grads(t.bn1, plan), 1 | cx.rnd() | plan.bn, False, G,
-                          plan.params and cx.wgrad_reads_lo(x.shape, w_shape, 2, 3))
-    if plan.params:
+    wgrad = plan.wgrad(t.conv1)
+    dy, _ = O.bn_backward(d_f0, f0, stem.y, stem.saved, plan.grad_of(t.bn1.weight), plan.grad_of(t.bn1.bias),
+                          1 | cx.rnd() | stem.bn_flags, False, G, wgrad and cx.wgrad_reads_lo(x.shape, w_shape, 2, 3))
+    if wgrad:
         if x.shape[-1] != t.conv1.weight.shape[1]:
             # padded-channel stem (tensor-core modes): weight gradient in the padded layout, then folded into the gradient arena
             dw = torch.zeros(t.conv1.weight.shape[0], t.conv1.k, t.conv1.k, x.shape[-1], device=x.device, dtype=torch.float32)
@@ -676,16 +789,17 @@ class DispResNet(ArenaNet):
         return per if self.training else [p[0] for p in per]
 
     # -- forward ------------------------------------------------------------------------------
-    def _forward_impl(self, groups, x, fused=False):
-        """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs)."""
+    def _forward_impl(self, groups, x, fused=False, plan=None):
+        """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs).
+        Recording: plan (BackwardPlan) says which units' backward will run."""
         from . import lib as L
         x = L.dev_f32(x, "DispResNet input")
         self.refresh_operand_weights()
         training = self.training
         cx = self.ctx
-        enc_rec, feats = encoder_forward(_Forward(self, groups, fused), self.encoder, (x,))
+        enc_rec, feats = self._encoder_forward(groups, (x,), fused, plan)
         dec = self.decoder
-        rec = {"enc": enc_rec, "stages": {}, "training": training}
+        rec = {"enc": enc_rec, "stages": {}, "plan": plan}
         cur = feats[4]
         disps = {}
         for i in range(4, -1, -1):
@@ -713,7 +827,7 @@ class DispResNet(ArenaNet):
         return None if fused else rec, [disps[s].view(disps[s].shape[0], 1, disps[s].shape[1], disps[s].shape[2]) for s in order]
 
     # -- backward -----------------------------------------------------------------------------
-    def _backward_impl(self, rec, grads, plan=TRAIN_PLAN):
+    def _backward_impl(self, rec, grads, plan):
         """Returns [gradient of the input images or None] (see encoder_backward)."""
         dec = self.decoder
         g = ArenaNet.g
@@ -725,14 +839,18 @@ class DispResNet(ArenaNet):
         for i in range(0, 5):
             st = rec["stages"][i]
             b = st["b"]
+            c1, c0 = dec.up(i, 1), dec.up(i, 0)
+            live = plan.runs[id(c1)]        # the gradient w.r.t. b is needed (pending is set only then)
             have = pending is not None
-            d_b = pending
-            if i in d_disp:
+            d_b, pending = pending, None
+            if i in d_disp and (live or plan.wgrad(dec.disp(i))):
                 dc = dec.disp(i)
                 disp = rec["disps"][i]
                 dpre = O.act_bwd_(d_disp[i].reshape(disp.shape).clone(), disp, O.ACT_DISP)
-                if plan.params:
-                    O.head_wgrad(b, dpre, g(dc.weight), dc.bias.grad)
+                if plan.wgrad(dc):
+                    O.head_wgrad(b, dpre, g(dc.weight), g(dc.bias))
+                if not live:
+                    continue
                 dpad = O.head_dgrad(dpre, dc.w_khwc(), b.shape)
                 if not have:
                     d_b = torch.empty_like(b)
@@ -740,19 +858,21 @@ class DispResNet(ArenaNet):
             elif have:
                 O.act_bwd_(d_b, b, O.ACT_ELU | cx.rnd())
             else:
-                continue            # nothing reaches this stage (cannot happen: stage 0 always has scale 0)
+                continue            # nothing reaches this stage, or nothing upstream of it trains
             # up(i,1): b = ELU(conv(reflect_pad(cat)))
-            c1 = dec.up(i, 1)
-            if plan.params:
-                cx.conv_wgrad(st["cat"], d_b, g(c1.weight), c1.bias.grad, 1, 1, O.PAD_REFLECT)
+            if plan.wgrad(c1):
+                cx.conv_wgrad(st["cat"], d_b, g(c1.weight), plan.grad_of(c1.bias), 1, 1, O.PAD_REFLECT)
+            if not plan.dgrad[id(c1)]:
+                continue
             dpad = cx.conv_dgrad(d_b, c1.w_op(cx), st["cat"].shape, 1, 1, None, padded_input=True)
-            d_a, d_skip = O.fold_upcat(dpad, st["a"].shape[-1], st["a"], O.ACT_ELU | cx.rnd())
+            d_a, d_skip = O.fold_upcat(dpad, st["a"].shape[-1], st["a"], O.ACT_ELU | cx.rnd(), with_skip=i > 0 and plan.feats[i - 1])
             if i > 0:
                 d_feats[i - 1] = d_skip
             # up(i,0): a = ELU(conv(reflect_pad(in0)))
-            c0 = dec.up(i, 0)
-            if plan.params:
-                cx.conv_wgrad(st["in0"], d_a, g(c0.weight), c0.bias.grad, 1, 1, O.PAD_REFLECT)
+            if plan.wgrad(c0):
+                cx.conv_wgrad(st["in0"], d_a, g(c0.weight), plan.grad_of(c0.bias), 1, 1, O.PAD_REFLECT)
+            if not plan.dgrad[id(c0)]:
+                continue
             dpad = cx.conv_dgrad(d_a, c0.w_op(cx), st["in0"].shape, 1, 1, None, padded_input=True)
             d_in = torch.empty_like(st["in0"])
             O.fold_plain(dpad, d_in, None, O.ACT_NONE, accumulate=False)
@@ -760,6 +880,8 @@ class DispResNet(ArenaNet):
                 pending = d_in          # = raw gradient of b_{i+1}; ELU' applied once all consumers are in
             else:
                 d_feats[4] = d_in
+        if not plan.feats[4]:
+            return [None] * len(plan.dimg)
         return encoder_backward(cx, self.encoder, rec["enc"], d_feats, plan)
 
 
@@ -783,13 +905,14 @@ class PoseResNet(ArenaNet):
         per = self._call((torch.cat([a for a, _ in pairs], 0), torch.cat([b for _, b in pairs], 0)), len(pairs))
         return [p[0] for p in per]
 
-    def _forward_impl(self, groups, img1, img2, fused=False):
-        """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs)."""
+    def _forward_impl(self, groups, img1, img2, fused=False, plan=None):
+        """fused (eval mode, autograd off): no record, BatchNorm in the convolution epilogues; returns (None, outputs).
+        Recording: plan (BackwardPlan) says which units' backward will run."""
         from . import lib as L
         img1, img2 = L.dev_f32(img1, "PoseResNet input"), L.dev_f32(img2, "PoseResNet input")
         self.refresh_operand_weights()
         cx = self.ctx
-        enc_rec, feats = encoder_forward(_Forward(self, groups, fused), self.encoder, (img1, img2))
+        enc_rec, feats = self._encoder_forward(groups, (img1, img2), fused, plan)
         x = feats[4]
         del feats                       # the fused forward frees f0-f3 here
         head = None if fused else [x]   # recording: the input of every head convolution, then the head's output
@@ -801,18 +924,20 @@ class PoseResNet(ArenaNet):
                             with_lo=fused and cx.split and k < 2)
             if head is not None:
                 head.append(x)
-        rec = None if fused else {"enc": enc_rec, "head": head, "training": self.training}
+        rec = None if fused else {"enc": enc_rec, "head": head, "plan": plan}
         return rec, [O.spatial_mean_fwd(x, 0.01)]
 
-    def _backward_impl(self, rec, grads, plan=TRAIN_PLAN):
+    def _backward_impl(self, rec, grads, plan):
         """Returns [gradient of img1 or None, gradient of img2 or None] (see encoder_backward)."""
         cx = self.ctx
         head = rec["head"]
         d = O.spatial_mean_bwd(grads[0], head[-1].shape, 0.01)
         for k in range(len(POSE_HEAD) - 1, -1, -1):
             conv, pad, inp = self.decoder.net[k], POSE_HEAD[k][0], head[k]
-            if plan.params:
-                cx.conv_wgrad(inp, d, ArenaNet.g(conv.weight), conv.bias.grad, 1, pad, O.PAD_ZERO)
+            if plan.wgrad(conv):
+                cx.conv_wgrad(inp, d, ArenaNet.g(conv.weight), plan.grad_of(conv.bias), 1, pad, O.PAD_ZERO)
+            if not plan.dgrad[id(conv)]:
+                return [None] * len(plan.dimg)
             d = cx.conv_dgrad(d, conv.w_op(cx), inp.shape, 1, pad)
             if k > 0:
                 O.act_bwd_(d, inp, _pose_act(cx, k - 1))       # inp is the output of convolution k - 1
@@ -828,13 +953,27 @@ class ArenaAdam:
     --num-scales 1, the scale 1-3 disparity heads) are left unchanged exactly as Adam skips
     `grad is None` parameters in the reference -- for weight_decay == 0 (the reference's scripts); with
     weight_decay > 0 the whole arena is decayed, those unused tensors included (documented deviation).  The step counter lives on the device so that the whole
-    training step can be captured in a CUDA graph."""
+    training step can be captured in a CUDA graph.  Frozen parameters (requires_grad False, whose .grad the networks keep
+    None) are skipped as torch.optim.Adam skips them: a network with any of them is updated by the masked kernel, which does
+    not touch their values, moments or operand mirror, weight decay included."""
 
     def __init__(self, nets, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
         self.nets = list(nets)
         self.lr, self.betas, self.eps, self.weight_decay = lr, betas, eps, weight_decay
         self.state = {}
         self._step = None
+        self._masks = {}           # id(net) -> (arena, requires_grad pattern, chunk mask on the device)
+
+    def _chunk_mask(self, n):
+        """None when every parameter of network n is trainable, else its adam_step_masked chunk mask (rebuilt when the
+        pattern or the arena changes; the warm-up step before a CUDA-graph capture builds it)."""
+        flags = tuple(p.requires_grad for p, _ in n._views)
+        if all(flags):
+            return None
+        hit = self._masks.get(id(n))
+        if hit is None or hit[0] is not n._flat or hit[1] != flags:
+            hit = self._masks[id(n)] = (n._flat, flags, O.chunk_mask([p.numel() for p, _ in n._views], flags, n._flat.device))
+        return hit[2]
 
     @property
     def step_count(self):
@@ -862,8 +1001,14 @@ class ArenaAdam:
             #                    the next step's gradient all-reduce; Trainer additionally checks that both were issued)
             m, v, _ = self.state[id(n)]
             mirror = n._flat_tf32 if n.ctx.tc else None
-            O.adam_step(n._flat, n._flat_grad, m, v, self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay,
-                        0, self._step, mirror, O.OPERAND_LO if n.ctx.split else O.OPERAND_TF32)
+            operand = O.OPERAND_LO if n.ctx.split else O.OPERAND_TF32
+            mask = self._chunk_mask(n)
+            if mask is None:
+                O.adam_step(n._flat, n._flat_grad, m, v, self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay,
+                            0, self._step, mirror, operand)
+            else:
+                O.adam_step_masked(n._flat, n._flat_grad, m, v, mask, self.lr, self.betas[0], self.betas[1], self.eps,
+                                   self.weight_decay, 0, self._step, mirror, operand)
             # the kernel writes through raw pointers (no torch version bump): with the mirror written the arena is in sync,
             # without it the next network call must re-round
             n._tf32_version = n._versions() if mirror is not None else None

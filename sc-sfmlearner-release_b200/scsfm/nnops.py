@@ -86,6 +86,7 @@ def _lib():
         lib.scsfm_spatial_mean_fwd.argtypes = [P, I, I, I, F, P, P]
         lib.scsfm_spatial_mean_bwd.argtypes = [P, I, I, I, F, P, P]
         lib.scsfm_adam_step.argtypes = [P, P, P, P, LL, F, F, F, F, F, I, P, P, I, P]
+        lib.scsfm_adam_step_masked.argtypes = [P, P, P, P, LL, P, F, F, F, F, F, I, P, P, I, P]
         _bound = True
     return lib
 
@@ -566,13 +567,14 @@ def fold_plain(dpad, d, act_out, act, accumulate):
              L.ptr(act_out), act, 1 if accumulate else 0, None, L.stream())
 
 
-def fold_upcat(dpad, C1, lo_act, act):
+def fold_upcat(dpad, C1, lo_act, act, with_skip=True):
+    """Gradient of the upsampled part (d_lo) and, with_skip, of the skip part (d_skip; None without) of a concatenation."""
     B, Hp, Wp, Ct = dpad.shape
     H, W, C2 = Hp - 2, Wp - 2, Ct - C1
     d_lo = empty((B, H // 2, W // 2, C1), dpad)
-    d_skip = empty((B, H, W, C2), dpad) if C2 > 0 else None
-    L.launch(_lib().scsfm_fold_bwd, "scsfm_fold_bwd", "fold", 2 if C2 > 0 else 1, 4.0 * dpad.numel(), L.ptr(dpad), B, H, W, C1, C2, 1,
-             L.ptr(d_lo), L.ptr(lo_act), act, 0, L.ptr(d_skip), L.stream())
+    d_skip = empty((B, H, W, C2), dpad) if C2 > 0 and with_skip else None
+    L.launch(_lib().scsfm_fold_bwd, "scsfm_fold_bwd", "fold", 2 if d_skip is not None else 1, 4.0 * dpad.numel(), L.ptr(dpad), B, H, W, C1,
+             C2, 1, L.ptr(d_lo), L.ptr(lo_act), act, 0, L.ptr(d_skip), L.stream())
     return d_lo, d_skip
 
 
@@ -600,3 +602,26 @@ def adam_step(param, grad, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, weight_de
     L.launch(_lib().scsfm_adam_step, "scsfm_adam_step", "adam", 1, (32.0 if mirror is not None else 28.0) * param.numel(), L.ptr(param),
              L.ptr(grad), L.ptr(exp_avg), L.ptr(exp_avg_sq), param.numel(), lr, beta1, beta2, eps, weight_decay, step, L.ptr(step_dev),
              L.ptr(mirror), mirror_operand, L.stream())
+
+
+def adam_step_masked(param, grad, exp_avg, exp_avg_sq, chunk_mask, lr, beta1, beta2, eps, weight_decay, step, step_dev=None,
+                     mirror=None, mirror_operand=OPERAND_TF32):
+    """adam_step over the chunks of 64 floats whose chunk_mask byte (uint8 [ceil(n / 64)], see chunk_mask()) is nonzero; the
+    others -- frozen parameters -- are not touched at all."""
+    if chunk_mask.dtype != torch.uint8 or chunk_mask.numel() != (param.numel() + 63) // 64:
+        raise ValueError("adam_step_masked: chunk_mask must be uint8 with ceil(n / 64) = %d entries" % ((param.numel() + 63) // 64))
+    L.launch(_lib().scsfm_adam_step_masked, "scsfm_adam_step_masked", "adam", 1, (32.0 if mirror is not None else 28.0) * param.numel(),
+             L.ptr(param), L.ptr(grad), L.ptr(exp_avg), L.ptr(exp_avg_sq), param.numel(), L.ptr(chunk_mask), lr, beta1, beta2, eps,
+             weight_decay, step, L.ptr(step_dev), L.ptr(mirror), mirror_operand, L.stream())
+
+
+def chunk_mask(sizes, trainable, device):
+    """uint8 mask of adam_step_masked for an arena that packs tensors of `sizes` elements at aligned64 offsets: 1 on the chunks of
+    the tensors flagged in `trainable`."""
+    mask = torch.zeros(sum(aligned64(n) for n in sizes) // 64, dtype=torch.uint8)
+    off = 0
+    for n, t in zip(sizes, trainable):
+        if t:
+            mask[off // 64:(off + aligned64(n)) // 64] = 1
+        off += aligned64(n)
+    return mask.to(device)

@@ -2,6 +2,9 @@
 H100, and its data-parallel form: one process per GPU, each rank runs the complete step on its shard of
 the batch, the two gradient arenas are all-reduced (NCCL over NVLink) as soon as the backward of the
 owning network has finished, then every rank applies the identical fused Adam update.
+
+Fine-tuning: parameters may be frozen (requires_grad False) and BatchNorm modules put in eval mode, per module, before the
+first step (or before capture()); the step then skips their gradients and updates, and capture() refuses a later change.
 """
 import torch
 import torch.distributed as dist
@@ -109,6 +112,9 @@ class Trainer:
         """train.py:259-282 without a single host synchronisation; returns device scalars
         (loss, photo, smooth, geometry).  After `capture()` the step is one CUDA-graph replay."""
         if self._graph is not None:
+            if self._flag_patterns() != self._captured_flags:
+                raise RuntimeError("the requires_grad / train-eval pattern of the networks changed after capture(): the captured "
+                                   "step computes the old one (drop_graph() and capture() again)")
             self._static[0].copy_(tgt_img, non_blocking=True)
             for dst, src in zip(self._static[1], ref_imgs):
                 dst.copy_(src, non_blocking=True)
@@ -150,7 +156,12 @@ class Trainer:
             self._static_out = torch.stack(self._eager_step(*self._static))
         self.launches_per_step = L.launch_count() - before
         self._graph = graph
+        self._captured_flags = self._flag_patterns()
         L.PROF.update(prof)
+
+    def _flag_patterns(self):
+        """What a captured step depends on beyond its inputs: which parameters are frozen and which modules are in eval mode."""
+        return self.disp_net.flag_pattern(), self.pose_net.flag_pattern()
 
     def drop_graph(self):
         """Forget a captured graph: later steps run eagerly."""
