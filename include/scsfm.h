@@ -119,6 +119,18 @@ int scsfm_inverse_warp2_bwd(const float* img, const float* depth, const float* r
                             float* grad_depth, float* grad_ref_depth, float* grad_pose, void* scratch_12B_doubles,
                             void* stream);
 
+/* Gradients with respect to the camera intrinsics (learned / self-calibrated K; reference inverse_warp.py:253,258 differentiate
+ * K through intrinsics.inverse() and intrinsics @ pose_mat).  Both run after the matching backward on the same stream and read
+ * the per-(job, sample) sums d(loss)/d(K [R|t]) it left behind; d(loss)/dK follows from them in closed form, in fp64, with no
+ * per-pixel work.  The result is ADDED into grad_intrinsics [B,3,3] (fp32); one thread per entry sums the jobs in order, so
+ * the result is deterministic given the sums.
+ *   scsfm_pairwise_intrinsics_grad: after scsfm_pairwise_bwd, with the same jobs, intrinsics and stats.
+ *   scsfm_inverse_warp2_intrinsics_grad: after scsfm_inverse_warp2_bwd, with the same pose, intrinsics and scratch. */
+int scsfm_pairwise_intrinsics_grad(const ScsfmPairJob* jobs_host, int njobs, const float* intrinsics, int B, const void* stats,
+                                   float* grad_intrinsics, void* stream);
+int scsfm_inverse_warp2_intrinsics_grad(const float* pose, const float* intrinsics, int B, const void* scratch_12B_doubles,
+                                        float* grad_intrinsics, void* stream);
+
 /* pose_vec2mat (reference inverse_warp.py:139-154): [B,6] -> [B,3,4]; rotation_mode 0 = euler, 1 = quat. */
 int scsfm_pose_vec2mat(const float* vec, int B, int rotation_mode, float* out, void* stream);
 

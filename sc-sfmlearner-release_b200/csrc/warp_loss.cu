@@ -590,6 +590,60 @@ __global__ void inverse_warp2_pose_grad_kernel(const float* __restrict__ pose, c
     pose_grad_from_gM(Kmat + b * 9, pose + b * 6, gM_all + (size_t)b * 12, g_pose + b * 6);
 }
 
+// ---------------------------------------------------------------------------------------------
+// intrinsics gradient (camera self-calibration), from the same d(K [R|t]) sums as the pose gradient
+// ---------------------------------------------------------------------------------------------
+// Entry (r, c) of d(loss)/dK for one (job, sample), in fp64.  Per pixel c_px = K^-1 (D pix) and P = M3 c_px + m4 with
+// M = [M3 | m4] = K [R|t]; gM = sum_px dL/dP [c_px^T 1].  K enters twice (reference inverse_warp.py:253,258):
+//   through M:     gM3 R^T + gm4 t^T
+//   through K^-1:  -K^-T (dL/dK^-1) K^-T with dL/dK^-1 = M3^T sum_px dL/dP (D pix)^T = M3^T gM3 K^T,  i.e.  -K^-T R^T K^T gM3
+// The two terms cancel to a large part (exactly at R = I, t = 0), hence fp64 throughout.  K^-1 is the general 3x3 inverse.
+__device__ inline double intrinsics_grad_entry(const float* __restrict__ Kf, const float* __restrict__ pose, const double* gM,
+                                               int r, int c) {
+    double k[9];
+    for (int i = 0; i < 9; ++i) k[i] = Kf[i];
+    const double A = k[4] * k[8] - k[5] * k[7], Bc = k[5] * k[6] - k[3] * k[8], C = k[3] * k[7] - k[4] * k[6];
+    const double inv = 1.0 / (k[0] * A + k[1] * Bc + k[2] * C);
+    const double kinv[9] = {A * inv, (k[2] * k[7] - k[1] * k[8]) * inv, (k[1] * k[5] - k[2] * k[4]) * inv,
+                            Bc * inv, (k[0] * k[8] - k[2] * k[6]) * inv, (k[2] * k[3] - k[0] * k[5]) * inv,
+                            C * inv, (k[1] * k[6] - k[0] * k[7]) * inv, (k[0] * k[4] - k[1] * k[3]) * inv};
+    const double sx = sin((double)pose[3]), cx = cos((double)pose[3]), sy = sin((double)pose[4]), cy = cos((double)pose[4]);
+    const double sz = sin((double)pose[5]), cz = cos((double)pose[5]);
+    const double R[9] = {cy * cz, -cy * sz, sy,
+                         cx * sz + sx * sy * cz, cx * cz - sx * sy * sz, -sx * cy,
+                         sx * sz - cx * sy * cz, sx * cz + cx * sy * sz, cx * cy};
+    // through M = K [R|t]
+    double through_m = gM[r * 4 + 3] * (double)pose[c];
+    for (int j = 0; j < 3; ++j) through_m += gM[r * 4 + j] * R[c * 3 + j];
+    // column c of K^T gM3, then of R^T K^T gM3, then entry r of K^-T R^T K^T gM3
+    double a[3], bcol[3];
+    for (int j = 0; j < 3; ++j) a[j] = k[0 * 3 + j] * gM[0 * 4 + c] + k[1 * 3 + j] * gM[1 * 4 + c] + k[2 * 3 + j] * gM[2 * 4 + c];
+    for (int i = 0; i < 3; ++i) bcol[i] = R[0 * 3 + i] * a[0] + R[1 * 3 + i] * a[1] + R[2 * 3 + i] * a[2];
+    const double through_kinv = kinv[0 * 3 + r] * bcol[0] + kinv[1 * 3 + r] * bcol[1] + kinv[2 * 3 + r] * bcol[2];
+    return through_m - through_kinv;
+}
+
+// One thread per (sample, entry of K): sums the jobs in their order and adds the result into grad_K (no atomics: the chunks of
+// one backward are launched one after the other on one stream).
+__global__ void pairwise_intrinsics_grad_kernel(PairJobs jobs, int njobs, const float* __restrict__ Kmat, int B,
+                                                const double* __restrict__ gM_all, float* __restrict__ grad_K) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * 9) return;
+    const int b = i / 9, e = i - b * 9;
+    double s = 0.0;
+    for (int job = 0; job < njobs; ++job)
+        s += intrinsics_grad_entry(Kmat + b * 9, jobs.j[job].pose + b * 6, gM_all + ((size_t)job * B + b) * 12, e / 3, e % 3);
+    grad_K[i] += (float)s;
+}
+
+__global__ void inverse_warp2_intrinsics_grad_kernel(const float* __restrict__ pose, const float* __restrict__ Kmat, int B,
+                                                     const double* __restrict__ gM_all, float* __restrict__ grad_K) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * 9) return;
+    const int b = i / 9, e = i - b * 9;
+    grad_K[i] += (float)intrinsics_grad_entry(Kmat + b * 9, pose + b * 6, gM_all + (size_t)b * 12, e / 3, e % 3);
+}
+
 __global__ void pose_vec2mat_kernel(const float* __restrict__ vec, int B, int mode, float* __restrict__ out) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
@@ -720,6 +774,35 @@ extern "C" int scsfm_inverse_warp2_bwd(const float* img, const float* depth, con
         inverse_warp2_pose_grad_kernel<<<(B + 63) / 64, 64, 0, st>>>(pose, intrinsics, B, (const double*)scratch, grad_pose);
         SCSFM_CHECK_LAUNCH();
     }
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_pairwise_intrinsics_grad(const ScsfmPairJob* jobs_host, int njobs, const float* intrinsics, int B,
+                                              const void* stats, float* grad_intrinsics, void* stream) {
+    SCSFM_CHECK_ARG(jobs_host != nullptr && njobs >= 1 && njobs <= SCSFM_MAX_JOBS,
+                    "pairwise_intrinsics_grad: njobs must be in [1,%d], got %d", SCSFM_MAX_JOBS, njobs);
+    SCSFM_CHECK_ARG(B >= 1 && (long long)njobs * B <= 65535, "pairwise_intrinsics_grad: wrong batch size B=%d", B);
+    SCSFM_CHECK_ARG(intrinsics && stats && grad_intrinsics, "pairwise_intrinsics_grad: null intrinsics/stats/grad_intrinsics");
+    PairJobs pj;
+    memset(&pj, 0, sizeof(pj));
+    for (int i = 0; i < njobs; ++i) {
+        SCSFM_CHECK_ARG(jobs_host[i].pose != nullptr, "pairwise_intrinsics_grad: job %d has a null pose", i);
+        pj.j[i] = jobs_host[i];
+    }
+    const double* gM = (const double*)stats + (size_t)njobs * STATS_PER_JOB;
+    pairwise_intrinsics_grad_kernel<<<(B * 9 + 127) / 128, 128, 0, (cudaStream_t)stream>>>(pj, njobs, intrinsics, B, gM,
+                                                                                            grad_intrinsics);
+    SCSFM_CHECK_LAUNCH();
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_inverse_warp2_intrinsics_grad(const float* pose, const float* intrinsics, int B, const void* scratch,
+                                                   float* grad_intrinsics, void* stream) {
+    SCSFM_CHECK_ARG(pose && intrinsics && scratch && grad_intrinsics, "inverse_warp2_intrinsics_grad: null input");
+    SCSFM_CHECK_ARG(B >= 1 && B <= 65535, "inverse_warp2_intrinsics_grad: wrong batch size B=%d", B);
+    inverse_warp2_intrinsics_grad_kernel<<<(B * 9 + 127) / 128, 128, 0, (cudaStream_t)stream>>>(pose, intrinsics, B,
+                                                                                                 (const double*)scratch, grad_intrinsics);
+    SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
 

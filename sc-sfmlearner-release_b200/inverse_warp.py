@@ -99,7 +99,7 @@ def inverse_warp2(img, depth, ref_depth, pose, intrinsics, padding_mode="zeros")
 
     img [B,3,H,W], depth / ref_depth [B,1,H,W], pose [B,6], intrinsics [B,3,3] ->
     (projected_img, valid_mask, projected_depth, computed_depth).  Differentiable w.r.t.
-    depth, ref_depth and pose through a hand-written backward kernel.
+    depth, ref_depth, pose and intrinsics through hand-written backward kernels.
     """
     check_sizes(img, "img", "B3HW")
     check_sizes(depth, "depth", "B1HW")

@@ -63,6 +63,8 @@ def load():
     lib.scsfm_pairwise_bwd.argtypes = [ctypes.POINTER(PairJob), I, P, I, I, I, I, I, P, P, P]
     lib.scsfm_inverse_warp2_fwd.argtypes = [P, P, P, P, P, I, I, I, I, P, P, P, P, P]
     lib.scsfm_inverse_warp2_bwd.argtypes = [P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P, P]
+    lib.scsfm_pairwise_intrinsics_grad.argtypes = [ctypes.POINTER(PairJob), I, P, I, P, P, P]
+    lib.scsfm_inverse_warp2_intrinsics_grad.argtypes = [P, P, I, P, P, P]
     lib.scsfm_pose_vec2mat.argtypes = [P, I, I, P, P]
     lib.scsfm_smooth_fwd.argtypes = [ctypes.POINTER(SmoothJob), I, I, I, I, P, P, P]
     lib.scsfm_smooth_bwd.argtypes = [ctypes.POINTER(SmoothJob), I, I, I, I, P, P, P]

@@ -137,12 +137,17 @@ class PhotoGeoLoss(torch.autograd.Function):
                 grads[key] = torch.zeros_like(t)
         gout = torch.stack([g_photo, g_geo]).to(torch.float32).contiguous()
         jobs = PhotoGeoLoss._jobs(cfg, tgt_img, ref_imgs, tgt_depth, ref_depths, poses, poses_inv, grads)
+        # learned intrinsics: d(loss)/dK from the d(K [R|t]) sums each chunk's backward leaves in its stats, added chunk by chunk
+        g_K = torch.zeros(B, 3, 3, device=tgt_img.device, dtype=torch.float32) if ctx.needs_input_grad[2] else None
         for k, c0 in enumerate(range(0, len(jobs), L.MAX_JOBS)):
             chunk = jobs[c0:c0 + L.MAX_JOBS]
             arr = (L.PairJob * len(chunk))(*chunk)
             L.launch(lib.scsfm_pairwise_bwd, "scsfm_pairwise_bwd", "pair_bwd", 2, 44.0 * len(chunk) * B * H * W, arr, len(chunk),
                      L.ptr(intrinsics), B, H, W, flags, padding, L.ptr(ctx.stats[k]), L.ptr(gout), L.stream())
-        return (None, None, None) + tuple(grads.get(k) if k is not None else None for k in order)
+            if g_K is not None:
+                L.launch(lib.scsfm_pairwise_intrinsics_grad, "scsfm_pairwise_intrinsics_grad", "pair_bwd", 1, 0.0, arr, len(chunk),
+                         L.ptr(intrinsics), B, L.ptr(ctx.stats[k]), L.ptr(g_K), L.stream())
+        return (None, None, g_K) + tuple(grads.get(k) if k is not None else None for k in order)
 
 
 def photo_and_geometry_loss(tgt_img, ref_imgs, intrinsics, tgt_depth, ref_depths, poses, poses_inv, max_scales,
@@ -275,7 +280,12 @@ class InverseWarp2(torch.autograd.Function):
                                             B, H, W, ctx.padding, L.ptr(g_warped), L.ptr(g_proj), L.ptr(g_comp),
                                             L.ptr(g_depth), L.ptr(g_ref), L.ptr(g_pose), L.ptr(scratch), L.stream()),
                 "scsfm_inverse_warp2_bwd")
-        return None, g_depth, g_ref, g_pose, None, None
+        g_K = None
+        if ctx.needs_input_grad[4]:
+            g_K = torch.zeros(B, 3, 3, device=img.device, dtype=torch.float32)
+            L.check(lib.scsfm_inverse_warp2_intrinsics_grad(L.ptr(pose), L.ptr(intrinsics), B, L.ptr(scratch), L.ptr(g_K),
+                                                            L.stream()), "scsfm_inverse_warp2_intrinsics_grad")
+        return None, g_depth, g_ref, g_pose, g_K, None
 
 
 def pose_vec2mat(vec, rotation_mode="euler"):

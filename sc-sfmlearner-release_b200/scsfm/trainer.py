@@ -110,7 +110,11 @@ class Trainer:
 
     def step(self, tgt_img, ref_imgs, intrinsics):
         """train.py:259-282 without a single host synchronisation; returns device scalars
-        (loss, photo, smooth, geometry).  After `capture()` the step is one CUDA-graph replay."""
+        (loss, photo, smooth, geometry).  After `capture()` the step is one CUDA-graph replay.
+
+        Intrinsics that require a gradient (a learned / self-calibrated K) get it in an eager single-GPU step, accumulated
+        into their .grad as in the reference loop; updating them is left to the caller's own optimizer."""
+        self._check_intrinsics(intrinsics)
         if self._graph is not None:
             if self._flag_patterns() != self._captured_flags:
                 raise RuntimeError("the requires_grad / train-eval pattern of the networks changed after capture(): the captured "
@@ -131,7 +135,8 @@ class Trainer:
         if self.exchange is not None and not allow_distributed:
             raise RuntimeError("graph capture of the data-parallel step is opt-in (allow_distributed=True): capturing the NCCL "
                                "all-reduce on the side stream has not been validated on this pod yet")
-        self._static = (tgt_img.clone(), [r.clone() for r in ref_imgs], intrinsics.clone())
+        self._check_intrinsics(intrinsics, capturing=True)
+        self._static =(tgt_img.clone(), [r.clone() for r in ref_imgs], intrinsics.clone())
         snap = self.optimizer.snapshot()
         prof = dict(L.PROF)
         L.PROF.update(enabled=False)
@@ -158,6 +163,19 @@ class Trainer:
         self._graph = graph
         self._captured_flags = self._flag_patterns()
         L.PROF.update(prof)
+
+    def _check_intrinsics(self, intrinsics, capturing=False):
+        """Learned intrinsics are supported by the eager single-GPU step only; elsewhere their gradient would be lost."""
+        if not (torch.is_grad_enabled() and intrinsics.requires_grad):
+            return
+        if capturing or self._graph is not None:
+            raise RuntimeError("intrinsics that require a gradient cannot go through a captured step: the graph works on a "
+                               "static copy of K, so its gradient would never reach the caller's tensor (drop_graph() and "
+                               "step eagerly, or pass intrinsics.detach())")
+        if self.exchange is not None:
+            raise RuntimeError("intrinsics that require a gradient are not supported by the data-parallel step: only the two "
+                               "networks' gradients are all-reduced, so the per-rank gradients of K would silently diverge "
+                               "(pass intrinsics.detach())")
 
     def _flag_patterns(self):
         """What a captured step depends on beyond its inputs: which parameters are frozen and which modules are in eval mode."""
