@@ -440,10 +440,21 @@ int scsfm_adam_step_masked(float* param, const float* grad, float* exp_avg, floa
  *     reference's intrinsics update (custom_transforms.py:56-57, 74-75, 83-84) on a float32 matrix: with theta equal to a
  *     dataset's K, bit for bit the K the augmentation hands out.
  *   scsfm_camera_grad: ADDS d(loss)/dtheta = sum_b dK_b/dtheta . dK[b] into dtheta [4] (fp32).  One CTA, fp64 sums in a fixed
- *     order, no atomics: deterministic. */
+ *     order, no atomics: deterministic.
+ * A bank of cameras (one per calibration or per scene of a multi-camera dataset): theta [n_cams, 4] and one camera index per
+ * sample, idx [B] (int32).
+ *   scsfm_camera_build_indexed: K_out[b] = theta[idx[b]] seen through record b, as above; an index outside [0, n_cams) gives
+ *     nine NaNs in K_out[b] and reads nothing out of bounds.
+ *   scsfm_camera_grad_indexed: ADDS into dtheta [n_cams, 4] the gradient of each camera, summed over the samples that use it
+ *     (none from an out-of-range index).  One CTA per camera, each with the fixed-order fp64 sum above: deterministic.
+ * scsfm_camera_build / scsfm_camera_grad are the n_cams = 1 calls of the same kernels with every sample on camera 0. */
 #define SCSFM_CAMERA_AUG_DOUBLES 6
 int scsfm_camera_build(const float* theta, const double* aug, int B, float* K_out, void* stream);
 int scsfm_camera_grad(const double* aug, const float* dK, int B, float* dtheta, void* stream);
+int scsfm_camera_build_indexed(const float* theta, int n_cams, const double* aug, const int* idx, int B, float* K_out,
+                               void* stream);
+int scsfm_camera_grad_indexed(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta,
+                              void* stream);
 
 #ifdef __cplusplus
 }

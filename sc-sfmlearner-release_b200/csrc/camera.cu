@@ -8,39 +8,56 @@
 //    (a float32 row times a float64 scalar).  With theta equal to the dataset's K the result is GpuAugment's K bit for bit;
 //  * scsfm_camera_grad is the chain rule through that map (roundings taken as identity): each entry of K_b is an affine function
 //    of one parameter, so d(loss)/dtheta = sum_b of four scaled entries of dK_b.  One CTA sums them in fp64 in a fixed order.
+// A multi-camera dataset (one calibration per KITTI raw recording day, one camera per uncalibrated video) learns a bank of cameras
+// theta [n_cams, 4]; sample b then sees camera idx[b] (scsfm_camera_*_indexed).  Both kernels take the index: the build reads
+// theta + 4 idx[b], the gradient runs one CTA per camera over the samples that use it.  The single-camera entries are the
+// n_cams = 1 calls with a null index (every sample on camera 0), with the same arithmetic as before.
 #include "common.cuh"
 
 namespace scsfm {
 
 constexpr int CAM_GRAD_THREADS = 256;
 
-__global__ void camera_build_kernel(const float* __restrict__ theta, const double* __restrict__ aug, int B, float* __restrict__ K) {
+// sample b sees camera idx[b] (camera 0 for every sample when idx is null); an index outside [0, n_cams) gives a NaN K, and
+// theta is never read out of bounds
+__global__ void camera_build_kernel(const float* __restrict__ theta, int n_cams, const double* __restrict__ aug,
+                                    const int* __restrict__ idx, int B, float* __restrict__ K) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
+    float* k = K + (size_t)b * 9;
+    const int c = idx ? idx[b] : 0;
+    if (c < 0 || c >= n_cams) {
+#pragma unroll
+        for (int i = 0; i < 9; ++i) k[i] = __int_as_float(0x7fc00000);
+        return;
+    }
+    const float* th = theta + (size_t)c * 4;
     const double* a = aug + (size_t)b * SCSFM_CAMERA_AUG_DOUBLES;
     const double xs = a[0], ys = a[1];
-    float cx = theta[2];
+    float cx = th[2];
     if (a[2] != 0.0) cx = __fsub_rn((float)a[5], cx);                        // K[0, 2] = in_w - K[0, 2]
-    float* k = K + (size_t)b * 9;
-    k[0] = __double2float_rn(__dmul_rn((double)theta[0], xs));              // K[0] *= x_scaling
+    k[0] = __double2float_rn(__dmul_rn((double)th[0], xs));                 // K[0] *= x_scaling
     k[1] = 0.f;                                                              // zero skew (0 * x_scaling)
     k[2] = __fsub_rn(__double2float_rn(__dmul_rn((double)cx, xs)), (float)a[3]);          // ... then K[0, 2] -= offset_x
     k[3] = 0.f;
-    k[4] = __double2float_rn(__dmul_rn((double)theta[1], ys));              // K[1] *= y_scaling
-    k[5] = __fsub_rn(__double2float_rn(__dmul_rn((double)theta[3], ys)), (float)a[4]);    // ... then K[1, 2] -= offset_y
+    k[4] = __double2float_rn(__dmul_rn((double)th[1], ys));                 // K[1] *= y_scaling
+    k[5] = __fsub_rn(__double2float_rn(__dmul_rn((double)th[3], ys)), (float)a[4]);       // ... then K[1, 2] -= offset_y
     k[6] = 0.f;
     k[7] = 0.f;
     k[8] = 1.f;
 }
 
-// dtheta += sum_b (x_scale dK00, y_scale dK11, +-x_scale dK02, y_scale dK12): thread t sums samples t, t + 256, ... in order,
-// then a fixed shared-memory tree; no atomics, so two runs give the same bits
+// dtheta[c] += sum over the samples b with idx[b] == c of (x_scale dK00, y_scale dK11, +-x_scale dK02, y_scale dK12); one CTA
+// per camera (gridDim.x = n_cams), a null idx puts every sample on camera 0 and an out-of-range index on none.  Thread t sums
+// samples t, t + 256, ... in order, then a fixed shared-memory tree; no atomics, so two runs give the same bits
 __global__ void __launch_bounds__(CAM_GRAD_THREADS)
-camera_grad_kernel(const double* __restrict__ aug, const float* __restrict__ dK, int B, float* __restrict__ dtheta) {
+camera_grad_kernel(const double* __restrict__ aug, const int* __restrict__ idx, const float* __restrict__ dK, int B,
+                   float* __restrict__ dtheta) {
     __shared__ double red[4][CAM_GRAD_THREADS];
-    const int t = threadIdx.x;
+    const int t = threadIdx.x, c = blockIdx.x;
     double s[4] = {0.0, 0.0, 0.0, 0.0};
     for (int b = t; b < B; b += CAM_GRAD_THREADS) {
+        if ((idx ? idx[b] : 0) != c) continue;
         const double* a = aug + (size_t)b * SCSFM_CAMERA_AUG_DOUBLES;
         const float* g = dK + (size_t)b * 9;
         const double xs = a[0], ys = a[1];
@@ -59,17 +76,26 @@ camera_grad_kernel(const double* __restrict__ aug, const float* __restrict__ dK,
         }
         __syncthreads();
     }
-    if (t < 4) dtheta[t] = __fadd_rn(dtheta[t], (float)red[t][0]);
+    float* d = dtheta + (size_t)c * 4;
+    if (t < 4) d[t] = __fadd_rn(d[t], (float)red[t][0]);
 }
 
 }  // namespace scsfm
 
 using namespace scsfm;
 
+static void launch_build(const float* theta, int n_cams, const double* aug, const int* idx, int B, float* K_out, void* stream) {
+    camera_build_kernel<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(theta, n_cams, aug, idx, B, K_out);
+}
+
+static void launch_grad(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta, void* stream) {
+    camera_grad_kernel<<<n_cams, CAM_GRAD_THREADS, 0, (cudaStream_t)stream>>>(aug, idx, dK, B, dtheta);
+}
+
 extern "C" int scsfm_camera_build(const float* theta, const double* aug, int B, float* K_out, void* stream) {
     SCSFM_CHECK_ARG(theta && aug && K_out, "camera_build: null pointer (theta, aug and K_out are required)");
     SCSFM_CHECK_ARG(B > 0, "camera_build: batch size must be positive, got %d", B);
-    camera_build_kernel<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(theta, aug, B, K_out);
+    launch_build(theta, 1, aug, nullptr, B, K_out, stream);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
@@ -77,7 +103,27 @@ extern "C" int scsfm_camera_build(const float* theta, const double* aug, int B, 
 extern "C" int scsfm_camera_grad(const double* aug, const float* dK, int B, float* dtheta, void* stream) {
     SCSFM_CHECK_ARG(aug && dK && dtheta, "camera_grad: null pointer (aug, dK and dtheta are required)");
     SCSFM_CHECK_ARG(B > 0, "camera_grad: batch size must be positive, got %d", B);
-    camera_grad_kernel<<<1, CAM_GRAD_THREADS, 0, (cudaStream_t)stream>>>(aug, dK, B, dtheta);
+    launch_grad(aug, nullptr, dK, B, 1, dtheta, stream);
+    SCSFM_CHECK_LAUNCH();
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_camera_build_indexed(const float* theta, int n_cams, const double* aug, const int* idx, int B, float* K_out,
+                                          void* stream) {
+    SCSFM_CHECK_ARG(theta && aug && idx && K_out, "camera_build_indexed: null pointer (theta, aug, idx and K_out are required)");
+    SCSFM_CHECK_ARG(n_cams > 0, "camera_build_indexed: number of cameras must be positive, got %d", n_cams);
+    SCSFM_CHECK_ARG(B > 0, "camera_build_indexed: batch size must be positive, got %d", B);
+    launch_build(theta, n_cams, aug, idx, B, K_out, stream);
+    SCSFM_CHECK_LAUNCH();
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_camera_grad_indexed(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta,
+                                         void* stream) {
+    SCSFM_CHECK_ARG(aug && idx && dK && dtheta, "camera_grad_indexed: null pointer (aug, idx, dK and dtheta are required)");
+    SCSFM_CHECK_ARG(B > 0, "camera_grad_indexed: batch size must be positive, got %d", B);
+    SCSFM_CHECK_ARG(n_cams > 0, "camera_grad_indexed: number of cameras must be positive, got %d", n_cams);
+    launch_grad(aug, idx, dK, B, n_cams, dtheta, stream);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }

@@ -5,6 +5,10 @@ the GPU transforms every sample is flipped, zoomed and cropped (custom_transform
 one per sample: K_b = aug_b(theta).  `records()` turns the random draws of a batch into device records; `LearnedCamera(records)`
 builds the batch's K with the augmentation's own arithmetic and back-propagates into theta in one small deterministic kernel.
 The K it returns feeds the loss entry points unchanged (their intrinsics gradient supplies dK).
+
+A dataset recorded with several cameras (KITTI raw: one calibration per recording day; Cityscapes: one per sequence; uncalibrated
+video: one per clip) learns a bank of cameras instead: `LearnedCamera.bank(thetas [C,4], ...)` holds theta [C,4], and
+`forward(aug, index)` gives sample b the view of camera index[b] through its own record (scsfm_camera_*_indexed).
 """
 import ctypes
 
@@ -25,6 +29,8 @@ def _lib():
         P, I = ctypes.c_void_p, ctypes.c_int
         lib.scsfm_camera_build.argtypes = [P, P, I, P, P]
         lib.scsfm_camera_grad.argtypes = [P, P, I, P, P]
+        lib.scsfm_camera_build_indexed.argtypes = [P, I, P, P, I, P, P]
+        lib.scsfm_camera_grad_indexed.argtypes = [P, P, P, I, I, P, P]
         _bound = True
     return lib
 
@@ -55,56 +61,87 @@ def identity_records(B, in_w, device="cuda"):
     return r.to(device)
 
 
-def _check(theta, aug):
+def _check(theta, aug, index=None):
+    """Types, shapes and devices of a call, checked before any launch.  theta [4] takes no index, theta [C,4] requires one:
+    int32 or int64 [B] on the GPU.  Returns the index as int32 (or None)."""
     if not (theta.is_cuda and aug.is_cuda):
         raise RuntimeError("the learned camera runs on the GPU: theta and the augmentation records must be CUDA tensors "
                            "(there is no CPU fallback)")
-    if theta.dtype != torch.float32 or theta.shape != (4,):
-        raise TypeError("theta must be float32 [4] (fx, fy, cx, cy), got %s %s" % (theta.dtype, tuple(theta.shape)))
+    if theta.dtype != torch.float32 or not (theta.shape == (4,) or (theta.dim() == 2 and theta.shape[1] == 4 and theta.shape[0] >= 1)):
+        raise TypeError("theta must be float32 [4] (fx, fy, cx, cy) or [C,4] (a bank of C cameras), got %s %s"
+                        % (theta.dtype, tuple(theta.shape)))
     if aug.dtype != torch.float64 or aug.dim() != 2 or aug.shape[1] != AUG_DOUBLES or aug.shape[0] < 1:
         raise TypeError("augmentation records must be float64 [B, %d] (scsfm.camera.records), got %s %s"
                         % (AUG_DOUBLES, aug.dtype, tuple(aug.shape)))
+    if theta.dim() == 1:
+        if index is not None:
+            raise TypeError("a camera index is for a bank of cameras (theta [C,4]); this camera has theta [4]")
+        return None
+    if index is None:
+        raise TypeError("a bank of %d cameras needs the camera index of every sample (index: int32 or int64 [%d] CUDA tensor)"
+                        % (theta.shape[0], aug.shape[0]))
+    if not isinstance(index, torch.Tensor) or index.dtype not in (torch.int32, torch.int64) or tuple(index.shape) != (aug.shape[0],):
+        raise TypeError("camera index must be an int32 or int64 tensor [%d], got %s" % (
+            aug.shape[0], "%s %s" % (index.dtype, tuple(index.shape)) if isinstance(index, torch.Tensor) else type(index).__name__))
+    if not index.is_cuda or index.device != theta.device:
+        raise RuntimeError("camera index must be on the camera's device %s, got %s" % (theta.device, index.device))
+    return index.to(torch.int32).contiguous()
 
 
-def build(theta, aug):
-    """K [B,3,3] float32 of theta through every record (no autograd)."""
-    _check(theta, aug)
+def build(theta, aug, index=None):
+    """K [B,3,3] float32 of theta through every record (no autograd).  theta [C,4] with index [B]: sample b sees camera index[b]
+    (an index outside [0, C) gives a NaN K)."""
+    index = _check(theta, aug, index)
     theta, aug = theta.detach().contiguous(), aug.contiguous()
     K = torch.empty(aug.shape[0], 3, 3, device=theta.device, dtype=torch.float32)
-    L.launch(_lib().scsfm_camera_build, "scsfm_camera_build", "camera", 1, 0.0, L.ptr(theta), L.ptr(aug), aug.shape[0], L.ptr(K),
-             L.stream())
+    if index is None:
+        L.launch(_lib().scsfm_camera_build, "scsfm_camera_build", "camera", 1, 0.0, L.ptr(theta), L.ptr(aug), aug.shape[0], L.ptr(K),
+                 L.stream())
+    else:
+        L.launch(_lib().scsfm_camera_build_indexed, "scsfm_camera_build_indexed", "camera", 1, 0.0, L.ptr(theta), theta.shape[0],
+                 L.ptr(aug), L.ptr(index), aug.shape[0], L.ptr(K), L.stream())
     return K
 
 
-def grad(aug, dK, dtheta):
-    """dtheta [4] += d(loss)/dtheta given dK = d(loss)/dK [B,3,3]."""
+def grad(aug, dK, dtheta, index=None):
+    """dtheta [4] (or [C,4] with index [B]) += d(loss)/dtheta given dK = d(loss)/dK [B,3,3]."""
     if dK.dtype != torch.float32 or tuple(dK.shape) != (aug.shape[0], 3, 3):
         raise TypeError("dK must be float32 [%d,3,3], got %s %s" % (aug.shape[0], dK.dtype, tuple(dK.shape)))
-    _check(dtheta, aug)
+    index = _check(dtheta, aug, index)
+    if not dtheta.is_contiguous():
+        raise TypeError("dtheta must be contiguous (the gradient is added in place)")
     dK = dK.contiguous()
-    L.launch(_lib().scsfm_camera_grad, "scsfm_camera_grad", "camera", 1, 0.0, L.ptr(aug), L.ptr(dK), aug.shape[0], L.ptr(dtheta),
-             L.stream())
+    if index is None:
+        L.launch(_lib().scsfm_camera_grad, "scsfm_camera_grad", "camera", 1, 0.0, L.ptr(aug), L.ptr(dK), aug.shape[0],
+                 L.ptr(dtheta), L.stream())
+    else:
+        L.launch(_lib().scsfm_camera_grad_indexed, "scsfm_camera_grad_indexed", "camera", 1, 0.0, L.ptr(aug), L.ptr(index),
+                 L.ptr(dK), aug.shape[0], dtheta.shape[0], L.ptr(dtheta), L.stream())
     return dtheta
 
 
 class CameraBuild(torch.autograd.Function):
-    """apply(theta [4], aug [B, AUG_DOUBLES]) -> K [B,3,3]; the backward is scsfm_camera_grad."""
+    """apply(theta [4] or [C,4], aug [B, AUG_DOUBLES], index None or [B]) -> K [B,3,3]; the backward is scsfm_camera_grad(_indexed)."""
 
     @staticmethod
-    def forward(ctx, theta, aug):
-        ctx.save_for_backward(aug)
-        return build(theta, aug)
+    def forward(ctx, theta, aug, index=None):
+        index = _check(theta, aug, index)
+        ctx.save_for_backward(aug, index)
+        ctx.theta_shape = tuple(theta.shape)
+        return build(theta, aug, index)
 
     @staticmethod
     def backward(ctx, dK):
-        aug, = ctx.saved_tensors
-        dtheta = torch.zeros(4, device=dK.device, dtype=torch.float32)
-        return grad(aug, dK.to(torch.float32), dtheta), None
+        aug, index = ctx.saved_tensors
+        dtheta = torch.zeros(ctx.theta_shape, device=dK.device, dtype=torch.float32)
+        return grad(aug, dK.to(torch.float32), dtheta, index), None, None
 
 
 class LearnedCamera(torch.nn.Module):
-    """One pinhole camera, theta = (fx, fy, cx, cy) float32 in pixels at the training resolution height x width.
-    forward(aug) -> K [B,3,3] of every sample's view through its augmentation record, differentiable in theta.
+    """One pinhole camera, theta = (fx, fy, cx, cy) float32 in pixels at the training resolution height x width, or a bank of C
+    cameras (LearnedCamera.bank), theta [C,4] with one label per camera in `groups`.
+    forward(aug) -> K [B,3,3] of every sample's view through its augmentation record, differentiable in theta; a bank takes
+    forward(aug, index) with index [B] (int32 or int64 CUDA): sample b sees camera index[b].
     state_dict: {'theta', 'height', 'width'}."""
 
     def __init__(self, fx, fy, cx, cy, height=0, width=0):
@@ -112,10 +149,26 @@ class LearnedCamera(torch.nn.Module):
         self.theta = torch.nn.Parameter(torch.tensor([fx, fy, cx, cy], dtype=torch.float32))
         self.register_buffer("height", torch.tensor(int(height), dtype=torch.int64))
         self.register_buffer("width", torch.tensor(int(width), dtype=torch.int64))
+        self.groups = None
 
-    def forward(self, aug):
-        return CameraBuild.apply(self.theta, aug)
+    @classmethod
+    def bank(cls, thetas, height=0, width=0, groups=None):
+        """C cameras: thetas [C,4] (fx, fy, cx, cy per row); groups: C labels (what each camera stands for, e.g. its cam.txt)."""
+        thetas = torch.as_tensor(thetas, dtype=torch.float32)
+        if thetas.dim() != 2 or thetas.shape[1] != 4 or thetas.shape[0] < 1:
+            raise TypeError("a camera bank takes thetas [C,4] with C >= 1, got %s" % (tuple(thetas.shape),))
+        groups = ["camera %d" % c for c in range(thetas.shape[0])] if groups is None else [str(g) for g in groups]
+        if len(groups) != thetas.shape[0]:
+            raise ValueError("%d group labels for %d cameras" % (len(groups), thetas.shape[0]))
+        cam = cls(0.0, 0.0, 0.0, 0.0, height, width)
+        cam.theta = torch.nn.Parameter(thetas.clone())
+        cam.groups = groups
+        return cam
+
+    def forward(self, aug, index=None):
+        return CameraBuild.apply(self.theta, aug, index)
 
     def extra_repr(self):
-        return "fx, fy, cx, cy = %s at %dx%d" % (", ".join("%.3f" % v for v in self.theta.detach().cpu().tolist()),
-                                                  int(self.height), int(self.width))
+        rows = self.theta.detach().cpu().reshape(-1, 4).tolist()
+        return "; ".join("fx, fy, cx, cy = %s" % ", ".join("%.3f" % v for v in r) for r in rows) + \
+            " at %dx%d" % (int(self.height), int(self.width))

@@ -10,6 +10,11 @@ Self-calibration: Trainer(..., camera=LearnedCamera(...)) owns a learned camera 
 batch's augmentation records (scsfm.camera.records, GpuAugment(..., return_records=True)) in place of intrinsics, builds every
 sample's K from theta, back-propagates into theta, all-reduces d(loss)/dtheta with the arenas (data parallel) and updates theta
 with its own Adam after the networks' -- all of it inside the captured step too.
+
+A bank of cameras (LearnedCamera.bank, theta [C,4]: one camera per calibration or per scene) also takes each sample's camera
+index, step(..., aug=records, camera_index=idx).  theta's Adam is dense over [C,4], as torch.optim.Adam on one [C,4] parameter:
+a camera that no sample has used yet has zero moments and does not move; a camera used earlier and absent from the current batch
+moves by its momentum.
 """
 import torch
 import torch.distributed as dist
@@ -40,8 +45,8 @@ def compute_pose_with_inv(pose_net, tgt_img, ref_imgs):
 
 class Trainer:
     """Holds the two networks, the fused Adam, (optionally) the data-parallel gradient exchange and (optionally) a learned camera:
-    camera = scsfm.camera.LearnedCamera on the networks' device, updated by Adam with learning rate camera_lr (the networks' betas
-    and eps, no weight decay)."""
+    camera = scsfm.camera.LearnedCamera on the networks' device (one camera, or a bank of C), updated by Adam with learning rate
+    camera_lr (the networks' betas and eps, no weight decay)."""
 
     def __init__(self, disp_net, pose_net, lr=1e-4, betas=(0.9, 0.999), weight_decay=0.0, num_scales=1, with_ssim=1,
                  with_mask=1, with_auto_mask=0, padding_mode="zeros", w1=1.0, w2=0.1, w3=0.5, distributed=None, conv_mode=None,
@@ -76,8 +81,9 @@ class Trainer:
         self.camera, self.camera_lr = camera, camera_lr
         if camera is not None:
             th = camera.theta
-            if not th.is_cuda or th.dtype != torch.float32 or th.shape != (4,):
-                raise TypeError("camera: a LearnedCamera whose theta is a float32 [4] CUDA parameter (move it to the GPU first)")
+            if not th.is_cuda or th.dtype != torch.float32 or not (th.shape == (4,) or (th.dim() == 2 and th.shape[1] == 4)):
+                raise TypeError("camera: a LearnedCamera whose theta is a float32 [4] or [C,4] CUDA parameter (move it to the GPU "
+                                "first)")
             # theta's Adam state: exp_avg, exp_avg_sq and the step counter, on the device (capturable, like ArenaAdam's)
             self._cam_state = (torch.zeros_like(th.data), torch.zeros_like(th.data), torch.zeros(1, device=th.device, dtype=torch.int32))
         if self.distributed:
@@ -124,14 +130,15 @@ class Trainer:
         w1, w2, w3 = self.w
         return w1 * photo + w2 * smooth + w3 * geo, photo, smooth, geo
 
-    def step(self, tgt_img, ref_imgs, intrinsics=None, aug=None):
+    def step(self, tgt_img, ref_imgs, intrinsics=None, aug=None, camera_index=None):
         """train.py:259-282 without a single host synchronisation; returns device scalars
         (loss, photo, smooth, geometry).  After `capture()` the step is one CUDA-graph replay.
 
         Intrinsics that require a gradient (a learned / self-calibrated K) get it in an eager single-GPU step, accumulated
         into their .grad as in the reference loop; updating them is left to the caller's own optimizer.
-        With a camera the step takes `aug`, the batch's augmentation records, and no intrinsics: K is built from the camera."""
-        intrinsics = self._camera_inputs(tgt_img, intrinsics, aug)
+        With a camera the step takes `aug`, the batch's augmentation records, and no intrinsics: K is built from the camera; a bank
+        of cameras also takes `camera_index`, each sample's camera (int32 or int64 [B] on the GPU)."""
+        intrinsics = self._camera_inputs(tgt_img, intrinsics, aug, camera_index)
         self._check_intrinsics(intrinsics)
         if self._graph is not None:
             if self._flag_patterns() != self._captured_flags:
@@ -141,30 +148,35 @@ class Trainer:
             for dst, src in zip(self._static[1], ref_imgs):
                 dst.copy_(src, non_blocking=True)
             self._static[2].copy_(intrinsics if self.camera is None else aug, non_blocking=True)
+            if camera_index is not None:
+                self._static[3].copy_(camera_index, non_blocking=True)
             self._graph.replay()
             return tuple(self._static_out.unbind(0))
-        return self._eager_step(tgt_img, ref_imgs, intrinsics, aug)
+        return self._eager_step(tgt_img, ref_imgs, intrinsics, aug, camera_index)
 
-    def capture(self, tgt_img, ref_imgs, intrinsics=None, allow_distributed=False, aug=None):
+    def capture(self, tgt_img, ref_imgs, intrinsics=None, allow_distributed=False, aug=None, camera_index=None):
         """Record the whole step (7 network calls forward + backward, losses, Adam) into one CUDA graph: ~2500
         kernel launches become a single graph launch.  One eager warm-up step runs first (lazy allocations,
         Adam state) and is undone, so capturing does not advance training.  Single-GPU path.  With a camera, `aug` takes the
-        place of intrinsics (as in step()); the records become a static buffer and the camera's theta and Adam state are undone too."""
+        place of intrinsics (as in step()); the records (and a bank's camera index) become static buffers and the camera's theta and
+        Adam state are undone too."""
         from . import lib as L
         if self.exchange is not None and not allow_distributed:
             raise RuntimeError("graph capture of the data-parallel step is opt-in (allow_distributed=True): capturing the NCCL "
                                "all-reduce on the side stream has not been validated on this pod yet")
-        intrinsics = self._camera_inputs(tgt_img, intrinsics, aug)
+        intrinsics = self._camera_inputs(tgt_img, intrinsics, aug, camera_index)
         self._check_intrinsics(intrinsics, capturing=True)
         third = intrinsics if self.camera is None else aug
         self._static = (tgt_img.clone(), [r.clone() for r in ref_imgs], third.clone())
+        if camera_index is not None:
+            self._static += (camera_index.to(torch.int32, copy=True),)
         snap = self.optimizer.snapshot()
         cam_snap = self._camera_snapshot()
         prof = dict(L.PROF)
         L.PROF.update(enabled=False)
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
-        static_args = self._static if self.camera is None else self._static[:2] + (None, self._static[2])
+        static_args = self._static if self.camera is None else self._static[:2] + (None,) + self._static[2:]
         with torch.cuda.stream(side):
             self._eager_step(*static_args)
         torch.cuda.current_stream().wait_stream(side)
@@ -188,8 +200,22 @@ class Trainer:
         self._captured_flags = self._flag_patterns()
         L.PROF.update(prof)
 
-    def _camera_inputs(self, tgt_img, intrinsics, aug):
-        """The intrinsics argument of a step: the caller's K without a camera; None with one, whose records are checked here."""
+    def _camera_inputs(self, tgt_img, intrinsics, aug, camera_index=None):
+        """The intrinsics argument of a step: the caller's K without a camera; None with one, whose records (and a bank's camera
+        index) are checked here."""
+        bank = self.camera is not None and self.camera.theta.dim() == 2
+        if camera_index is not None and not bank:
+            raise TypeError("a camera index is the input of a Trainer with a bank of cameras (LearnedCamera.bank(...)); this "
+                            "Trainer has %s" % ("no camera" if self.camera is None else "one camera"))
+        if bank:
+            if camera_index is None:
+                raise TypeError("a Trainer with a bank of %d cameras needs each sample's camera (camera_index=int32 [%d] CUDA "
+                                "tensor)" % (self.camera.theta.shape[0], tgt_img.shape[0]))
+            if (not isinstance(camera_index, torch.Tensor) or not camera_index.is_cuda
+                    or camera_index.dtype not in (torch.int32, torch.int64) or tuple(camera_index.shape) != (tgt_img.shape[0],)):
+                raise TypeError("camera_index must be an int32 or int64 CUDA tensor [%d], got %s" % (
+                    tgt_img.shape[0], "%s %s %s" % (camera_index.device, camera_index.dtype, tuple(camera_index.shape))
+                    if isinstance(camera_index, torch.Tensor) else type(camera_index).__name__))
         if self.camera is None:
             if aug is not None:
                 raise TypeError("augmentation records are the input of a Trainer with a camera (Trainer(..., camera=LearnedCamera(...)))")
@@ -245,11 +271,12 @@ class Trainer:
         self._graph = None
         self.launches_per_step = None
 
-    def _eager_step(self, tgt_img, ref_imgs, intrinsics, aug=None):
+    def _eager_step(self, tgt_img, ref_imgs, intrinsics, aug=None, camera_index=None):
         cam = self.camera
         if cam is not None:
             cam.theta.grad = None
-            intrinsics = cam(aug)                    # scsfm_camera_build; its backward adds d(loss)/dtheta (scsfm_camera_grad)
+            # scsfm_camera_build(_indexed); its backward adds d(loss)/dtheta (scsfm_camera_grad(_indexed))
+            intrinsics = cam(aug) if camera_index is None else cam(aug, camera_index)
         loss, photo, smooth, geo = self.losses(tgt_img, ref_imgs, intrinsics)
         self.optimizer.zero_grad()
         loss.backward()

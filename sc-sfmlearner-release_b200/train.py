@@ -19,6 +19,9 @@ Checkpoints keep the reference's file names and layout (utils.py:57-66): {'epoch
 through its own flip / zoom / crop (scsfm.camera.LearnedCamera), trained with the networks inside the captured / data-parallel
 step.  It needs the GPU transforms.  The camera is saved as camera_checkpoint.pth.tar {'epoch', 'state_dict'} next to the
 networks' files (camera_model_best.pth.tar with the same best-copy rule).
+--camera-groups calibration | scene learns a bank of cameras instead: one per distinct cam.txt (KITTI raw's recording days,
+Cityscapes' sequences) or one per training scene (uncalibrated video), each sample seeing its own group's camera.  The
+checkpoint then holds theta [C,4] and a top-level 'groups' list of the cameras' labels.
 """
 import argparse
 import csv
@@ -86,13 +89,18 @@ parser.add_argument("--gpu-augment", type=int, default=None, choices=[0, 1],
                          "host-side chain inside the loader workers.  Default: 1 for real datasets, 0 for DIR = synthetic")
 parser.add_argument("--learn-intrinsics", type=int, default=0, choices=[0, 1],
                     help="1: learn the camera intrinsics fx, fy, cx, cy (self-calibration) with the networks; needs --gpu-augment 1 and "
-                         "one camera for all training scenes")
+                         "one camera for all training scenes, or --camera-groups")
 parser.add_argument("--intrinsics-init", type=float, nargs=4, default=None, metavar=("FX", "FY", "CX", "CY"),
                     help="initial camera, in pixels at the training resolution.  Default: the first training scene's cam.txt "
                          "(DIR = synthetic: the synthetic K)")
 parser.add_argument("--intrinsics-lr", type=float, default=0.1,
                     help="Adam learning rate of the learned intrinsics (pixels per step at most, roughly): 0.1 recovers fx, fy to "
                          "1%% from 20%% off in a few hundred steps (tests/test_camera_gpu.py)")
+parser.add_argument("--camera-groups", choices=["one", "calibration", "scene"], default="one",
+                    help="with --learn-intrinsics 1: one camera shared by every training scene (one); one camera per distinct cam.txt "
+                         "matrix, per sample's intrinsics file with --folder-type pair (calibration: KITTI raw's recording days, "
+                         "Cityscapes' sequences); one camera per training scene (scene: uncalibrated video).  Each camera starts from "
+                         "its group's cam.txt, or every one from --intrinsics-init")
 
 best_error = -1
 n_iter = 0
@@ -122,26 +130,29 @@ class SyntheticLoader:
 class RawFrames(torch.utils.data.Dataset):
     """A reference dataset built with transform=None (datasets/sequence_folders.py:55-66, pair_folders.py): sample -> (frames
     uint8 [n_img, H, W, 3] with the target first, intrinsics).  uint8 is exact for decoded JPEG/PNG frames and a quarter of the
-    bytes through the worker pipes and PCIe."""
+    bytes through the worker pipes and PCIe.  With groups (one camera index per sample, see CameraTable): (frames, K, group)."""
 
-    def __init__(self, ds):
-        self.ds = ds
+    def __init__(self, ds, groups=None):
+        self.ds, self.groups = ds, groups
 
     def __len__(self):
         return len(self.ds)
 
     def __getitem__(self, i):
         tgt, refs, K, _ = self.ds[i]
-        return np.stack([tgt] + list(refs)).astype(np.uint8), np.asarray(K, np.float32)
+        out = np.stack([tgt] + list(refs)).astype(np.uint8), np.asarray(K, np.float32)
+        return out if self.groups is None else out + (self.groups[i],)
 
 
 class GpuAugmentLoader:
     """Wraps a loader of (frames uint8 [B, n_img, H, W, 3], K [B, 3, 3]) batches: upload, device-side transforms, and the
-    loop's (tgt_img, ref_imgs, intrinsics, intrinsics_inv) tuple comes out resident on the GPU."""
+    loop's (tgt_img, ref_imgs, intrinsics, intrinsics_inv) tuple comes out resident on the GPU.  records=True appends the
+    augmentation records; groups=True reads (frames, K, group) batches (RawFrames with groups) and appends the camera index of
+    every sample, int32 [B] on the device."""
 
-    def __init__(self, loader, device, train=True, records=False):
+    def __init__(self, loader, device, train=True, records=False, groups=False):
         from scsfm.augment import GpuAugment
-        self.loader, self.device, self.records = loader, device, records
+        self.loader, self.device, self.records, self.groups = loader, device, records, groups
         self.aug = GpuAugment(mean=(0.45, 0.45, 0.45), std=(0.225, 0.225, 0.225), train=train, device=device)
         self.sampler = getattr(loader, "sampler", None)
 
@@ -149,14 +160,18 @@ class GpuAugmentLoader:
         return len(self.loader)
 
     def __iter__(self):
-        for frames, K in self.loader:
+        for batch in self.loader:
+            frames, K = batch[:2]
             frames = frames.to(self.device, non_blocking=True).transpose(0, 1).contiguous()     # image slot major
             if self.records:                   # + the augmentation records a learned camera builds each sample's K from
                 imgs, K, rec = self.aug(frames, K, return_records=True)
-                yield imgs[0], imgs[1:], K, torch.linalg.inv(K), rec
-                continue
-            imgs, K = self.aug(frames, K)
-            yield imgs[0], imgs[1:], K, torch.linalg.inv(K)
+                out = imgs[0], imgs[1:], K, torch.linalg.inv(K), rec
+            else:
+                imgs, K = self.aug(frames, K)
+                out = imgs[0], imgs[1:], K, torch.linalg.inv(K)
+            if self.groups:                    # + each sample's camera in a bank of learned cameras
+                out += (batch[2].to(self.device, torch.int32, non_blocking=True),)
+            yield out
 
 
 def _reference_dataset_module(name):
@@ -195,14 +210,96 @@ def training_scene_cameras(root):
     return {s: np.genfromtxt(os.path.join(root, s, "cam.txt")).astype(np.float32).reshape(3, 3) for s in scenes}
 
 
+def _read_intrinsics(path):
+    """A 3x3 float32 intrinsics file, read as the reference's SequenceFolder / PairFolder read it."""
+    return np.genfromtxt(path).astype(np.float32).reshape(3, 3)
+
+
+def _training_scenes(root, split="train.txt"):
+    with open(os.path.join(root, split)) as f:
+        return [line.strip() for line in f if line.strip()]
+
+
+def _intrinsics_files(scene_dir, folder_type):
+    """The intrinsics files the reference's loader reads in one scene, in its order: cam.txt (SequenceFolder), or one sorted
+    *.txt per image pair (PairFolder, datasets/pair_folders.py:37-42)."""
+    if folder_type != "pair":
+        return [os.path.join(scene_dir, "cam.txt")]
+    names = sorted(os.listdir(scene_dir))
+    imgs = [n for n in names if n.endswith(".jpg")]
+    txts = [os.path.join(scene_dir, n) for n in names if n.endswith(".txt") and os.path.isfile(os.path.join(scene_dir, n))]
+    return [txts[i // 2] for i in range(0, len(imgs) - 1, 2)]
+
+
+class CameraTable:
+    """The cameras of --camera-groups calibration | scene.  Camera c stands for a group of samples: keys[c] is the group's key
+    (calibration: the float32 bytes of its intrinsics matrix; scene: its scene directory), labels[c] names it (the first
+    intrinsics file of the group, relative to DIR, or the scene) and Ks[c] is the matrix it starts from.  Cameras are numbered in
+    the order of the first train.txt scene that uses them, so every rank and every run builds the same table whatever the sample
+    shuffle."""
+
+    def __init__(self, root, mode, folder_type="sequence"):
+        if mode not in ("calibration", "scene"):
+            raise ValueError("camera groups: 'calibration' or 'scene', got %r" % (mode,))
+        self.mode, self.keys, self.labels, self.Ks, self._index = mode, [], [], [], {}
+        for scene in _training_scenes(root):
+            d = os.path.join(root, scene)
+            for f in _intrinsics_files(d, folder_type):
+                K = _read_intrinsics(f)
+                key = K.tobytes() if mode == "calibration" else os.path.abspath(d)
+                if key not in self._index:
+                    self._index[key] = len(self.keys)
+                    self.keys.append(key)
+                    self.labels.append(os.path.relpath(f, root) if mode == "calibration" else scene)
+                    self.Ks.append(K)
+
+    def __len__(self):
+        return len(self.keys)
+
+    def key(self, sample):
+        """The group key of a reference dataset sample (an entry of SequenceFolder / PairFolder .samples)."""
+        if self.mode == "calibration":
+            return np.asarray(sample["intrinsics"], np.float32).reshape(3, 3).tobytes()
+        return os.path.abspath(os.path.dirname(str(sample["tgt"])))
+
+    def index(self, sample):
+        """The camera of a sample; -1 for a sample whose group no training scene has."""
+        return self._index.get(self.key(sample), -1)
+
+    def thetas(self, init=None):
+        """[C][fx, fy, cx, cy]: each group's intrinsics, or init (--intrinsics-init) for every camera."""
+        return [list(init) if init is not None else [float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])] for K in self.Ks]
+
+
+def _initial_camera_arg(args):
+    if args.intrinsics_init is not None:
+        fx, fy, cx, cy = args.intrinsics_init
+        if not (fx > 0 and fy > 0):
+            raise SystemExit("--intrinsics-init: focal lengths must be positive, got fx %g fy %g" % (fx, fy))
+        return (fx, fy, cx, cy)
+    return None
+
+
 def check_learn_intrinsics(args):
     """--learn-intrinsics 1: the GPU transforms must be on (they hand out the augmentation records) and the training scenes must
-    share one camera.  Returns the initial (fx, fy, cx, cy); SystemExit with the reason otherwise."""
+    share one camera.  Returns the initial (fx, fy, cx, cy); SystemExit with the reason otherwise.  With --camera-groups
+    calibration | scene the training scenes may have several cameras: returns their CameraTable."""
+    groups = getattr(args, "camera_groups", "one")
+    if groups != "one" and not args.learn_intrinsics:
+        raise SystemExit("--camera-groups %s groups the cameras learned by --learn-intrinsics 1, which is off" % groups)
     if not args.learn_intrinsics:
         return None
     if not gpu_augment_on(args):
         raise SystemExit("--learn-intrinsics 1 needs the GPU transforms (--gpu-augment 1): the learned camera is built per sample "
                          "from the flip / zoom / crop records they hand out; learning K under the host-side chain is not supported")
+    if groups != "one":
+        if args.data == "synthetic":
+            raise SystemExit("--camera-groups %s: DIR = synthetic has one camera (use --camera-groups one)" % groups)
+        table = CameraTable(args.data, groups, args.folder_type)
+        if not len(table):
+            raise SystemExit("--learn-intrinsics 1: %s/train.txt lists no scene with intrinsics" % args.data)
+        _initial_camera_arg(args)
+        return table
     if args.data == "synthetic":
         H, W = args.synthetic_size
         K = synth.intrinsics(1, H, W, args.dataset)[0].numpy()
@@ -214,19 +311,21 @@ def check_learn_intrinsics(args):
         other = [s for s, K in cams.items() if not np.array_equal(K, first)]
         if other:
             raise SystemExit("--learn-intrinsics 1 learns ONE camera, but %d of the %d training scenes have a cam.txt different from "
-                             "the first's (e.g. %s): several cameras are not supported" % (len(other), len(cams), other[0]))
+                             "the first's (e.g. %s): several cameras are not supported (--camera-groups calibration learns one "
+                             "camera per cam.txt)" % (len(other), len(cams), other[0]))
         K = first
-    if args.intrinsics_init is not None:
-        fx, fy, cx, cy = args.intrinsics_init
-        if not (fx > 0 and fy > 0):
-            raise SystemExit("--intrinsics-init: focal lengths must be positive, got fx %g fy %g" % (fx, fy))
-        return (fx, fy, cx, cy)
+    init = _initial_camera_arg(args)
+    if init is not None:
+        return init
     return (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
 
 
-def make_loaders(args, rank, world, device="cuda"):
+def make_loaders(args, rank, world, device="cuda", cameras=None):
+    """cameras: the CameraTable of --camera-groups calibration | scene (None otherwise): every sample then carries its camera
+    index, -1 for a validation sample whose group is not a training camera's."""
     gpu_aug = gpu_augment_on(args)
     rec = {"records": True} if args.learn_intrinsics else {}       # the augmentation records, for a learned camera
+    grp = {"groups": True} if cameras is not None else {}
     if args.data == "synthetic":
         H, W = args.synthetic_size
         n_ref = 1 if args.folder_type == "pair" else args.sequence_length - 1
@@ -254,7 +353,9 @@ def make_loaders(args, rank, world, device="cuda"):
     else:
         train_set = PairFolder(args.data, seed=args.seed, train=True, transform=train_tf)
     if gpu_aug:
-        train_set = RawFrames(train_set)
+        train_set = RawFrames(train_set, None if cameras is None else [cameras.index(s) for s in train_set.samples])
+        if cameras is not None and -1 in train_set.groups:
+            raise SystemExit("--camera-groups %s: a training sample belongs to no camera group" % args.camera_groups)
     if args.with_gt:
         ValidationSet = _reference_dataset_module("validation_folders").ValidationSet
         val_set = ValidationSet(args.data, transform=valid_tf, dataset=args.dataset)
@@ -263,15 +364,21 @@ def make_loaders(args, rank, world, device="cuda"):
                                  sequence_length=args.sequence_length, dataset=args.dataset)
         if gpu_aug:
             val_set = RawFrames(val_set)     # (the ground-truth validation set above keeps the host chain: it also returns depth maps)
+            if cameras is not None:
+                val_set.groups = [cameras.index(s) for s in val_set.ds.samples]
+                if rank == 0:
+                    n = sum(g >= 0 for g in val_set.groups)
+                    print("=> validation: {} samples use their training group's learned camera, {} keep their dataset K".format(
+                        n, len(val_set.groups) - n))
     sampler = torch.utils.data.distributed.DistributedSampler(train_set, world, rank, shuffle=True, seed=args.seed) if world > 1 else None
     train_loader = torch.utils.data.DataLoader(train_set, batch_size=args.batch_size, shuffle=sampler is None, sampler=sampler,
                                                num_workers=args.workers, pin_memory=True, drop_last=True)
     val_loader = torch.utils.data.DataLoader(val_set, batch_size=args.batch_size, shuffle=False, num_workers=args.workers,
                                              pin_memory=True)
     if gpu_aug:
-        train_loader = GpuAugmentLoader(train_loader, device, train=True, **rec)
+        train_loader = GpuAugmentLoader(train_loader, device, train=True, **rec, **grp)
         if not args.with_gt:
-            val_loader = GpuAugmentLoader(val_loader, device, train=False)      # ArrayToTensor + Normalize only
+            val_loader = GpuAugmentLoader(val_loader, device, train=False, **grp)      # ArrayToTensor + Normalize only
     return train_loader, val_loader
 
 
@@ -287,7 +394,7 @@ def save_checkpoint(save_path, dispnet_state, exp_pose_state, is_best, filename=
 
 def save_camera_checkpoint(save_path, camera_state, is_best, filename="checkpoint.pth.tar"):
     """The learned camera next to the networks' files, with the same best-copy rule: camera_checkpoint.pth.tar
-    {'epoch', 'state_dict': {'theta', 'height', 'width'}}."""
+    {'epoch', 'state_dict': {'theta', 'height', 'width'}}, plus 'groups' (the labels of the cameras) for a bank."""
     state = dict(camera_state, state_dict={k: v.detach().clone().cpu() for k, v in camera_state["state_dict"].items()})
     torch.save(state, os.path.join(save_path, "camera_{}".format(filename)))
     if is_best:
@@ -297,7 +404,7 @@ def save_camera_checkpoint(save_path, camera_state, is_best, filename="checkpoin
 def training_size(args, train_loader):
     if args.data == "synthetic":
         return tuple(args.synthetic_size)
-    frames, _ = train_loader.loader.dataset[0]            # RawFrames: uint8 [n_img, H, W, 3]
+    frames = train_loader.loader.dataset[0][0]            # RawFrames: uint8 [n_img, H, W, 3]
     return tuple(frames.shape[1:3])
 
 
@@ -322,7 +429,8 @@ def main():
         os.makedirs(args.save_path, exist_ok=True)
     torch.manual_seed(args.seed)
 
-    train_loader, val_loader = make_loaders(args, rank, world, device)
+    table = init if isinstance(init, CameraTable) else None
+    train_loader, val_loader = make_loaders(args, rank, world, device, table)
     if args.epoch_size == 0:
         args.epoch_size = len(train_loader)
 
@@ -338,7 +446,12 @@ def main():
     if args.pretrained_pose:
         pose_net.load_state_dict(torch.load(args.pretrained_pose, map_location=device)["state_dict"], strict=False)
     camera = None
-    if init is not None:
+    if table is not None:
+        from scsfm.camera import LearnedCamera
+        camera = LearnedCamera.bank(table.thetas(args.intrinsics_init), *training_size(args, train_loader), groups=table.labels).to(device)
+        if rank == 0:
+            print("=> learning {} cameras (--camera-groups {})".format(len(table), args.camera_groups))
+    elif init is not None:
         from scsfm.camera import LearnedCamera
         camera = LearnedCamera(*init, *training_size(args, train_loader)).to(device)
 
@@ -365,7 +478,12 @@ def main():
         if rank == 0:
             print(" * epoch {} train loss {:.4f} | ".format(epoch, train_loss) +
                   ", ".join("{} : {:.3f}".format(n, e) for n, e in zip(names, errors)))
-            if camera is not None:
+            if table is not None:
+                for c, (label, th) in enumerate(zip(camera.groups, camera.theta.tolist())):
+                    K = table.Ks[c]
+                    print(" * epoch {} camera {} {}: learned fx {:.3f} fy {:.3f} cx {:.3f} cy {:.3f} | cam.txt fx {:.3f} fy {:.3f} "
+                          "cx {:.3f} cy {:.3f}".format(epoch, c, label, *th, K[0, 0], K[1, 1], K[0, 2], K[1, 2]))
+            elif camera is not None:
                 print(" * epoch {} learned camera fx {:.3f} fy {:.3f} cx {:.3f} cy {:.3f}".format(epoch, *camera.theta.tolist()))
             decisive = errors[1]
             if best_error < 0:
@@ -375,7 +493,10 @@ def main():
             save_checkpoint(args.save_path, {"epoch": epoch + 1, "state_dict": disp_net.state_dict()},
                             {"epoch": epoch + 1, "state_dict": pose_net.state_dict()}, is_best)
             if camera is not None:
-                save_camera_checkpoint(args.save_path, {"epoch": epoch + 1, "state_dict": camera.state_dict()}, is_best)
+                state = {"epoch": epoch + 1, "state_dict": camera.state_dict()}
+                if table is not None:
+                    state["groups"] = list(camera.groups)
+                save_camera_checkpoint(args.save_path, state, is_best)
             with open(os.path.join(args.save_path, args.log_summary), "a") as f:
                 csv.writer(f, delimiter="\t").writerow([train_loss, decisive])
     if world > 1:
@@ -395,6 +516,8 @@ def train(args, train_loader, trainer, device, rank, world):
         ref_imgs = [img.to(device, non_blocking=True) for img in ref_imgs]
         intrinsics = intrinsics.to(device, non_blocking=True)
         inputs = dict(intrinsics=intrinsics) if trainer.camera is None else dict(aug=batch[4])    # a learned camera builds K itself
+        if len(batch) > 5:
+            inputs["camera_index"] = batch[5]        # a bank of cameras: each sample's
         if args.cuda_graph and world == 1 and trainer._graph is None and i == 0 and n_iter == 0:
             trainer.capture(tgt_img, ref_imgs, **inputs)
         out = trainer.step(tgt_img, ref_imgs, **inputs)
@@ -422,17 +545,24 @@ def train(args, train_loader, trainer, device, rank, world):
 @torch.no_grad()
 def validate_without_gt(args, val_loader, disp_net, pose_net, device, camera=None):
     """train.py:302-362: eval-mode networks, the same losses, auto-mask forced off.  With a learned camera its K (the identity
-    draw: the validation frames are not flipped, zoomed or cropped) replaces the dataset's."""
+    draw: the validation frames are not flipped, zoomed or cropped) replaces the dataset's.  With a bank of cameras only the
+    samples of a training group (camera index >= 0) take their camera's K; the others keep the dataset's."""
     disp_net.eval()
     pose_net.eval()
     acc, n = torch.zeros(4, device=device), 0
-    for tgt_img, ref_imgs, intrinsics, _ in val_loader:
+    for batch in val_loader:
+        tgt_img, ref_imgs, intrinsics = batch[:3]
         tgt_img = tgt_img.to(device)
         ref_imgs = [img.to(device) for img in ref_imgs]
         intrinsics = intrinsics.to(device)
         if camera is not None:
             from scsfm.camera import identity_records
-            intrinsics = camera(identity_records(tgt_img.shape[0], tgt_img.shape[-1], device))
+            rec = identity_records(tgt_img.shape[0], tgt_img.shape[-1], device)
+            if camera.theta.dim() == 1:
+                intrinsics = camera(rec)
+            else:                                     # (an index of -1 builds a NaN K, which the where() drops)
+                idx = batch[4]
+                intrinsics = torch.where((idx >= 0)[:, None, None], camera(rec, idx), intrinsics)
         tgt_depth = [1 / disp_net(tgt_img)]
         ref_depths = [[1 / disp_net(r)] for r in ref_imgs]
         poses = [pose_net(tgt_img, r) for r in ref_imgs]
