@@ -431,26 +431,21 @@ int scsfm_adam_step_masked(float* param, const float* grad, float* exp_avg, floa
                            const unsigned char* chunk_mask, float lr, float beta1, float beta2, float eps, float weight_decay,
                            int step, const int* step_dev, float* mirror, int mirror_operand, void* stream);
 
-/* Learned camera (self-calibration under the training transforms).  theta = (fx, fy, cx, cy): one camera, fp32, in pixels at
- * the training resolution (zero skew, bottom row 0 0 1).  aug: one record per sample of SCSFM_CAMERA_AUG_DOUBLES doubles,
+/* Learned cameras (self-calibration under the training transforms).  theta [n_cams, 4]: a bank of n_cams >= 1 cameras, each
+ * (fx, fy, cx, cy), fp32, in pixels at the training resolution (zero skew, bottom row 0 0 1): one per calibration or per scene
+ * of a multi-camera dataset, or n_cams = 1 for one camera.  idx [B] (int32): the camera of every sample; a null idx, allowed
+ * with n_cams = 1 only, puts every sample on camera 0.  aug: one record per sample of SCSFM_CAMERA_AUG_DOUBLES doubles,
  * {x_scale, y_scale, flip (0 / 1), offset_x, offset_y, in_w}: the flip, zoom factors and crop offsets of the sample's
  * RandomHorizontalFlip / RandomScaleCrop (custom_transforms.py:46-89) and the input width; the identity record is
  * {1, 1, 0, 0, 0, W}.  The zoom factors are the values numpy multiplies the float32 rows by (float64 draws stay float64).
- *   scsfm_camera_build: K_out[b] [3,3] = theta seen through record b, with the operations, order and roundings of the
- *     reference's intrinsics update (custom_transforms.py:56-57, 74-75, 83-84) on a float32 matrix: with theta equal to a
- *     dataset's K, bit for bit the K the augmentation hands out.
- *   scsfm_camera_grad: ADDS d(loss)/dtheta = sum_b dK_b/dtheta . dK[b] into dtheta [4] (fp32).  One CTA, fp64 sums in a fixed
- *     order, no atomics: deterministic.
- * A bank of cameras (one per calibration or per scene of a multi-camera dataset): theta [n_cams, 4] and one camera index per
- * sample, idx [B] (int32).
- *   scsfm_camera_build_indexed: K_out[b] = theta[idx[b]] seen through record b, as above; an index outside [0, n_cams) gives
- *     nine NaNs in K_out[b] and reads nothing out of bounds.
- *   scsfm_camera_grad_indexed: ADDS into dtheta [n_cams, 4] the gradient of each camera, summed over the samples that use it
- *     (none from an out-of-range index).  One CTA per camera, each with the fixed-order fp64 sum above: deterministic.
- * scsfm_camera_build / scsfm_camera_grad are the n_cams = 1 calls of the same kernels with every sample on camera 0. */
+ *   scsfm_camera_build_indexed: K_out[b] [3,3] = theta[idx[b]] seen through record b, with the operations, order and
+ *     roundings of the reference's intrinsics update (custom_transforms.py:56-57, 74-75, 83-84) on a float32 matrix: with
+ *     theta equal to a dataset's K, bit for bit the K the augmentation hands out.  An index outside [0, n_cams) gives nine
+ *     NaNs in K_out[b] and reads nothing out of bounds.
+ *   scsfm_camera_grad_indexed: ADDS into dtheta [n_cams, 4] (fp32) the gradient of each camera, sum_b dK_b/dtheta . dK[b]
+ *     over the samples that use it (none from an out-of-range index).  One CTA per camera, fp64 sums in a fixed order, no
+ *     atomics: deterministic. */
 #define SCSFM_CAMERA_AUG_DOUBLES 6
-int scsfm_camera_build(const float* theta, const double* aug, int B, float* K_out, void* stream);
-int scsfm_camera_grad(const double* aug, const float* dK, int B, float* dtheta, void* stream);
 int scsfm_camera_build_indexed(const float* theta, int n_cams, const double* aug, const int* idx, int B, float* K_out,
                                void* stream);
 int scsfm_camera_grad_indexed(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta,

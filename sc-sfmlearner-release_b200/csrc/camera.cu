@@ -1,17 +1,16 @@
-// Learned camera for self-calibration under the training transforms.  One camera theta = (fx, fy, cx, cy) in pixels at the
-// training resolution; every sample of a batch sees it through its own flip / zoom / crop (custom_transforms.py:46-89), so its
-// intrinsics are K_b = aug_b(theta):
+// Learned cameras for self-calibration under the training transforms.  A bank of n_cams cameras theta [n_cams, 4], each
+// (fx, fy, cx, cy) in pixels at the training resolution, and one camera index per sample; one camera is the bank of one, with a
+// null index meaning camera 0 for every sample.  Every sample of a batch sees its camera through its own flip / zoom / crop
+// (custom_transforms.py:46-89), so its intrinsics are K_b = aug_b(theta[idx_b]):
 //
-//  * scsfm_camera_build evaluates aug_b with the operations, order and roundings of scsfm/augment.py:update_intrinsics on a
-//    float32 matrix (the reference's expressions under numpy's casting rules): the flip and the crop offsets are float32
+//  * scsfm_camera_build_indexed evaluates aug_b with the operations, order and roundings of scsfm/augment.py:update_intrinsics
+//    on a float32 matrix (the reference's expressions under numpy's casting rules): the flip and the crop offsets are float32
 //    subtractions (a Python int against a float32 scalar), each zoom is a float64 product rounded back into the float32 matrix
 //    (a float32 row times a float64 scalar).  With theta equal to the dataset's K the result is GpuAugment's K bit for bit;
-//  * scsfm_camera_grad is the chain rule through that map (roundings taken as identity): each entry of K_b is an affine function
-//    of one parameter, so d(loss)/dtheta = sum_b of four scaled entries of dK_b.  One CTA sums them in fp64 in a fixed order.
-// A multi-camera dataset (one calibration per KITTI raw recording day, one camera per uncalibrated video) learns a bank of cameras
-// theta [n_cams, 4]; sample b then sees camera idx[b] (scsfm_camera_*_indexed).  Both kernels take the index: the build reads
-// theta + 4 idx[b], the gradient runs one CTA per camera over the samples that use it.  The single-camera entries are the
-// n_cams = 1 calls with a null index (every sample on camera 0), with the same arithmetic as before.
+//  * scsfm_camera_grad_indexed is the chain rule through that map (roundings taken as identity): each entry of K_b is an affine
+//    function of one parameter, so d(loss)/dtheta[c] = sum over the samples b of camera c of four scaled entries of dK_b.  One CTA
+//    per camera sums them in fp64 in a fixed order.
+// (One calibration per KITTI raw recording day or one camera per uncalibrated video gives n_cams > 1.)
 #include "common.cuh"
 
 namespace scsfm {
@@ -84,46 +83,26 @@ camera_grad_kernel(const double* __restrict__ aug, const int* __restrict__ idx, 
 
 using namespace scsfm;
 
-static void launch_build(const float* theta, int n_cams, const double* aug, const int* idx, int B, float* K_out, void* stream) {
-    camera_build_kernel<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(theta, n_cams, aug, idx, B, K_out);
-}
-
-static void launch_grad(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta, void* stream) {
-    camera_grad_kernel<<<n_cams, CAM_GRAD_THREADS, 0, (cudaStream_t)stream>>>(aug, idx, dK, B, dtheta);
-}
-
-extern "C" int scsfm_camera_build(const float* theta, const double* aug, int B, float* K_out, void* stream) {
-    SCSFM_CHECK_ARG(theta && aug && K_out, "camera_build: null pointer (theta, aug and K_out are required)");
-    SCSFM_CHECK_ARG(B > 0, "camera_build: batch size must be positive, got %d", B);
-    launch_build(theta, 1, aug, nullptr, B, K_out, stream);
-    SCSFM_CHECK_LAUNCH();
-    return SCSFM_OK;
-}
-
-extern "C" int scsfm_camera_grad(const double* aug, const float* dK, int B, float* dtheta, void* stream) {
-    SCSFM_CHECK_ARG(aug && dK && dtheta, "camera_grad: null pointer (aug, dK and dtheta are required)");
-    SCSFM_CHECK_ARG(B > 0, "camera_grad: batch size must be positive, got %d", B);
-    launch_grad(aug, nullptr, dK, B, 1, dtheta, stream);
-    SCSFM_CHECK_LAUNCH();
-    return SCSFM_OK;
-}
-
 extern "C" int scsfm_camera_build_indexed(const float* theta, int n_cams, const double* aug, const int* idx, int B, float* K_out,
                                           void* stream) {
-    SCSFM_CHECK_ARG(theta && aug && idx && K_out, "camera_build_indexed: null pointer (theta, aug, idx and K_out are required)");
+    SCSFM_CHECK_ARG(theta && aug && K_out, "camera_build_indexed: null pointer (theta, aug and K_out are required)");
     SCSFM_CHECK_ARG(n_cams > 0, "camera_build_indexed: number of cameras must be positive, got %d", n_cams);
+    SCSFM_CHECK_ARG(idx || n_cams == 1, "camera_build_indexed: null idx with %d cameras (a null idx means camera 0 for every "
+                    "sample, for n_cams = 1 only)", n_cams);
     SCSFM_CHECK_ARG(B > 0, "camera_build_indexed: batch size must be positive, got %d", B);
-    launch_build(theta, n_cams, aug, idx, B, K_out, stream);
+    camera_build_kernel<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(theta, n_cams, aug, idx, B, K_out);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
 
 extern "C" int scsfm_camera_grad_indexed(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta,
                                          void* stream) {
-    SCSFM_CHECK_ARG(aug && idx && dK && dtheta, "camera_grad_indexed: null pointer (aug, idx, dK and dtheta are required)");
-    SCSFM_CHECK_ARG(B > 0, "camera_grad_indexed: batch size must be positive, got %d", B);
+    SCSFM_CHECK_ARG(aug && dK && dtheta, "camera_grad_indexed: null pointer (aug, dK and dtheta are required)");
     SCSFM_CHECK_ARG(n_cams > 0, "camera_grad_indexed: number of cameras must be positive, got %d", n_cams);
-    launch_grad(aug, idx, dK, B, n_cams, dtheta, stream);
+    SCSFM_CHECK_ARG(idx || n_cams == 1, "camera_grad_indexed: null idx with %d cameras (a null idx means camera 0 for every "
+                    "sample, for n_cams = 1 only)", n_cams);
+    SCSFM_CHECK_ARG(B > 0, "camera_grad_indexed: batch size must be positive, got %d", B);
+    camera_grad_kernel<<<n_cams, CAM_GRAD_THREADS, 0, (cudaStream_t)stream>>>(aug, idx, dK, B, dtheta);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }

@@ -1,14 +1,15 @@
-"""A learned camera for self-calibration under the training transforms (csrc/camera.cu, include/scsfm.h: scsfm_camera_*).
+"""Learned cameras for self-calibration under the training transforms (csrc/camera.cu, include/scsfm.h: scsfm_camera_*).
 
-There is one camera theta = (fx, fy, cx, cy), in pixels at the training resolution (what cam.txt holds after preparation).  With
-the GPU transforms every sample is flipped, zoomed and cropped (custom_transforms.py:46-89), so the intrinsics the losses see are
-one per sample: K_b = aug_b(theta).  `records()` turns the random draws of a batch into device records; `LearnedCamera(records)`
-builds the batch's K with the augmentation's own arithmetic and back-propagates into theta in one small deterministic kernel.
-The K it returns feeds the loss entry points unchanged (their intrinsics gradient supplies dK).
+A camera theta = (fx, fy, cx, cy) is in pixels at the training resolution (what cam.txt holds after preparation).  With the GPU
+transforms every sample is flipped, zoomed and cropped (custom_transforms.py:46-89), so the intrinsics the losses see are one per
+sample: K_b = aug_b(theta).  `records()` turns the random draws of a batch into device records; `LearnedCamera(records)` builds
+the batch's K with the augmentation's own arithmetic and back-propagates into theta in one small deterministic kernel.  The K it
+returns feeds the loss entry points unchanged (their intrinsics gradient supplies dK).
 
 A dataset recorded with several cameras (KITTI raw: one calibration per recording day; Cityscapes: one per sequence; uncalibrated
 video: one per clip) learns a bank of cameras instead: `LearnedCamera.bank(thetas [C,4], ...)` holds theta [C,4], and
-`forward(aug, index)` gives sample b the view of camera index[b] through its own record (scsfm_camera_*_indexed).
+`forward(aug, index)` gives sample b the view of camera index[b] through its own record.  One camera is the same kernels' bank of
+one with a null index.
 """
 import ctypes
 
@@ -27,8 +28,6 @@ def _lib():
     lib = L.load()
     if not _bound:
         P, I = ctypes.c_void_p, ctypes.c_int
-        lib.scsfm_camera_build.argtypes = [P, P, I, P, P]
-        lib.scsfm_camera_grad.argtypes = [P, P, I, P, P]
         lib.scsfm_camera_build_indexed.argtypes = [P, I, P, P, I, P, P]
         lib.scsfm_camera_grad_indexed.argtypes = [P, P, P, I, I, P, P]
         _bound = True
@@ -61,45 +60,59 @@ def identity_records(B, in_w, device="cuda"):
     return r.to(device)
 
 
-def _check(theta, aug, index=None):
-    """Types, shapes and devices of a call, checked before any launch.  theta [4] takes no index, theta [C,4] requires one:
-    int32 or int64 [B] on the GPU.  Returns the index as int32 (or None)."""
-    if not (theta.is_cuda and aug.is_cuda):
-        raise RuntimeError("the learned camera runs on the GPU: theta and the augmentation records must be CUDA tensors "
-                           "(there is no CPU fallback)")
+class _DeviceError(TypeError, RuntimeError):
+    """A camera input on the wrong device: a RuntimeError as torch reports device mismatches, and a TypeError as the Trainer
+    reports its malformed step inputs."""
+
+
+def _check_theta(theta):
+    if not theta.is_cuda:
+        raise _DeviceError("the learned camera runs on the GPU: theta must be a CUDA tensor (move the camera to the GPU first; "
+                           "there is no CPU fallback)")
     if theta.dtype != torch.float32 or not (theta.shape == (4,) or (theta.dim() == 2 and theta.shape[1] == 4 and theta.shape[0] >= 1)):
         raise TypeError("theta must be float32 [4] (fx, fy, cx, cy) or [C,4] (a bank of C cameras), got %s %s"
                         % (theta.dtype, tuple(theta.shape)))
-    if aug.dtype != torch.float64 or aug.dim() != 2 or aug.shape[1] != AUG_DOUBLES or aug.shape[0] < 1:
-        raise TypeError("augmentation records must be float64 [B, %d] (scsfm.camera.records), got %s %s"
-                        % (AUG_DOUBLES, aug.dtype, tuple(aug.shape)))
+
+
+def _check(theta, aug, index=None, B=None):
+    """Types, shapes and devices of a call, checked before any launch: records float64 [B, AUG_DOUBLES] on the GPU; theta [4]
+    takes no index, theta [C,4] requires one, int32 or int64 [B] on theta's device.  B is the batch size (the records' own by
+    default)."""
+    _check_theta(theta)
+    if not aug.is_cuda:
+        raise _DeviceError("the learned camera runs on the GPU: the augmentation records must be a CUDA tensor (there is no CPU "
+                           "fallback)")
+    B = len(aug) if B is None else B
+    if aug.dtype != torch.float64 or tuple(aug.shape) != (B, AUG_DOUBLES) or B < 1:
+        raise TypeError("augmentation records must be float64 [%d, %d] (scsfm.camera.records), got %s %s"
+                        % (B, AUG_DOUBLES, aug.dtype, tuple(aug.shape)))
     if theta.dim() == 1:
         if index is not None:
-            raise TypeError("a camera index is for a bank of cameras (theta [C,4]); this camera has theta [4]")
-        return None
+            raise TypeError("a camera index is for a bank of cameras (theta [C,4]); this is one camera, theta [4]")
+        return
     if index is None:
-        raise TypeError("a bank of %d cameras needs the camera index of every sample (index: int32 or int64 [%d] CUDA tensor)"
-                        % (theta.shape[0], aug.shape[0]))
-    if not isinstance(index, torch.Tensor) or index.dtype not in (torch.int32, torch.int64) or tuple(index.shape) != (aug.shape[0],):
-        raise TypeError("camera index must be an int32 or int64 tensor [%d], got %s" % (
-            aug.shape[0], "%s %s" % (index.dtype, tuple(index.shape)) if isinstance(index, torch.Tensor) else type(index).__name__))
-    if not index.is_cuda or index.device != theta.device:
-        raise RuntimeError("camera index must be on the camera's device %s, got %s" % (theta.device, index.device))
-    return index.to(torch.int32).contiguous()
+        raise TypeError("a bank of %d cameras needs the camera index of every sample (int32 or int64 [%d] CUDA tensor)"
+                        % (theta.shape[0], B))
+    if not isinstance(index, torch.Tensor) or index.dtype not in (torch.int32, torch.int64) or tuple(index.shape) != (B,):
+        raise TypeError("camera index must be an int32 or int64 CUDA tensor [%d], got %s" % (
+            B, "%s %s" % (index.dtype, tuple(index.shape)) if isinstance(index, torch.Tensor) else type(index).__name__))
+    if index.device != theta.device:
+        raise _DeviceError("camera index must be an int32 or int64 CUDA tensor on the camera's device %s, got %s"
+                           % (theta.device, index.device))
+
+
+def _index32(index):
+    return None if index is None else index.to(torch.int32).contiguous()
 
 
 def build(theta, aug, index=None):
     """K [B,3,3] float32 of theta through every record (no autograd).  theta [C,4] with index [B]: sample b sees camera index[b]
     (an index outside [0, C) gives a NaN K)."""
-    index = _check(theta, aug, index)
-    theta, aug = theta.detach().contiguous(), aug.contiguous()
+    _check(theta, aug, index)
+    theta, aug, index = theta.detach().contiguous(), aug.contiguous(), _index32(index)
     K = torch.empty(aug.shape[0], 3, 3, device=theta.device, dtype=torch.float32)
-    if index is None:
-        L.launch(_lib().scsfm_camera_build, "scsfm_camera_build", "camera", 1, 0.0, L.ptr(theta), L.ptr(aug), aug.shape[0], L.ptr(K),
-                 L.stream())
-    else:
-        L.launch(_lib().scsfm_camera_build_indexed, "scsfm_camera_build_indexed", "camera", 1, 0.0, L.ptr(theta), theta.shape[0],
-                 L.ptr(aug), L.ptr(index), aug.shape[0], L.ptr(K), L.stream())
+    L.launch(_lib().scsfm_camera_build_indexed, "scsfm_camera_build_indexed", "camera", 1, 0.0, L.ptr(theta), theta.numel() // 4,
+             L.ptr(aug), L.ptr(index), aug.shape[0], L.ptr(K), L.stream())
     return K
 
 
@@ -107,25 +120,22 @@ def grad(aug, dK, dtheta, index=None):
     """dtheta [4] (or [C,4] with index [B]) += d(loss)/dtheta given dK = d(loss)/dK [B,3,3]."""
     if dK.dtype != torch.float32 or tuple(dK.shape) != (aug.shape[0], 3, 3):
         raise TypeError("dK must be float32 [%d,3,3], got %s %s" % (aug.shape[0], dK.dtype, tuple(dK.shape)))
-    index = _check(dtheta, aug, index)
+    _check(dtheta, aug, index)
     if not dtheta.is_contiguous():
         raise TypeError("dtheta must be contiguous (the gradient is added in place)")
-    dK = dK.contiguous()
-    if index is None:
-        L.launch(_lib().scsfm_camera_grad, "scsfm_camera_grad", "camera", 1, 0.0, L.ptr(aug), L.ptr(dK), aug.shape[0],
-                 L.ptr(dtheta), L.stream())
-    else:
-        L.launch(_lib().scsfm_camera_grad_indexed, "scsfm_camera_grad_indexed", "camera", 1, 0.0, L.ptr(aug), L.ptr(index),
-                 L.ptr(dK), aug.shape[0], dtheta.shape[0], L.ptr(dtheta), L.stream())
+    dK, index = dK.contiguous(), _index32(index)
+    L.launch(_lib().scsfm_camera_grad_indexed, "scsfm_camera_grad_indexed", "camera", 1, 0.0, L.ptr(aug), L.ptr(index), L.ptr(dK),
+             aug.shape[0], dtheta.numel() // 4, L.ptr(dtheta), L.stream())
     return dtheta
 
 
 class CameraBuild(torch.autograd.Function):
-    """apply(theta [4] or [C,4], aug [B, AUG_DOUBLES], index None or [B]) -> K [B,3,3]; the backward is scsfm_camera_grad(_indexed)."""
+    """apply(theta [4] or [C,4], aug [B, AUG_DOUBLES], index None or [B]) -> K [B,3,3]; the backward is scsfm_camera_grad_indexed."""
 
     @staticmethod
     def forward(ctx, theta, aug, index=None):
-        index = _check(theta, aug, index)
+        _check(theta, aug, index)
+        index = _index32(index)
         ctx.save_for_backward(aug, index)
         ctx.theta_shape = tuple(theta.shape)
         return build(theta, aug, index)

@@ -22,6 +22,7 @@ import torch.distributed as dist
 import loss_functions as LF
 
 from . import nnops as O
+from .camera import _check as _check_camera_inputs, _check_theta
 from .exchange import GradExchange
 from .nets import ArenaAdam
 
@@ -81,9 +82,7 @@ class Trainer:
         self.camera, self.camera_lr = camera, camera_lr
         if camera is not None:
             th = camera.theta
-            if not th.is_cuda or th.dtype != torch.float32 or not (th.shape == (4,) or (th.dim() == 2 and th.shape[1] == 4)):
-                raise TypeError("camera: a LearnedCamera whose theta is a float32 [4] or [C,4] CUDA parameter (move it to the GPU "
-                                "first)")
+            _check_theta(th)
             # theta's Adam state: exp_avg, exp_avg_sq and the step counter, on the device (capturable, like ArenaAdam's)
             self._cam_state = (torch.zeros_like(th.data), torch.zeros_like(th.data), torch.zeros(1, device=th.device, dtype=torch.int32))
         if self.distributed:
@@ -144,12 +143,13 @@ class Trainer:
             if self._flag_patterns() != self._captured_flags:
                 raise RuntimeError("the requires_grad / train-eval pattern of the networks changed after capture(): the captured "
                                    "step computes the old one (drop_graph() and capture() again)")
-            self._static[0].copy_(tgt_img, non_blocking=True)
-            for dst, src in zip(self._static[1], ref_imgs):
-                dst.copy_(src, non_blocking=True)
-            self._static[2].copy_(intrinsics if self.camera is None else aug, non_blocking=True)
-            if camera_index is not None:
-                self._static[3].copy_(camera_index, non_blocking=True)
+            given = dict(tgt_img=tgt_img, intrinsics=intrinsics, aug=aug, camera_index=camera_index)
+            for name, dst in self._static.items():
+                if name == "ref_imgs":
+                    for d, src in zip(dst, ref_imgs):
+                        d.copy_(src, non_blocking=True)
+                else:
+                    dst.copy_(given[name], non_blocking=True)
             self._graph.replay()
             return tuple(self._static_out.unbind(0))
         return self._eager_step(tgt_img, ref_imgs, intrinsics, aug, camera_index)
@@ -166,19 +166,19 @@ class Trainer:
                                "all-reduce on the side stream has not been validated on this pod yet")
         intrinsics = self._camera_inputs(tgt_img, intrinsics, aug, camera_index)
         self._check_intrinsics(intrinsics, capturing=True)
-        third = intrinsics if self.camera is None else aug
-        self._static = (tgt_img.clone(), [r.clone() for r in ref_imgs], third.clone())
-        if camera_index is not None:
-            self._static += (camera_index.to(torch.int32, copy=True),)
+        # the static inputs, by _eager_step's keyword: the images, and K or the records (and a bank's camera index)
+        self._static = dict(tgt_img=tgt_img.clone(), ref_imgs=[r.clone() for r in ref_imgs])
+        for name, t in (("intrinsics", intrinsics), ("aug", aug), ("camera_index", camera_index)):
+            if t is not None:
+                self._static[name] = t.to(torch.int32, copy=True) if name == "camera_index" else t.clone()
         snap = self.optimizer.snapshot()
         cam_snap = self._camera_snapshot()
         prof = dict(L.PROF)
         L.PROF.update(enabled=False)
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
-        static_args = self._static if self.camera is None else self._static[:2] + (None,) + self._static[2:]
         with torch.cuda.stream(side):
-            self._eager_step(*static_args)
+            self._eager_step(**self._static)
         torch.cuda.current_stream().wait_stream(side)
         self.optimizer.restore(snap)
         self._camera_restore(cam_snap)
@@ -194,31 +194,19 @@ class Trainer:
         # events); NCCL's watchdog thread may touch CUDA meanwhile, hence the thread-local capture mode
         mode = "thread_local" if self.exchange is not None else "global"
         with torch.cuda.graph(graph, capture_error_mode=mode):
-            self._static_out = torch.stack(self._eager_step(*static_args))
+            self._static_out = torch.stack(self._eager_step(**self._static))
         self.launches_per_step = L.launch_count() - before
         self._graph = graph
         self._captured_flags = self._flag_patterns()
         L.PROF.update(prof)
 
-    def _camera_inputs(self, tgt_img, intrinsics, aug, camera_index=None):
+    def _camera_inputs(self, tgt_img, intrinsics, aug, camera_index):
         """The intrinsics argument of a step: the caller's K without a camera; None with one, whose records (and a bank's camera
-        index) are checked here."""
-        bank = self.camera is not None and self.camera.theta.dim() == 2
-        if camera_index is not None and not bank:
-            raise TypeError("a camera index is the input of a Trainer with a bank of cameras (LearnedCamera.bank(...)); this "
-                            "Trainer has %s" % ("no camera" if self.camera is None else "one camera"))
-        if bank:
-            if camera_index is None:
-                raise TypeError("a Trainer with a bank of %d cameras needs each sample's camera (camera_index=int32 [%d] CUDA "
-                                "tensor)" % (self.camera.theta.shape[0], tgt_img.shape[0]))
-            if (not isinstance(camera_index, torch.Tensor) or not camera_index.is_cuda
-                    or camera_index.dtype not in (torch.int32, torch.int64) or tuple(camera_index.shape) != (tgt_img.shape[0],)):
-                raise TypeError("camera_index must be an int32 or int64 CUDA tensor [%d], got %s" % (
-                    tgt_img.shape[0], "%s %s %s" % (camera_index.device, camera_index.dtype, tuple(camera_index.shape))
-                    if isinstance(camera_index, torch.Tensor) else type(camera_index).__name__))
+        index) are checked here against the batch."""
         if self.camera is None:
-            if aug is not None:
-                raise TypeError("augmentation records are the input of a Trainer with a camera (Trainer(..., camera=LearnedCamera(...)))")
+            if aug is not None or camera_index is not None:
+                raise TypeError("augmentation records and a camera index are the inputs of a Trainer with a camera (Trainer(..., "
+                                "camera=LearnedCamera(...))); this Trainer has no camera")
             if intrinsics is None:
                 raise TypeError("intrinsics are required (or give the Trainer a camera and pass augmentation records)")
             return intrinsics
@@ -228,10 +216,7 @@ class Trainer:
         if aug is None:
             raise TypeError("a Trainer with a camera needs the batch's augmentation records (aug=scsfm.camera.records(...), "
                             "or GpuAugment(..., return_records=True))")
-        from .camera import AUG_DOUBLES
-        if not aug.is_cuda or aug.dtype != torch.float64 or tuple(aug.shape) != (tgt_img.shape[0], AUG_DOUBLES):
-            raise TypeError("augmentation records must be a float64 CUDA tensor [%d, %d], got %s %s %s"
-                            % (tgt_img.shape[0], AUG_DOUBLES, aug.device, aug.dtype, tuple(aug.shape)))
+        _check_camera_inputs(self.camera.theta, aug, camera_index, tgt_img.shape[0])
         return None
 
     def _camera_snapshot(self):
@@ -271,12 +256,12 @@ class Trainer:
         self._graph = None
         self.launches_per_step = None
 
-    def _eager_step(self, tgt_img, ref_imgs, intrinsics, aug=None, camera_index=None):
+    def _eager_step(self, tgt_img, ref_imgs, intrinsics=None, aug=None, camera_index=None):
         cam = self.camera
         if cam is not None:
             cam.theta.grad = None
-            # scsfm_camera_build(_indexed); its backward adds d(loss)/dtheta (scsfm_camera_grad(_indexed))
-            intrinsics = cam(aug) if camera_index is None else cam(aug, camera_index)
+            # scsfm_camera_build_indexed; its backward adds d(loss)/dtheta (scsfm_camera_grad_indexed)
+            intrinsics = cam(aug, camera_index)
         loss, photo, smooth, geo = self.losses(tgt_img, ref_imgs, intrinsics)
         self.optimizer.zero_grad()
         loss.backward()

@@ -203,13 +203,6 @@ def gpu_augment_on(args):
     return args.gpu_augment if args.gpu_augment is not None else (0 if args.data == "synthetic" else 1)
 
 
-def training_scene_cameras(root):
-    """{scene: 3x3 K} of the training scenes listed in root/train.txt, read as the reference's SequenceFolder does (cam.txt)."""
-    with open(os.path.join(root, "train.txt")) as f:
-        scenes = [line.strip() for line in f if line.strip()]
-    return {s: np.genfromtxt(os.path.join(root, s, "cam.txt")).astype(np.float32).reshape(3, 3) for s in scenes}
-
-
 def _read_intrinsics(path):
     """A 3x3 float32 intrinsics file, read as the reference's SequenceFolder / PairFolder read it."""
     return np.genfromtxt(path).astype(np.float32).reshape(3, 3)
@@ -232,33 +225,44 @@ def _intrinsics_files(scene_dir, folder_type):
 
 
 class CameraTable:
-    """The cameras of --camera-groups calibration | scene.  Camera c stands for a group of samples: keys[c] is the group's key
-    (calibration: the float32 bytes of its intrinsics matrix; scene: its scene directory), labels[c] names it (the first
-    intrinsics file of the group, relative to DIR, or the scene) and Ks[c] is the matrix it starts from.  Cameras are numbered in
-    the order of the first train.txt scene that uses them, so every rank and every run builds the same table whatever the sample
-    shuffle."""
+    """The cameras of --camera-groups.  Camera c stands for a group of samples: keys[c] is the group's key (one, calibration: the
+    float32 bytes of its intrinsics matrix; scene: its scene directory), labels[c] names it (the first intrinsics file of the
+    group, relative to DIR, or the scene) and Ks[c] is the matrix it starts from.  Cameras are numbered in the order of the first
+    train.txt scene that uses them, so every rank and every run builds the same table whatever the sample shuffle.  'one' groups
+    as 'calibration' does, and learns a single camera (check_learn_intrinsics refuses more than one)."""
 
     def __init__(self, root, mode, folder_type="sequence"):
-        if mode not in ("calibration", "scene"):
-            raise ValueError("camera groups: 'calibration' or 'scene', got %r" % (mode,))
+        if mode not in ("one", "calibration", "scene"):
+            raise ValueError("camera groups: 'one', 'calibration' or 'scene', got %r" % (mode,))
         self.mode, self.keys, self.labels, self.Ks, self._index = mode, [], [], [], {}
         for scene in _training_scenes(root):
             d = os.path.join(root, scene)
             for f in _intrinsics_files(d, folder_type):
                 K = _read_intrinsics(f)
-                key = K.tobytes() if mode == "calibration" else os.path.abspath(d)
-                if key not in self._index:
-                    self._index[key] = len(self.keys)
-                    self.keys.append(key)
-                    self.labels.append(os.path.relpath(f, root) if mode == "calibration" else scene)
-                    self.Ks.append(K)
+                key = os.path.abspath(d) if mode == "scene" else K.tobytes()
+                self._add(key, scene if mode == "scene" else os.path.relpath(f, root), K)
+
+    @classmethod
+    def single(cls, K, label):
+        """One camera starting from K (DIR = synthetic)."""
+        table = cls.__new__(cls)
+        table.mode, table.keys, table.labels, table.Ks, table._index = "one", [], [], [], {}
+        table._add(K.tobytes(), label, K)
+        return table
+
+    def _add(self, key, label, K):
+        if key not in self._index:
+            self._index[key] = len(self.keys)
+            self.keys.append(key)
+            self.labels.append(label)
+            self.Ks.append(K)
 
     def __len__(self):
         return len(self.keys)
 
     def key(self, sample):
         """The group key of a reference dataset sample (an entry of SequenceFolder / PairFolder .samples)."""
-        if self.mode == "calibration":
+        if self.mode != "scene":
             return np.asarray(sample["intrinsics"], np.float32).reshape(3, 3).tobytes()
         return os.path.abspath(os.path.dirname(str(sample["tgt"])))
 
@@ -270,20 +274,18 @@ class CameraTable:
         """[C][fx, fy, cx, cy]: each group's intrinsics, or init (--intrinsics-init) for every camera."""
         return [list(init) if init is not None else [float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])] for K in self.Ks]
 
-
-def _initial_camera_arg(args):
-    if args.intrinsics_init is not None:
-        fx, fy, cx, cy = args.intrinsics_init
-        if not (fx > 0 and fy > 0):
-            raise SystemExit("--intrinsics-init: focal lengths must be positive, got fx %g fy %g" % (fx, fy))
-        return (fx, fy, cx, cy)
-    return None
+    def camera(self, init, height, width):
+        """The LearnedCamera of the table: one camera (theta [4]) for 'one', a bank (theta [C,4], labelled) otherwise."""
+        from scsfm.camera import LearnedCamera
+        if self.mode == "one":
+            return LearnedCamera(*self.thetas(init)[0], height, width)
+        return LearnedCamera.bank(self.thetas(init), height, width, groups=self.labels)
 
 
 def check_learn_intrinsics(args):
-    """--learn-intrinsics 1: the GPU transforms must be on (they hand out the augmentation records) and the training scenes must
-    share one camera.  Returns the initial (fx, fy, cx, cy); SystemExit with the reason otherwise.  With --camera-groups
-    calibration | scene the training scenes may have several cameras: returns their CameraTable."""
+    """--learn-intrinsics 1: the GPU transforms must be on (they hand out the augmentation records) and, with --camera-groups one,
+    the training scenes must share one camera.  Returns the CameraTable of the cameras to learn (None without
+    --learn-intrinsics); SystemExit with the reason otherwise."""
     groups = getattr(args, "camera_groups", "one")
     if groups != "one" and not args.learn_intrinsics:
         raise SystemExit("--camera-groups %s groups the cameras learned by --learn-intrinsics 1, which is off" % groups)
@@ -292,32 +294,24 @@ def check_learn_intrinsics(args):
     if not gpu_augment_on(args):
         raise SystemExit("--learn-intrinsics 1 needs the GPU transforms (--gpu-augment 1): the learned camera is built per sample "
                          "from the flip / zoom / crop records they hand out; learning K under the host-side chain is not supported")
-    if groups != "one":
-        if args.data == "synthetic":
-            raise SystemExit("--camera-groups %s: DIR = synthetic has one camera (use --camera-groups one)" % groups)
-        table = CameraTable(args.data, groups, args.folder_type)
-        if not len(table):
-            raise SystemExit("--learn-intrinsics 1: %s/train.txt lists no scene with intrinsics" % args.data)
-        _initial_camera_arg(args)
-        return table
     if args.data == "synthetic":
+        if groups != "one":
+            raise SystemExit("--camera-groups %s: DIR = synthetic has one camera (use --camera-groups one)" % groups)
         H, W = args.synthetic_size
-        K = synth.intrinsics(1, H, W, args.dataset)[0].numpy()
+        table = CameraTable.single(synth.intrinsics(1, H, W, args.dataset)[0].numpy(), "synthetic")
     else:
-        cams = training_scene_cameras(args.data)
-        if not cams:
-            raise SystemExit("--learn-intrinsics 1: %s/train.txt lists no scene" % args.data)
-        first = next(iter(cams.values()))
-        other = [s for s, K in cams.items() if not np.array_equal(K, first)]
-        if other:
-            raise SystemExit("--learn-intrinsics 1 learns ONE camera, but %d of the %d training scenes have a cam.txt different from "
-                             "the first's (e.g. %s): several cameras are not supported (--camera-groups calibration learns one "
-                             "camera per cam.txt)" % (len(other), len(cams), other[0]))
-        K = first
-    init = _initial_camera_arg(args)
-    if init is not None:
-        return init
-    return (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
+        table = CameraTable(args.data, groups, args.folder_type)
+    if not len(table):
+        raise SystemExit("--learn-intrinsics 1: %s/train.txt lists no scene with intrinsics" % args.data)
+    if groups == "one" and len(table) > 1:
+        raise SystemExit("--learn-intrinsics 1 learns ONE camera, but the training scenes have %d different intrinsics matrices "
+                         "(e.g. %s differs from %s): several cameras are not supported (--camera-groups calibration learns one "
+                         "camera per cam.txt)" % (len(table), table.labels[1], table.labels[0]))
+    if args.intrinsics_init is not None:
+        fx, fy = args.intrinsics_init[:2]
+        if not (fx > 0 and fy > 0):
+            raise SystemExit("--intrinsics-init: focal lengths must be positive, got fx %g fy %g" % (fx, fy))
+    return table
 
 
 def make_loaders(args, rank, world, device="cuda", cameras=None):
@@ -411,7 +405,7 @@ def training_size(args, train_loader):
 def main():
     global best_error, n_iter
     args = parser.parse_args()
-    init = check_learn_intrinsics(args)
+    cameras = check_learn_intrinsics(args)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -429,8 +423,8 @@ def main():
         os.makedirs(args.save_path, exist_ok=True)
     torch.manual_seed(args.seed)
 
-    table = init if isinstance(init, CameraTable) else None
-    train_loader, val_loader = make_loaders(args, rank, world, device, table)
+    bank = cameras is not None and cameras.mode != "one"          # every sample then carries its camera index
+    train_loader, val_loader = make_loaders(args, rank, world, device, cameras if bank else None)
     if args.epoch_size == 0:
         args.epoch_size = len(train_loader)
 
@@ -446,14 +440,10 @@ def main():
     if args.pretrained_pose:
         pose_net.load_state_dict(torch.load(args.pretrained_pose, map_location=device)["state_dict"], strict=False)
     camera = None
-    if table is not None:
-        from scsfm.camera import LearnedCamera
-        camera = LearnedCamera.bank(table.thetas(args.intrinsics_init), *training_size(args, train_loader), groups=table.labels).to(device)
-        if rank == 0:
-            print("=> learning {} cameras (--camera-groups {})".format(len(table), args.camera_groups))
-    elif init is not None:
-        from scsfm.camera import LearnedCamera
-        camera = LearnedCamera(*init, *training_size(args, train_loader)).to(device)
+    if cameras is not None:
+        camera = cameras.camera(args.intrinsics_init, *training_size(args, train_loader)).to(device)
+        if bank and rank == 0:
+            print("=> learning {} cameras (--camera-groups {})".format(len(cameras), args.camera_groups))
 
     trainer = Trainer(disp_net, pose_net, lr=args.lr, betas=(args.momentum, args.beta), weight_decay=args.weight_decay,
                       num_scales=args.num_scales, with_ssim=args.with_ssim, with_mask=args.with_mask,
@@ -478,13 +468,14 @@ def main():
         if rank == 0:
             print(" * epoch {} train loss {:.4f} | ".format(epoch, train_loss) +
                   ", ".join("{} : {:.3f}".format(n, e) for n, e in zip(names, errors)))
-            if table is not None:
-                for c, (label, th) in enumerate(zip(camera.groups, camera.theta.tolist())):
-                    K = table.Ks[c]
-                    print(" * epoch {} camera {} {}: learned fx {:.3f} fy {:.3f} cx {:.3f} cy {:.3f} | cam.txt fx {:.3f} fy {:.3f} "
-                          "cx {:.3f} cy {:.3f}".format(epoch, c, label, *th, K[0, 0], K[1, 1], K[0, 2], K[1, 2]))
-            elif camera is not None:
-                print(" * epoch {} learned camera fx {:.3f} fy {:.3f} cx {:.3f} cy {:.3f}".format(epoch, *camera.theta.tolist()))
+            for c, th in enumerate([] if camera is None else camera.theta.reshape(-1, 4).tolist()):
+                learned = "fx {:.3f} fy {:.3f} cx {:.3f} cy {:.3f}".format(*th)
+                if camera.groups is None:
+                    print(" * epoch {} learned camera {}".format(epoch, learned))
+                else:                                   # a bank: each camera beside its group's cam.txt
+                    K = cameras.Ks[c]
+                    print(" * epoch {} camera {} {}: learned {} | cam.txt fx {:.3f} fy {:.3f} cx {:.3f} cy {:.3f}".format(
+                        epoch, c, camera.groups[c], learned, K[0, 0], K[1, 1], K[0, 2], K[1, 2]))
             decisive = errors[1]
             if best_error < 0:
                 best_error = decisive
@@ -494,7 +485,7 @@ def main():
                             {"epoch": epoch + 1, "state_dict": pose_net.state_dict()}, is_best)
             if camera is not None:
                 state = {"epoch": epoch + 1, "state_dict": camera.state_dict()}
-                if table is not None:
+                if camera.groups is not None:
                     state["groups"] = list(camera.groups)
                 save_camera_checkpoint(args.save_path, state, is_best)
             with open(os.path.join(args.save_path, args.log_summary), "a") as f:
@@ -557,12 +548,10 @@ def validate_without_gt(args, val_loader, disp_net, pose_net, device, camera=Non
         intrinsics = intrinsics.to(device)
         if camera is not None:
             from scsfm.camera import identity_records
-            rec = identity_records(tgt_img.shape[0], tgt_img.shape[-1], device)
-            if camera.theta.dim() == 1:
-                intrinsics = camera(rec)
-            else:                                     # (an index of -1 builds a NaN K, which the where() drops)
-                idx = batch[4]
-                intrinsics = torch.where((idx >= 0)[:, None, None], camera(rec, idx), intrinsics)
+            idx = batch[4] if len(batch) > 4 else None        # a bank's camera index
+            K = camera(identity_records(tgt_img.shape[0], tgt_img.shape[-1], device), idx)
+            # (an index of -1 builds a NaN K, which the where() drops)
+            intrinsics = K if idx is None else torch.where((idx >= 0)[:, None, None], K, intrinsics)
         tgt_depth = [1 / disp_net(tgt_img)]
         ref_depths = [[1 / disp_net(r)] for r in ref_imgs]
         poses = [pose_net(tgt_img, r) for r in ref_imgs]

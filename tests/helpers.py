@@ -1,4 +1,6 @@
 """Shared helpers for the parity tests."""
+import socket
+
 import numpy as np
 import torch
 
@@ -91,3 +93,12 @@ def reference_loader_env():
     env["PYTHONPATH"] = os.pathsep.join([stubs, ref] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
     env["PYTHONDONTWRITEBYTECODE"] = "1"
     return env
+
+
+def free_port():
+    """A free TCP port on 127.0.0.1 for a process group's rendezvous."""
+    s = socket.socket()
+    s.bind(("127.0.0.1", 0))
+    p = s.getsockname()[1]
+    s.close()
+    return p

@@ -1,6 +1,7 @@
-"""The learned camera, CPU side: the C ABI of scsfm_camera_build / scsfm_camera_grad (declared, exported, argument errors reported
-without a launch), the augmentation record derived from a Draw (a numpy restatement of the build kernel's arithmetic reproduces
-update_intrinsics bit for bit), and train.py's --learn-intrinsics validation."""
+"""The learned camera, CPU side: the C ABI (one build and one gradient entry, scsfm_camera_build_indexed /
+scsfm_camera_grad_indexed, whose null camera index means one camera; argument errors reported without a launch), the augmentation
+record derived from a Draw (a numpy restatement of the build kernel's arithmetic reproduces update_intrinsics bit for bit), and
+train.py's --learn-intrinsics validation."""
 import ctypes
 import os
 import random
@@ -9,58 +10,57 @@ import re
 import numpy as np
 import pytest
 
+from camera_helpers import kernel_build
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def kernel_build(theta, rec):
-    """scsfm_camera_build restated in numpy for one record: float32 subtractions for the flip and the crop, float64 products
-    rounded to float32 for the zoom (csrc/camera.cu)."""
-    xs, ys, flip, ox, oy, in_w = rec
-    f32, f64 = np.float32, np.float64
-    fx, fy, cx, cy = (f32(v) for v in theta)
-    if flip != 0.0:
-        cx = f32(f32(in_w) - cx)
-    K = np.zeros((3, 3), np.float32)
-    K[0, 0] = f32(f64(fx) * f64(xs))
-    K[0, 2] = f32(f32(f64(cx) * f64(xs)) - f32(ox))
-    K[1, 1] = f32(f64(fy) * f64(ys))
-    K[1, 2] = f32(f32(f64(cy) * f64(ys)) - f32(oy))
-    K[2, 2] = 1.0
-    return K
-
-
-def test_header_declares_and_library_exports_the_camera_entries():
+def test_header_and_library_have_only_the_indexed_camera_entries():
+    """The indexed entries are the only camera entries: the one-camera entries scsfm_camera_build / scsfm_camera_grad are gone."""
     src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "scsfm.h")).read(), flags=re.S)
-    for name in ("scsfm_camera_build", "scsfm_camera_grad"):
+    for name in ("scsfm_camera_build_indexed", "scsfm_camera_grad_indexed"):
         assert re.search(r"\b%s\s*\(" % name, src), name
+    for name in ("scsfm_camera_build", "scsfm_camera_grad"):
+        assert not re.search(r"\b%s\s*\(" % name, src), name
     assert re.search(r"#define SCSFM_CAMERA_AUG_DOUBLES 6\b", src)
     from scsfm import camera
     from scsfm import lib
     assert camera.AUG_DOUBLES == 6
     L = lib.load()
-    assert hasattr(L, "scsfm_camera_build") and hasattr(L, "scsfm_camera_grad")
+    assert hasattr(L, "scsfm_camera_build_indexed") and hasattr(L, "scsfm_camera_grad_indexed")
+    assert not hasattr(L, "scsfm_camera_build") and not hasattr(L, "scsfm_camera_grad")
 
 
-def test_camera_entries_reject_bad_arguments_without_a_launch():
+def test_null_camera_index_means_one_camera_and_bad_arguments_launch_nothing():
+    """A null camera index passes the argument checks with one camera (the call below then fails on its batch size) and is
+    refused with more; the other refusals hold for one camera as well."""
     from scsfm import camera
     from scsfm import lib
     L = camera._lib()
     n0 = lib.launch_count()
     fake = ctypes.c_void_p(16)            # never dereferenced: every call below fails its argument check first
-    assert L.scsfm_camera_build(None, fake, 1, fake, None) == -1
-    assert b"camera_build" in L.scsfm_last_error() and b"theta" in L.scsfm_last_error()
-    assert L.scsfm_camera_build(fake, None, 1, fake, None) == -1
-    assert L.scsfm_camera_build(fake, fake, 1, None, None) == -1
-    assert L.scsfm_camera_build(fake, fake, 0, fake, None) == -1
+    assert L.scsfm_camera_build_indexed(fake, 1, fake, None, 0, fake, None) == -1
     assert b"batch size" in L.scsfm_last_error()
-    assert L.scsfm_camera_grad(None, fake, 1, fake, None) == -1
+    assert L.scsfm_camera_build_indexed(fake, 2, fake, None, 1, fake, None) == -1
+    assert b"camera_build_indexed" in L.scsfm_last_error() and b"null idx" in L.scsfm_last_error()
+    assert L.scsfm_camera_grad_indexed(fake, None, fake, 0, 1, fake, None) == -1
+    assert b"batch size" in L.scsfm_last_error()
+    assert L.scsfm_camera_grad_indexed(fake, None, fake, 1, 2, fake, None) == -1
+    assert b"camera_grad_indexed" in L.scsfm_last_error() and b"null idx" in L.scsfm_last_error()
+    assert L.scsfm_camera_build_indexed(None, 1, fake, None, 1, fake, None) == -1
+    assert b"camera_build" in L.scsfm_last_error() and b"theta" in L.scsfm_last_error()
+    assert L.scsfm_camera_build_indexed(fake, 1, None, None, 1, fake, None) == -1
+    assert L.scsfm_camera_build_indexed(fake, 1, fake, None, 1, None, None) == -1
+    assert L.scsfm_camera_build_indexed(fake, 1, fake, None, 0, fake, None) == -1
+    assert b"batch size" in L.scsfm_last_error()
+    assert L.scsfm_camera_grad_indexed(None, None, fake, 1, 1, fake, None) == -1
     assert b"camera_grad" in L.scsfm_last_error()
-    assert L.scsfm_camera_grad(fake, None, 1, fake, None) == -1
-    assert L.scsfm_camera_grad(fake, fake, 1, None, None) == -1
-    assert L.scsfm_camera_grad(fake, fake, -3, fake, None) == -1
+    assert L.scsfm_camera_grad_indexed(fake, None, None, 1, 1, fake, None) == -1
+    assert L.scsfm_camera_grad_indexed(fake, None, fake, 1, 1, None, None) == -1
+    assert L.scsfm_camera_grad_indexed(fake, None, fake, -3, 1, fake, None) == -1
     assert b"batch size" in L.scsfm_last_error()
     with pytest.raises(ValueError, match="camera_grad"):
-        lib.check(L.scsfm_camera_grad(None, None, 1, None, None), "scsfm_camera_grad")
+        lib.check(L.scsfm_camera_grad_indexed(None, None, None, 1, 1, None, None), "scsfm_camera_grad_indexed")
     assert lib.launch_count() == n0
 
 
@@ -133,14 +133,14 @@ def test_learn_intrinsics_needs_the_gpu_transforms():
         T.check_learn_intrinsics(T.parser.parse_args(["some/dir", "--name", "x", "--learn-intrinsics", "1", "--gpu-augment", "0"]))
 
 
-def test_learn_intrinsics_initial_camera():
+def test_learn_intrinsics_initial_camera_table():
     import train as T
     from scsfm import synth
-    got = T.check_learn_intrinsics(_args("--learn-intrinsics", "1", "--gpu-augment", "1", "--synthetic-size", "128", "416"))
+    t = T.check_learn_intrinsics(_args("--learn-intrinsics", "1", "--gpu-augment", "1", "--synthetic-size", "128", "416"))
     K = synth.intrinsics(1, 128, 416)[0]
-    assert got == (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
-    got = T.check_learn_intrinsics(_args("--learn-intrinsics", "1", "--gpu-augment", "1", "--intrinsics-init", "100", "110", "60", "30"))
-    assert got == (100.0, 110.0, 60.0, 30.0)
+    assert t.mode == "one" and t.thetas() == [[float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])]]
+    a = _args("--learn-intrinsics", "1", "--gpu-augment", "1", "--intrinsics-init", "100", "110", "60", "30")
+    assert T.check_learn_intrinsics(a).thetas(a.intrinsics_init) == [[100.0, 110.0, 60.0, 30.0]]
     with pytest.raises(SystemExit, match="positive"):
         T.check_learn_intrinsics(_args("--learn-intrinsics", "1", "--gpu-augment", "1", "--intrinsics-init", "-100", "110", "60", "30"))
 
@@ -154,15 +154,23 @@ def _scenes(root, cams):
         np.savetxt(os.path.join(root, s, "cam.txt"), np.asarray(K, np.float32))
 
 
-def test_learn_intrinsics_reads_the_first_scene_and_refuses_several_cameras(tmp_path):
+K1 = [[241.67, 0, 204.17], [0, 246.28, 59.0], [0, 0, 1]]
+K2 = [[245.0, 0, 200.0], [0, 246.28, 59.0], [0, 0, 1]]
+
+
+def _theta(K):
+    K = np.asarray(K, np.float32)
+    return [float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])]
+
+
+def test_one_camera_table_reads_the_scenes_and_refuses_several_cameras(tmp_path):
     import train as T
-    K1 = [[241.67, 0, 204.17], [0, 246.28, 59.0], [0, 0, 1]]
-    K2 = [[245.0, 0, 200.0], [0, 246.28, 59.0], [0, 0, 1]]
     one = str(tmp_path / "one")
     _scenes(one, {"seq_a": K1, "seq_b": K1})
     args = T.parser.parse_args([one, "--name", "x", "--learn-intrinsics", "1"])        # real data: GPU transforms by default
-    want = np.asarray(K1, np.float32)
-    assert T.check_learn_intrinsics(args) == (float(want[0, 0]), float(want[1, 1]), float(want[0, 2]), float(want[1, 2]))
+    t = T.check_learn_intrinsics(args)
+    assert len(t) == 1 and t.thetas() == [_theta(K1)]
+    assert t.camera(None, 10, 20).groups is None and tuple(t.camera(None, 10, 20).theta.shape) == (4,)
     two = str(tmp_path / "two")
     _scenes(two, {"seq_a": K1, "seq_b": K2})
     with pytest.raises(SystemExit, match="ONE camera.*seq_b"):
@@ -171,3 +179,24 @@ def test_learn_intrinsics_reads_the_first_scene_and_refuses_several_cameras(tmp_
     with pytest.raises(SystemExit, match="ONE camera"):
         T.check_learn_intrinsics(T.parser.parse_args([two, "--name", "x", "--learn-intrinsics", "1", "--intrinsics-init", "240", "240",
                                                       "200", "60"]))
+
+
+def test_learn_intrinsics_of_a_pair_folder_reads_its_pair_files(tmp_path):
+    """--folder-type pair with one camera: the intrinsics files PairFolder reads (one per image pair; there is no cam.txt) are the
+    ones checked and the camera starts from them."""
+    import train as T
+    root = str(tmp_path / "p")
+    for s, Ks in {"s1": [K1, K1], "s2": [K1, K2]}.items():
+        os.makedirs(os.path.join(root, s))
+        for i in range(4):
+            open(os.path.join(root, s, "%07d.jpg" % i), "wb").close()
+        for i, K in enumerate(Ks):
+            np.savetxt(os.path.join(root, s, "%07d.txt" % i), np.asarray(K, np.float32))
+    with open(os.path.join(root, "train.txt"), "w") as f:
+        f.write("s1\n")
+    args = T.parser.parse_args([root, "--name", "x", "--learn-intrinsics", "1", "--folder-type", "pair"])
+    assert T.check_learn_intrinsics(args).thetas() == [_theta(K1)]
+    with open(os.path.join(root, "train.txt"), "w") as f:
+        f.write("s1\ns2\n")
+    with pytest.raises(SystemExit, match="ONE camera.*" + re.escape(os.path.join("s2", "0000001.txt"))):
+        T.check_learn_intrinsics(args)

@@ -1,47 +1,22 @@
 """The learned camera on the GPU: the build kernel against GpuAugment's K (bit for bit), its gradient against fp64 autograd, the
-Trainer that owns a camera (eager against the fp64 oracle, captured against eager, without a camera unchanged, data parallel at
-world size 1 and on two GPUs) and self-calibration of all four intrinsics on a synthetic scene with a captured step."""
+Trainer that owns a camera (eager against the fp64 oracle, captured against eager, argument errors, data parallel at world size 1
+and on two GPUs: the checks of tests/camera_helpers.py with cameras = 1), the Trainer without a camera unchanged, and
+self-calibration of all four intrinsics on a synthetic scene with a captured step."""
 import os
 import random
-import socket
 import subprocess
 import sys
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
+from camera_helpers import (DEV, bank_build, captured_steps_track_eager, eager_step_vs_oracle, make_trainer, render_plane,
+                            seeded_records, theta_of, trainer_argument_errors, two_gpu_check, world_of_one)
 from helpers import rel_l2
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def torch_build(theta, rec):
-    """K_b(theta) restated in torch (differentiable; the dtype of theta), rec: float64 [B,6] records."""
-    rec = rec.to(theta.device, theta.dtype)
-    xs, ys, flip, ox, oy, in_w = rec.unbind(1)
-    fx, fy, cx, cy = theta.unbind(0)
-    cxb = torch.where(flip != 0, in_w - cx, cx)
-    zero, one = torch.zeros_like(xs), torch.ones_like(xs)
-    rows = [torch.stack([fx * xs, zero, cxb * xs - ox], 1), torch.stack([zero, fy * ys, cy * ys - oy], 1),
-            torch.stack([zero, zero, one], 1)]
-    return torch.stack(rows, 1)
-
-
-def seeded_records(seed, B, H, W):
-    from scsfm.augment import Draw
-    from scsfm.camera import record_rows
-    random.seed(seed)
-    np.random.seed(seed)
-    rows = record_rows([Draw.random(H, W) for _ in range(B)], W)
-    return torch.from_numpy(rows)
-
-
-def theta_of(K):
-    return torch.tensor([K[0, 0], K[1, 1], K[0, 2], K[1, 2]], dtype=torch.float32)
 
 
 @pytest.mark.parametrize("kind,H,W", [("kitti", 256, 832), ("nyu", 256, 320)])
@@ -76,7 +51,7 @@ def test_grad_matches_fp64_autograd_and_is_deterministic(B):
     gen = torch.Generator().manual_seed(B)
     dK = torch.randn(B, 3, 3, generator=gen)
     th64 = torch.tensor([483.4, 492.6, 408.3, 118.0], dtype=torch.float64, requires_grad=True)
-    (torch_build(th64, rec) * dK.double()).sum().backward()
+    (bank_build(th64[None], rec, torch.zeros(B, dtype=torch.long)) * dK.double()).sum().backward()
     runs = []
     for _ in range(2):
         d = torch.full((4,), 0.25, device=DEV)                             # the entry ADDS into dtheta
@@ -90,111 +65,12 @@ def test_grad_matches_fp64_autograd_and_is_deterministic(B):
     assert rel_l2(cam.theta.grad.cpu(), th64.grad) < 1e-6
 
 
-def _nets():
-    import models
-    from golden_util import det_weights
-    d, p = models.DispResNet(18, False), models.PoseResNet(18, False)
-    for n in (d, p):
-        n.load_state_dict(det_weights(n.state_dict()))
-    return d.to(DEV).train(), p.to(DEV).train()
-
-
-def _trainer(mode="fp32", theta=None, **kw):
-    from scsfm.camera import LearnedCamera
-    from scsfm.trainer import Trainer
-    d, p = _nets()
-    cam = None if theta is None else LearnedCamera(*[float(v) for v in theta]).to(DEV)
-    kw.setdefault("distributed", False)
-    return Trainer(d, p, lr=1e-4, with_auto_mask=0, conv_mode=mode, camera=cam, **kw)
-
-
 def test_eager_camera_step_gives_the_oracle_theta_gradient():
-    """theta.grad of an eager step against oracle.step.train_step in fp64 with K_b built from theta; yardstick and bound of
-    test_trainer_eager_step_gives_the_oracle_intrinsics_gradient (4x the larger fp32 error + 1e-3)."""
-    from golden_util import det_weights
-    from oracle import nets as N
-    from oracle import step as OS
-    from scsfm import synth
-    B, H, W = 2, 96, 160
-    tgt, refs, K = synth.triplet(5, B, H, W)
-    rec = seeded_records(11, B, H, W)
-    th0 = theta_of(K[0]) * torch.tensor([1.05, 0.97, 1.0, 1.0]) + torch.tensor([0.0, 0.0, 2.0, -1.5])
-    tr = _trainer("fp32", th0)
-    tr.step(tgt.to(DEV), [r.to(DEV) for r in refs], aug=rec.to(DEV))
-    mine = tr.camera.theta.grad.cpu()
-    assert not torch.equal(tr.camera.theta.detach().cpu(), th0)           # Adam moved theta
-    want = {}
-    tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        for key, dt, dev in (("64", torch.float64, "cpu"), ("32", torch.float32, "cpu"), ("32gpu", torch.float32, DEV)):
-            d, p = N.DispResNet(18).to(dt).to(dev), N.PoseResNet(18).to(dt).to(dev)
-            for n in (d, p):
-                n.load_state_dict({k: v.to(dt) for k, v in det_weights(n.state_dict()).items()})
-                n.train()
-            th = th0.to(dev, dt, copy=True).requires_grad_(True)
-            OS.train_step(d, p, OS.make_optimizer(d, p, lr=1e-4), tgt.to(dev, dt), [r.to(dev, dt) for r in refs], torch_build(th, rec),
-                          num_scales=1, with_ssim=1, with_mask=1, with_auto_mask=0)
-            want[key] = th.grad.cpu()
-    finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
-    errs = {k: rel_l2(g, want["64"]) for k, g in (("mine", mine), ("32", want["32"]), ("32gpu", want["32gpu"]))}
-    print("camera dtheta rel_l2 vs fp64: mine %.3g | fp32 CPU oracle %.3g | stock PyTorch fp32 on this GPU %.3g" %
-          (errs["mine"], errs["32"], errs["32gpu"]))
-    assert errs["mine"] < 4 * max(errs["32"], errs["32gpu"]) + 1e-3
+    eager_step_vs_oracle(1)
 
 
 def test_captured_camera_steps_track_eager_steps():
-    """Captured steps with a camera against the same eager steps (theta, losses, parameters) within the tolerances of
-    test_cuda_graph_replay_matches_eager_steps; capture() leaves theta and its Adam state bitwise unchanged.  The first step, from
-    identical states, gives the eager camera gradient and update; every replay applies Adam to the gradient it computed."""
-    from scsfm import synth
-    B, H, W = 2, 96, 160
-    tgt, refs, K = synth.triplet(2, B, H, W)
-    th0 = theta_of(K[0]) * 1.1
-    eager, graphed = _trainer("tf32x3", th0), _trainer("tf32x3", th0)
-    batches = [(tgt.to(DEV), [r.to(DEV) for r in refs], seeded_records(20 + i, B, H, W).to(DEV)) for i in range(4)]
-    before = [t.clone() for t in (graphed.camera.theta.detach(),) + graphed._cam_state]
-    graphed.capture(batches[0][0], batches[0][1], aug=batches[0][2])
-    torch.cuda.synchronize()
-    for a, b in zip(before, (graphed.camera.theta.detach(),) + graphed._cam_state):
-        assert torch.equal(a, b)
-    assert graphed.optimizer.step_count == 0
-    lr = eager.camera_lr
-    grads = {"eager": [], "captured": []}
-    for it, (t, r, rec) in enumerate(batches[1:]):
-        a = [float(v) for v in eager.step(t, r, aug=rec)]
-        b = [float(v) for v in graphed.step(t, r, aug=rec)]
-        np.testing.assert_allclose(b, a, rtol=2e-4 if it == 0 else 5e-3)
-        # the camera gradient the graph computes (theta.grad is the graph's own buffer); the first step starts from identical
-        # states, so it and its update are those of the eager step (measured on an H100: the same bits)
-        g_e, g_g = eager.camera.theta.grad.cpu(), graphed.camera.theta.grad.cpu()
-        print("step %d dtheta: eager %s captured %s rel %.2e" % (it, g_e.tolist(), g_g.tolist(), rel_l2(g_g, g_e)))
-        if it == 0:
-            assert rel_l2(g_g, g_e) < 1e-4
-            assert float((graphed.camera.theta - eager.camera.theta).abs().max()) < 1e-4
-        grads["eager"].append(g_e)
-        grads["captured"].append(g_g)
-    torch.cuda.synchronize()
-    # each run's theta is torch.optim.Adam (fp64) applied to that run's own gradients: the update happens in the graph, every replay
-    for name, th in (("eager", eager.camera.theta), ("captured", graphed.camera.theta)):
-        ref = th0.double().clone().requires_grad_(True)
-        opt = torch.optim.Adam([ref], lr=lr, betas=(0.9, 0.999), eps=1e-8)
-        for g in grads[name]:
-            ref.grad = g.double()
-            opt.step()
-        assert float((th.detach().cpu().double() - ref.detach()).abs().max()) < 1e-4, (name, th, ref)
-    assert graphed.camera_state_dict()["step"] == 3 and eager.camera_state_dict()["step"] == 3
-    th_e, th_g = eager.camera.theta.detach().cpu(), graphed.camera.theta.detach().cpu()
-    print("theta after 3 steps: eager", th_e.tolist(), "captured", th_g.tolist(), "start", th0.tolist())
-    assert float((th_e - th0).abs().min()) > 0                              # every parameter moved
-    # Later steps: theta and the networks' parameters against the bound of test_cuda_graph_replay_matches_eager_steps, 3 steps x
-    # 2 lr (+ fp32 rounding of the 100-pixel values).  Adam normalises each component's step, so a component whose gradient is at
-    # the level of the fp32 atomics noise of the networks' backward (fx here: K enters the warp through K t, and a freshly
-    # initialised PoseResNet gives near-zero translations) can step either way in the two runs, whatever its size; the gradients
-    # of the next step then follow the two different theta.
-    assert float((th_g - th_e).abs().max()) <= 3 * 2 * lr + 1e-4
-    assert float((graphed.disp_net.flat_params() - eager.disp_net.flat_params()).abs().max()) <= 6.1e-4
+    captured_steps_track_eager(1)
 
 
 def test_no_camera_step_is_unchanged_and_the_camera_path_adds_four_launches():
@@ -209,7 +85,7 @@ def test_no_camera_step_is_unchanged_and_the_camera_path_adds_four_launches():
     from scsfm.camera import identity_records
     runs = {}
     for name, th in (("plain", None), ("camera", theta_of(K[0]))):
-        tr = _trainer("tf32x3", th)
+        tr = make_trainer("tf32x3", th)
         inp = dict(intrinsics=K.to(DEV)) if th is None else dict(aug=identity_records(B, W))
         torch.cuda.synchronize()
         n0 = L.launch_count()
@@ -226,97 +102,19 @@ def test_no_camera_step_is_unchanged_and_the_camera_path_adds_four_launches():
 
 
 def test_trainer_camera_argument_errors():
-    from scsfm import synth
-    tgt, refs, K = synth.triplet(6, 2, 64, 128)
-    c = lambda x: x.to(DEV)  # noqa: E731
-    tr = _trainer("fp32", theta_of(K[0]))
-    with pytest.raises(ValueError, match="owns a learned camera"):
-        tr.step(c(tgt), [c(r) for r in refs], c(K))
-    with pytest.raises(TypeError, match="records"):
-        tr.step(c(tgt), [c(r) for r in refs])
-    with pytest.raises(TypeError, match="float64"):
-        tr.step(c(tgt), [c(r) for r in refs], aug=torch.zeros(2, 6, device=DEV))
-    plain = _trainer("fp32")
-    with pytest.raises(TypeError, match="camera"):
-        plain.step(c(tgt), [c(r) for r in refs], c(K), aug=torch.zeros(2, 6, dtype=torch.float64, device=DEV))
+    trainer_argument_errors(1)
 
 
 def test_data_parallel_world_of_one_gives_the_single_gpu_theta():
-    import torch.distributed as dist
-    from scsfm import synth
-    B, H, W = 2, 96, 160
-    tgt, refs, K = synth.triplet(8, B, H, W)
-    rec = seeded_records(3, B, H, W).to(DEV)
-    args = (tgt.to(DEV), [r.to(DEV) for r in refs])
-    th0 = theta_of(K[0]) * 0.9
-    single = _trainer("tf32x3", th0)
-    single.step(*args, aug=rec)
-    with tempfile.TemporaryDirectory() as tmp:
-        dist.init_process_group("nccl", init_method="file://" + os.path.join(tmp, "rendezvous"), rank=0, world_size=1,
-                                device_id=torch.device(DEV, torch.cuda.current_device()))
-        try:
-            ddp = _trainer("tf32x3", th0, distributed=True)
-            ddp.step(*args, aug=rec)
-            torch.cuda.synchronize()
-            assert ddp.exchange.pending() == 0
-            print("world 1 dtheta", ddp.camera.theta.grad.tolist(), "single", single.camera.theta.grad.tolist())
-            assert rel_l2(ddp.camera.theta.grad.cpu(), single.camera.theta.grad.cpu()) < 1e-5
-            assert float((ddp.camera.theta - single.camera.theta).abs().max()) < 1e-4
-        finally:
-            dist.destroy_process_group()
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+    world_of_one(1)
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_data_parallel_camera_on_two_gpus():
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(_free_port()), os.path.join(ROOT, "tests", "camera_ddp_check.py")]
-    out = subprocess.run(cmd, capture_output=True, text=True, timeout=1500)
-    print(out.stdout[-4000:])
-    assert out.returncode == 0, out.stderr[-4000:]
-    for mode in ("eager", "graph"):
-        assert "CAMERA_DDP_OK %s" % mode in out.stdout
+    two_gpu_check(1)
 
 
 # ---- self-calibration on a synthetic scene -------------------------------------------------------------------------------------
-def render_plane(theta, rec, H, W, Z0, t, seed):
-    """A textured fronto-parallel plane Z = Z0 (target camera coordinates) seen by the target camera and by a reference camera
-    at P_ref = P_tgt + t_b (t: fp64 [B,3], one translation per sample), both with the sample's augmented intrinsics
-    K_b = aug_b(theta); the texture is a seeded sum of sinusoids of the plane's metric coordinates, evaluated exactly (fp64) at
-    every pixel of both views.  Returns tgt, ref [B,3,H,W] float32, the two constant depth maps and the pose vectors
-    target->reference and back."""
-    B = rec.shape[0]
-    K = torch_build(torch.as_tensor(theta, dtype=torch.float64), rec).to(DEV)
-    g = torch.Generator().manual_seed(seed)
-    n = 12
-    lam = 1.0 + 2.0 * torch.rand(B, 3, n, 2, generator=g, dtype=torch.float64)          # wavelengths 1..3 m: 20..60 px at Z0
-    ang = 2 * np.pi * torch.rand(B, 3, n, generator=g, dtype=torch.float64)
-    kx = (2 * np.pi / lam[..., 0] * torch.cos(ang)).to(DEV)
-    ky = (2 * np.pi / lam[..., 1] * torch.sin(ang)).to(DEV)
-    ph = (2 * np.pi * torch.rand(B, 3, n, generator=g, dtype=torch.float64)).to(DEV)
-    v, u = torch.meshgrid(torch.arange(H, dtype=torch.float64, device=DEV), torch.arange(W, dtype=torch.float64, device=DEV),
-                          indexing="ij")
-    fx, fy, cx, cy = (K[:, 0, 0, None, None], K[:, 1, 1, None, None], K[:, 0, 2, None, None], K[:, 1, 2, None, None])
-
-    def tex(X, Y):                       # X, Y [B,H,W] -> [B,3,H,W]
-        arg = kx[..., None, None] * X[:, None, None] + ky[..., None, None] * Y[:, None, None] + ph[..., None, None]
-        return (0.9 * torch.cos(arg).mean(2)).float()
-    tgt = tex((u - cx) * Z0 / fx, (v - cy) * Z0 / fy)
-    tx, ty, tz = (t[:, i, None, None].to(DEV) for i in range(3))
-    Zr = Z0 + tz
-    ref = tex((u - cx) * Zr / fx - tx, (v - cy) * Zr / fy - ty)
-    pose = torch.cat([t, torch.zeros(B, 3, dtype=torch.float64)], 1).float().to(DEV)
-    ref_depth = Zr.float().expand(B, H, W)[:, None].contiguous()
-    return tgt, ref, torch.full((B, 1, H, W), Z0, device=DEV), ref_depth, pose, -pose
-
-
 def test_captured_self_calibration_recovers_the_camera():
     """The camera path alone in a captured step (K_b from theta, photometric + geometry loss, theta's gradient, Adam at the
     default --intrinsics-lr 0.1), on a plane at Z0 = 10 m rendered exactly for every augmented camera, each sample with its own

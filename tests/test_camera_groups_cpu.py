@@ -12,17 +12,10 @@ import sys
 import numpy as np
 import pytest
 
-from test_camera_cpu import kernel_build
+from camera_helpers import indexed_build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "sc-sfmlearner-release_b200")
-
-
-def indexed_build(thetas, rec, idx):
-    """scsfm_camera_build_indexed restated: camera idx of thetas through the record, nine NaNs for an index out of range."""
-    if not 0 <= idx < len(thetas):
-        return np.full((3, 3), np.nan, np.float32)
-    return kernel_build(thetas[idx], rec)
 
 
 def test_header_declares_and_library_exports_the_indexed_entries():
@@ -134,14 +127,17 @@ FOUR = {"2011_09_28_drive_0001_sync_02": K_B, "2011_09_26_drive_0001_sync_02": K
         "2011_09_28_drive_0002_sync_03": K_B}
 
 
-def test_camera_groups_defaults():
+def test_camera_groups_default_to_a_one_camera_table():
     import train as T
     a = _parse("synthetic", "--name", "x")
     assert a.camera_groups == "one"
     assert T.check_learn_intrinsics(a) is None
-    # with 'one' the returned initial camera is today's tuple
+    # with 'one' the table holds one camera, learned as theta [4] with no group labels
     a = _parse("synthetic", "--name", "x", "--learn-intrinsics", "1", "--gpu-augment", "1")
-    assert isinstance(T.check_learn_intrinsics(a), tuple)
+    t = T.check_learn_intrinsics(a)
+    assert isinstance(t, T.CameraTable) and t.mode == "one" and len(t) == 1
+    cam = t.camera(None, 256, 832)
+    assert tuple(cam.theta.shape) == (4,) and cam.groups is None
 
 
 def test_camera_groups_refusals(tmp_path):

@@ -1,35 +1,24 @@
 """A bank of learned cameras on the GPU: the indexed build against GpuAugment's K (bit for bit), one camera through the bank against
-the single-camera path (bit for bit), the per-camera gradient against fp64 autograd, the Trainer with a bank (eager against the
-fp64 oracle, dense Adam against torch.optim.Adam, captured against eager, launch counts, data parallel at world size 1 and on two
-GPUs), self-calibration of two cameras at once, and train.py --camera-groups calibration on a dataset on disk."""
+the single-camera path (bit for bit), the per-camera gradient against fp64 autograd, the Trainer with a bank (a bank of one against
+one camera, dense Adam against torch.optim.Adam, and with two cameras the checks of tests/camera_helpers.py that one camera runs
+too: eager against the fp64 oracle, captured against eager, argument errors, data parallel at world size 1 and on two GPUs),
+self-calibration of two cameras at once, and train.py --camera-groups calibration on a dataset on disk."""
 import os
 import random
 import subprocess
 import sys
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
+from camera_helpers import (DEV, bank_build, captured_steps_track_eager, eager_step_vs_oracle, make_trainer, render_plane,
+                            seeded_records, theta_of, trainer_argument_errors, two_gpu_check, world_of_one)
 from helpers import rel_l2
-from test_camera_gpu import _free_port, _nets, render_plane, seeded_records, theta_of, torch_build
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "sc-sfmlearner-release_b200")
-
-
-def bank_build(thetas, rec, idx):
-    """K_b = aug_b(thetas[idx_b]) restated in torch (differentiable; the dtype of thetas)."""
-    rec = rec.to(thetas.device, thetas.dtype)
-    xs, ys, flip, ox, oy, in_w = rec.unbind(1)
-    fx, fy, cx, cy = thetas[idx.long().to(thetas.device)].unbind(1)
-    cxb = torch.where(flip != 0, in_w - cx, cx)
-    zero, one = torch.zeros_like(xs), torch.ones_like(xs)
-    return torch.stack([torch.stack([fx * xs, zero, cxb * xs - ox], 1), torch.stack([zero, fy * ys, cy * ys - oy], 1),
-                        torch.stack([zero, zero, one], 1)], 1)
 
 
 def three_cameras(K):
@@ -142,20 +131,6 @@ def test_bank_argument_errors():
 
 
 # ---- the Trainer with a bank --------------------------------------------------------------------------------------------------
-def _trainer(mode="fp32", theta=None, bank=None, **kw):
-    """theta: one camera [4]; bank: thetas [C,4]."""
-    from scsfm.camera import LearnedCamera
-    from scsfm.trainer import Trainer
-    d, p = _nets()
-    cam = None
-    if theta is not None:
-        cam = LearnedCamera(*[float(v) for v in theta]).to(DEV)
-    elif bank is not None:
-        cam = LearnedCamera.bank(torch.as_tensor(bank, dtype=torch.float32)).to(DEV)
-    kw.setdefault("distributed", False)
-    return Trainer(d, p, lr=1e-4, with_auto_mask=0, conv_mode=mode, camera=cam, **kw)
-
-
 def test_one_camera_bank_trainer_is_todays_trainer():
     """Two eager steps and a capture: the bank of one camera with every index 0 against LearnedCamera(theta).  The launches are
     the same at every step, and the first step, from identical states, gives the same loss bits and theta.  After it the two
@@ -171,7 +146,7 @@ def test_one_camera_bank_trainer_is_todays_trainer():
     zeros = torch.zeros(B, dtype=torch.int32, device=DEV)
     runs = {}
     for name in ("single", "bank"):
-        tr = _trainer("tf32x3", theta=th0) if name == "single" else _trainer("tf32x3", bank=th0[None])
+        tr = make_trainer("tf32x3", theta=th0 if name == "single" else th0[None])
         ix = {} if name == "single" else {"camera_index": zeros}
         out, thetas, launches = [], [], []
         for t, r, rec in batches[:2]:
@@ -199,40 +174,7 @@ def test_one_camera_bank_trainer_is_todays_trainer():
 
 
 def test_eager_bank_step_gives_the_oracle_theta_gradient():
-    """dtheta [2,4] of an eager step against oracle.step.train_step in fp64 with K_b = aug_b(theta[idx_b]); the bound of
-    test_eager_camera_step_gives_the_oracle_theta_gradient (4x the larger fp32 error + 1e-3)."""
-    from golden_util import det_weights
-    from oracle import nets as N
-    from oracle import step as OS
-    from scsfm import synth
-    B, H, W = 2, 96, 160
-    tgt, refs, K = synth.triplet(5, B, H, W)
-    rec = seeded_records(11, B, H, W)
-    idx = torch.tensor([1, 0], dtype=torch.int32)
-    th0 = torch.stack([theta_of(K[0]) * torch.tensor([1.05, 0.97, 1.0, 1.0]) + torch.tensor([0.0, 0.0, 2.0, -1.5]),
-                       theta_of(K[0]) * torch.tensor([0.95, 1.02, 1.0, 1.0]) + torch.tensor([0.0, 0.0, -3.0, 1.0])])
-    tr = _trainer("fp32", bank=th0)
-    tr.step(tgt.to(DEV), [r.to(DEV) for r in refs], aug=rec.to(DEV), camera_index=idx.to(DEV))
-    mine = tr.camera.theta.grad.cpu()
-    want = {}
-    tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        for key, dt, dev in (("64", torch.float64, "cpu"), ("32", torch.float32, "cpu"), ("32gpu", torch.float32, DEV)):
-            d, p = N.DispResNet(18).to(dt).to(dev), N.PoseResNet(18).to(dt).to(dev)
-            for n in (d, p):
-                n.load_state_dict({k: v.to(dt) for k, v in det_weights(n.state_dict()).items()})
-                n.train()
-            th = th0.to(dev, dt, copy=True).requires_grad_(True)
-            OS.train_step(d, p, OS.make_optimizer(d, p, lr=1e-4), tgt.to(dev, dt), [r.to(dev, dt) for r in refs],
-                          bank_build(th, rec, idx), num_scales=1, with_ssim=1, with_mask=1, with_auto_mask=0)
-            want[key] = th.grad.cpu()
-    finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
-    errs = {k: rel_l2(g, want["64"]) for k, g in (("mine", mine), ("32", want["32"]), ("32gpu", want["32gpu"]))}
-    print("bank dtheta rel_l2 vs fp64: mine %.3g | fp32 CPU oracle %.3g | stock PyTorch fp32 on this GPU %.3g" %
-          (errs["mine"], errs["32"], errs["32gpu"]))
-    assert errs["mine"] < 4 * max(errs["32"], errs["32gpu"]) + 1e-3
+    eager_step_vs_oracle(2)
 
 
 def test_bank_adam_is_dense_torch_adam():
@@ -243,7 +185,7 @@ def test_bank_adam_is_dense_torch_adam():
     B, H, W = 2, 96, 160
     tgt, refs, K = synth.triplet(6, B, H, W)
     th0 = torch.stack([theta_of(K[0]) * s for s in (1.05, 0.95, 1.1)])
-    tr = _trainer("fp32", bank=th0)
+    tr = make_trainer("fp32", theta=th0)
     idxs = [[0, 1], [0, 0], [0, 0]]
     grads = []
     for i, ix in enumerate(idxs):
@@ -271,110 +213,20 @@ def test_bank_adam_is_dense_torch_adam():
 
 
 def test_captured_bank_steps_track_eager_steps():
-    """As test_captured_camera_steps_track_eager_steps with a bank of two cameras and mixed indices; capture() leaves theta and its
-    Adam state bitwise unchanged, and a captured bank step has the launches of a captured single-camera step."""
-    from scsfm import synth
-    B, H, W = 2, 96, 160
-    tgt, refs, K = synth.triplet(2, B, H, W)
-    th0 = torch.stack([theta_of(K[0]) * 1.1, theta_of(K[0]) * 0.93])
-    eager, graphed = _trainer("tf32x3", bank=th0), _trainer("tf32x3", bank=th0)
-    ixs = [[0, 1], [1, 1], [1, 0], [0, 0]]
-    batches = [(tgt.to(DEV), [r.to(DEV) for r in refs], seeded_records(20 + i, B, H, W).to(DEV),
-                torch.tensor(ix, dtype=torch.int64, device=DEV)) for i, ix in enumerate(ixs)]
-    before = [t.clone() for t in (graphed.camera.theta.detach(),) + graphed._cam_state]
-    graphed.capture(batches[0][0], batches[0][1], aug=batches[0][2], camera_index=batches[0][3])
-    torch.cuda.synchronize()
-    for a, b in zip(before, (graphed.camera.theta.detach(),) + graphed._cam_state):
-        assert torch.equal(a, b)
-    single = _trainer("tf32x3", theta=th0[0])
-    single.capture(batches[0][0], batches[0][1], aug=batches[0][2])
-    print("captured launches per step: bank %d, one camera %d" % (graphed.launches_per_step, single.launches_per_step))
-    assert graphed.launches_per_step == single.launches_per_step
-    lr = eager.camera_lr
-    grads = {"eager": [], "captured": []}
-    for it, (t, r, rec, ix) in enumerate(batches[1:]):
-        a = [float(v) for v in eager.step(t, r, aug=rec, camera_index=ix)]
-        b = [float(v) for v in graphed.step(t, r, aug=rec, camera_index=ix)]
-        np.testing.assert_allclose(b, a, rtol=2e-4 if it == 0 else 5e-3)
-        g_e, g_g = eager.camera.theta.grad.cpu(), graphed.camera.theta.grad.cpu()
-        print("step %d dtheta: eager %s captured %s rel %.2e" % (it, g_e.tolist(), g_g.tolist(), rel_l2(g_g, g_e)))
-        if it == 0:
-            assert rel_l2(g_g, g_e) < 1e-4
-            assert float((graphed.camera.theta - eager.camera.theta).abs().max()) < 1e-4
-        grads["eager"].append(g_e)
-        grads["captured"].append(g_g)
-    torch.cuda.synchronize()
-    for name, th in (("eager", eager.camera.theta), ("captured", graphed.camera.theta)):
-        ref = th0.double().clone().requires_grad_(True)
-        opt = torch.optim.Adam([ref], lr=lr, betas=(0.9, 0.999), eps=1e-8)
-        for g in grads[name]:
-            ref.grad = g.double()
-            opt.step()
-        assert float((th.detach().cpu().double() - ref.detach()).abs().max()) < 1e-4, (name, th, ref)
-    assert graphed.camera_state_dict()["step"] == 3
-    th_e, th_g = eager.camera.theta.detach().cpu(), graphed.camera.theta.detach().cpu()
-    assert float((th_g - th_e).abs().max()) <= 3 * 2 * lr + 1e-4
-    assert float((graphed.disp_net.flat_params() - eager.disp_net.flat_params()).abs().max()) <= 6.1e-4
+    captured_steps_track_eager(2)
 
 
 def test_trainer_bank_argument_errors():
-    from scsfm import synth
-    tgt, refs, K = synth.triplet(6, 2, 64, 128)
-    c = lambda x: x.to(DEV)  # noqa: E731
-    rec = seeded_records(1, 2, 64, 128).to(DEV)
-    ix = torch.zeros(2, dtype=torch.int32, device=DEV)
-    bank = _trainer("fp32", bank=torch.stack([theta_of(K[0])] * 2))
-    with pytest.raises(TypeError, match="bank of 2 cameras needs"):
-        bank.step(c(tgt), [c(r) for r in refs], aug=rec)
-    with pytest.raises(TypeError, match="int32 or int64 CUDA"):
-        bank.step(c(tgt), [c(r) for r in refs], aug=rec, camera_index=ix.cpu())
-    with pytest.raises(TypeError, match="int32 or int64 CUDA"):
-        bank.step(c(tgt), [c(r) for r in refs], aug=rec, camera_index=ix[:1])
-    with pytest.raises(TypeError, match="bank of 2 cameras needs"):
-        bank.capture(c(tgt), [c(r) for r in refs], aug=rec)
-    one = _trainer("fp32", theta=theta_of(K[0]))
-    with pytest.raises(TypeError, match="one camera"):
-        one.step(c(tgt), [c(r) for r in refs], aug=rec, camera_index=ix)
-    plain = _trainer("fp32")
-    with pytest.raises(TypeError, match="no camera"):
-        plain.step(c(tgt), [c(r) for r in refs], c(K), camera_index=ix)
+    trainer_argument_errors(2)
 
 
 def test_data_parallel_world_of_one_gives_the_single_gpu_bank():
-    import torch.distributed as dist
-    from scsfm import synth
-    B, H, W = 2, 96, 160
-    tgt, refs, K = synth.triplet(8, B, H, W)
-    rec = seeded_records(3, B, H, W).to(DEV)
-    ix = torch.tensor([1, 0], dtype=torch.int32, device=DEV)
-    args = (tgt.to(DEV), [r.to(DEV) for r in refs])
-    th0 = torch.stack([theta_of(K[0]) * 0.9, theta_of(K[0]) * 1.1])
-    single = _trainer("tf32x3", bank=th0)
-    single.step(*args, aug=rec, camera_index=ix)
-    with tempfile.TemporaryDirectory() as tmp:
-        dist.init_process_group("nccl", init_method="file://" + os.path.join(tmp, "rendezvous"), rank=0, world_size=1,
-                                device_id=torch.device(DEV, torch.cuda.current_device()))
-        try:
-            ddp = _trainer("tf32x3", bank=th0, distributed=True)
-            ddp.step(*args, aug=rec, camera_index=ix)
-            torch.cuda.synchronize()
-            assert ddp.exchange.pending() == 0
-            print("world 1 dtheta", ddp.camera.theta.grad.tolist(), "single", single.camera.theta.grad.tolist())
-            assert rel_l2(ddp.camera.theta.grad.cpu(), single.camera.theta.grad.cpu()) < 1e-5
-            assert rel_l2(ddp.camera.theta.detach().cpu(), single.camera.theta.detach().cpu()) < 1e-5
-        finally:
-            dist.destroy_process_group()
+    world_of_one(2)
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_data_parallel_bank_on_two_gpus():
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(_free_port()), os.path.join(ROOT, "tests", "camera_groups_ddp_check.py")]
-    out = subprocess.run(cmd, capture_output=True, text=True, timeout=1500)
-    print(out.stdout[-4000:])
-    assert out.returncode == 0, out.stderr[-4000:]
-    for mode in ("eager", "graph"):
-        assert "CAMERA_GROUPS_DDP_OK %s" % mode in out.stdout
+    two_gpu_check(2)
 
 
 # ---- self-calibration of two cameras ------------------------------------------------------------------------------------------

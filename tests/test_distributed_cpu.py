@@ -1,19 +1,12 @@
 """Host-side logic of the data-parallel path, world_size 2 over gloo on CPU (no GPU, no kernels):
 replica broadcast and the averaged gradient exchange used by scsfm.trainer / bench.py."""
 import os
-import socket
 
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+from helpers import free_port
 
 
 def _worker(rank, world, port, out):
@@ -50,5 +43,5 @@ def test_gradient_exchange_world2_gloo():
     world = 2
     with mp.Manager() as m:
         out = m.dict()
-        mp.spawn(_worker, args=(world, _free_port(), out), nprocs=world, join=True)
+        mp.spawn(_worker, args=(world, free_port(), out), nprocs=world, join=True)
         assert dict(out) == {0: True, 1: True}
