@@ -81,15 +81,6 @@ struct GatherIn {
     }
 };
 
-__device__ __forceinline__ float apply_act(float v, int act) {
-    switch (act & 0xff) {
-        case ACT_RELU: return fmaxf(v, 0.f);
-        case ACT_ELU: return v > 0.f ? v : expm1f(v);
-        case ACT_DISP: return 10.0f * (1.0f / (1.0f + expf(-v))) + 0.01f;   // alpha*sigmoid+beta, DispResNet.py:98
-        default: return v;
-    }
-}
-
 // ----- forward -------------------------------------------------------------------------------
 template <int BM, int BN>
 __global__ void __launch_bounds__(CT)

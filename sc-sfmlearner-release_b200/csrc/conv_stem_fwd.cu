@@ -231,7 +231,7 @@ conv_stem_fwd_kernel(ScsfmConv p, StemGeom g, const __grid_constant__ CUtensorMa
                         const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + off));
                         x.x += a.x; x.y += a.y;
                     }
-                    if (act != ACT_NONE) { x.x = tc_act(x.x, act); x.y = tc_act(x.y, act); }
+                    if (act != ACT_NONE) { x.x = apply_act(x.x, act); x.y = apply_act(x.y, act); }
                     if (round) { x.x = tf32_round(x.x); x.y = tf32_round(x.y); }
                     *reinterpret_cast<float2*>(p.out + off) = x;
                     if (p.out_lo != nullptr) *reinterpret_cast<float2*>(p.out_lo + off) = make_float2(tf32_lo(x.x), tf32_lo(x.y));
@@ -280,29 +280,6 @@ bool conv_stem_eligible(const ScsfmConv& p) {
     return true;
 }
 
-static int sm_count() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    }
-    return n;
-}
-
-static int encode_box(CUtensorMap* m, const float* base, const ScsfmConv& p, int view_cols, int col_step, int box_cols) {
-    const cuuint64_t gdim[4] = {(cuuint64_t)p.Cin, (cuuint64_t)view_cols, (cuuint64_t)p.Hi, (cuuint64_t)p.B};
-    const cuuint64_t gstride[3] = {(cuuint64_t)col_step * p.Cin * 4, (cuuint64_t)p.Wi * p.Cin * 4, (cuuint64_t)p.Hi * p.Wi * p.Cin * 4};
-    const cuuint32_t box[4] = {(cuuint32_t)p.Cin, (cuuint32_t)box_cols, (cuuint32_t)ST_ROWS, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstride, box, estr,
-                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(stem input %d x %d x %d x %d) failed with CUresult %d", p.B, p.Hi, p.Wi, p.Cin, (int)r);
-        return SCSFM_ERR_CUDA;
-    }
-    return SCSFM_OK;
-}
 
 template <int CIN, bool SPLIT>
 static int launch_stem_cfg(const ScsfmConv& p, cudaStream_t st) {
@@ -316,13 +293,20 @@ static int launch_stem_cfg(const ScsfmConv& p, cudaStream_t st) {
     const int fixed = 1024 + 1024 + Cfg::W_BYTES;              // alignment slack + barrier block + resident weights
     g.stages = (ST_SMEM_MAX - fixed) / Cfg::STAGE;
     if (g.stages > ST_MAX_STAGES) g.stages = ST_MAX_STAGES;
+    // box = all Cin channels x ST_UNITS 32-byte units (Cin 4: two columns each) x ST_ROWS rows, unswizzled
     CUtensorMap map0, map1;
+    const long long row = (long long)p.Wi * p.Cin, img = row * p.Hi;
     if (CIN == 8) {
         // odd input columns (view column v = input column 2 v + 1) and even ones (2 v)
-        if (int rc = encode_box(&map0, p.in + CIN, p, p.Wi / 2, 2, ST_UNITS)) return rc;
-        if (int rc = encode_box(&map1, p.in, p, (p.Wi + 1) / 2, 2, ST_UNITS)) return rc;
+        if (int rc = encode_nhwc(&map0, p.in + CIN, p.B, p.Hi, p.Wi / 2, p.Cin, 2 * p.Cin, row, img, p.Cin, ST_UNITS, ST_ROWS,
+                                 CU_TENSOR_MAP_SWIZZLE_NONE))
+            return rc;
+        if (int rc = encode_nhwc(&map1, p.in, p.B, p.Hi, (p.Wi + 1) / 2, p.Cin, 2 * p.Cin, row, img, p.Cin, ST_UNITS, ST_ROWS,
+                                 CU_TENSOR_MAP_SWIZZLE_NONE))
+            return rc;
     } else {
-        if (int rc = encode_box(&map0, p.in, p, p.Wi, 1, 2 * ST_UNITS)) return rc;
+        if (int rc = encode_nhwc(&map0, p.in, p.B, p.Hi, p.Wi, p.Cin, p.Cin, row, img, p.Cin, 2 * ST_UNITS, ST_ROWS, CU_TENSOR_MAP_SWIZZLE_NONE))
+            return rc;
         map1 = map0;
     }
     constexpr int HALVES = SPLIT ? 2 : 1;

@@ -252,7 +252,7 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
                     if (p.bias) x += __ldg(p.bias + n);
                     if (p.bn_scale) x = fmaf(x, __ldg(p.bn_scale + n), __ldg(p.bn_shift + n));    // eval-mode BatchNorm
                     if (p.addend) x += __ldg(p.addend + out_row * N + n);
-                    x = tc_act(x, p.act);
+                    x = apply_act(x, p.act);
                     if (p.act & ROUND_TF32) x = tf32_round(x);
                 } else {
                     x = 0.f;
@@ -520,28 +520,58 @@ CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, cuuint32_t ra
                       CUtensorMapSwizzle sw, CUtensorMapL2promotion l2, CUtensorMapFloatOOBfill oob) {
     using Fn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                             const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static Fn fn = nullptr;
-    if (fn == nullptr) {
+    static const Fn fn = []() -> Fn {                   // C++11 thread-safe one-time initialisation
         void* sym = nullptr;
         cudaDriverEntryPointQueryResult qres;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres) != cudaSuccess || sym == nullptr ||
             qres != cudaDriverEntryPointSuccess)
-            return CUDA_ERROR_NOT_FOUND;
-        fn = reinterpret_cast<Fn>(sym);
-    }
+            return nullptr;
+        return reinterpret_cast<Fn>(sym);
+    }();
+    if (fn == nullptr) return CUDA_ERROR_NOT_FOUND;
     return fn(map, dtype, rank, gaddr, gdim, gstride, box, estr, il, sw, l2, oob);
 }
 
-int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStream_t st);   // conv_simt.cu
-
-static int sm_count() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+int encode_nhwc(CUtensorMap* map, const float* base, int B, int rows, int cols, int C, long long col_step, long long row_step,
+                long long img_step, int box_c, int box_w, int box_h, CUtensorMapSwizzle sw) {
+    const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)B};
+    const cuuint64_t gstride[3] = {(cuuint64_t)col_step * 4, (cuuint64_t)row_step * 4, (cuuint64_t)img_step * 4};
+    const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUresult r = encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstride, box, estr,
+                                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled(activations %d x %d x %d x %d view) failed with CUresult %d", B, rows, cols, C, (int)r);
+        return SCSFM_ERR_CUDA;
     }
+    return SCSFM_OK;
+}
+
+int encode_weights(CUtensorMap* map, const float* w, int Cout, int K, int box_rows) {
+    const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)Cout};
+    const cuuint64_t gstride[1] = {(cuuint64_t)K * sizeof(float)};
+    const cuuint32_t box[2] = {(cuuint32_t)TBK, (cuuint32_t)box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(w), gdim, gstride, box, estr,
+                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled(weights %d x %d) failed with CUresult %d", Cout, K, (int)r);
+        return SCSFM_ERR_CUDA;
+    }
+    return SCSFM_OK;
+}
+
+int sm_count() {
+    static const int n = [] {                           // C++11 thread-safe one-time initialisation
+        int dev = 0, v = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
+        return v;
+    }();
     return n;
 }
+
+int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStream_t st);   // conv_simt.cu
 
 template <int BN, bool STACK = false>
 static int launch_wgrad_tc(const ScsfmConv& p, int border, cudaStream_t st) {
@@ -575,25 +605,11 @@ static int launch_fwd_tc(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
     static const cudaError_t attr_rc = cudaFuncSetAttribute(conv_fwd_tc_kernel<BN, STACK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     SCSFM_CHECK_CUDA(attr_rc);
     const int M = p.B * (v.border ? border_count(p.Ho, p.Wo) : p.Ho * p.Wo);
-    // TMA descriptor of the weight matrix [Cout rows][K columns] (K contiguous), box = 32 columns x BN rows, 128B swizzle
-    const int K = v.kh * v.kw * p.Cin;
-    CUtensorMap wmap, wmap_lo;
-    for (int lo = 0; lo < 2; ++lo) {
-        const float* base = lo ? p.w_lo : p.w;
-        CUtensorMap& wmap_ = lo ? wmap_lo : wmap;
-        if (base == nullptr) { wmap_lo = wmap; continue; }
-        const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)p.Cout};
-        const cuuint64_t gstride[1] = {(cuuint64_t)K * sizeof(float)};
-        const cuuint32_t box[2] = {(cuuint32_t)TBK, (cuuint32_t)(STACK ? BN / 2 : BN)};
-        const cuuint32_t estr[2] = {1, 1};
-        const CUresult r = encode_tiled(&wmap_, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-                                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            set_error("cuTensorMapEncodeTiled(weights %d x %d) failed with CUresult %d", p.Cout, K, (int)r);
-            return SCSFM_ERR_CUDA;
-        }
-    }
+    // the kernel reads wmap_lo only when p.w_lo is set (STACK is chosen for split mode only)
+    const int K = v.kh * v.kw * p.Cin, rows = STACK ? BN / 2 : BN;
+    CUtensorMap wmap, wmap_lo = {};
+    if (int rc = encode_weights(&wmap, p.w, p.Cout, K, rows)) return rc;
+    if (int rc = p.w_lo != nullptr ? encode_weights(&wmap_lo, p.w_lo, p.Cout, K, rows) : SCSFM_OK) return rc;
     dim3 grid((M + GBM - 1) / GBM, STACK ? 1 : (p.Cout + BN - 1) / BN);
     conv_fwd_tc_kernel<BN, STACK><<<grid, FW_THREADS, Cfg::SMEM, st>>>(p, v, wmap, wmap_lo);
     SCSFM_CHECK_LAUNCH();
@@ -777,6 +793,20 @@ extern "C" int scsfm_weight_flip_batched(const long long* table, int n_rows, int
     return SCSFM_OK;
 }
 
+// Output-parity class (py, px) of a stride-2 data gradient: the kernel rows dy_max, dy_max - 2, ... (jh of them) and
+// columns dx_max, dx_max - 2, ... (jw) reach it; jh or jw = 0: no tap does.
+struct S2Class {
+    int jh, jw, dy_max, dx_max;
+};
+static S2Class s2_class(int kh, int kw, int pad, int py, int px) {
+    S2Class k{0, 0, kh - 1, kw - 1};
+    while (k.dy_max >= 0 && ((py + pad - k.dy_max) & 1)) --k.dy_max;
+    while (k.dx_max >= 0 && ((px + pad - k.dx_max) & 1)) --k.dx_max;
+    k.jh = k.dy_max < 0 ? 0 : k.dy_max / 2 + 1;
+    k.jw = k.dx_max < 0 ? 0 : k.dx_max / 2 + 1;
+    return k;
+}
+
 // Stride-2 data gradient: wt4 receives the four parity-class weight sets back to back (class order (py,px) =
 // (0,0),(0,1),(1,0),(1,1)); total size = Cin*kh*kw*Cout floats, the same as the full flipped kernel.
 extern "C" int scsfm_weight_flip_s2(const float* w, int Cout, int kh, int kw, int Cin, int pad, float* wt4, int operand, void* stream) {
@@ -784,15 +814,13 @@ extern "C" int scsfm_weight_flip_s2(const float* w, int Cout, int kh, int kw, in
     size_t off = 0;
     for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px) {
-            int dy_max = kh - 1, dx_max = kw - 1;
-            while (dy_max >= 0 && ((py + pad - dy_max) & 1)) --dy_max;
-            while (dx_max >= 0 && ((px + pad - dx_max) & 1)) --dx_max;
-            const int jh = dy_max < 0 ? 0 : dy_max / 2 + 1, jw = dx_max < 0 ? 0 : dx_max / 2 + 1;
-            const long long total = (long long)Cout * jh * jw * Cin;
+            const S2Class k = s2_class(kh, kw, pad, py, px);
+            const long long total = (long long)Cout * k.jh * k.jw * Cin;
             if (total > 0) {
                 int grid = (int)((total + 255) / 256);
                 if (grid > sm_count() * 16) grid = sm_count() * 16;
-                weight_flip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, Cout, kh, kw, Cin, jh, jw, dy_max, dx_max, 2, wt4 + off, operand);
+                weight_flip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, Cout, kh, kw, Cin, k.jh, k.jw, k.dy_max, k.dx_max, 2, wt4 + off,
+                                                                           operand);
                 SCSFM_CHECK_LAUNCH();
             }
             off += (size_t)total;
@@ -823,43 +851,35 @@ extern "C" int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream) {
     // stride 2: p->w holds the four parity-class weight sets of scsfm_weight_flip_s2
     SCSFM_CHECK_ARG((q.Cin & 3) == 0, "conv2d_dgrad_tc: needs Cout %% 4 == 0");
     q.stride = 1;
-    size_t woff = 0;
     bool covered_all = true;
     for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px) {
-            int dy_max = p->kh - 1, dx_max = p->kw - 1;
-            while (dy_max >= 0 && ((py + p->pad - dy_max) & 1)) --dy_max;
-            while (dx_max >= 0 && ((px + p->pad - dx_max) & 1)) --dx_max;
-            const int jh = dy_max < 0 ? 0 : dy_max / 2 + 1, jw = dx_max < 0 ? 0 : dx_max / 2 + 1;
+            const S2Class k = s2_class(p->kh, p->kw, p->pad, py, px);
             const int Hs = (p->Hi - py + 1) / 2, Ws = (p->Wi - px + 1) / 2;
-            if (jh == 0 || jw == 0) { if (Hs > 0 && Ws > 0) covered_all = false; }
-            woff += (size_t)p->Cout * jh * jw * p->Cin;
+            if ((k.jh == 0 || k.jw == 0) && Hs > 0 && Ws > 0) covered_all = false;
         }
     if (!covered_all) {
-        // parity classes without taps (1x1 stride 2): their gradient is the addend alone (or zero)
+        // parity classes without taps (1x1 stride 2): their gradient is the addend alone (or zero).  Enqueued before the
+        // sub-convolutions, which write the other classes' pixels of din.
         const size_t bytes = (size_t)p->B * p->Hi * p->Wi * p->Cin * sizeof(float);
         if (p->addend) SCSFM_CHECK_CUDA(cudaMemcpyAsync(p->din, p->addend, bytes, cudaMemcpyDeviceToDevice, st));
         else SCSFM_CHECK_CUDA(cudaMemsetAsync(p->din, 0, bytes, st));
     }
-    woff = 0;
+    size_t woff = 0;
     for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px) {
-            int dy_max = p->kh - 1, dx_max = p->kw - 1;
-            while (dy_max >= 0 && ((py + p->pad - dy_max) & 1)) --dy_max;
-            while (dx_max >= 0 && ((px + p->pad - dx_max) & 1)) --dx_max;
-            const int jh = dy_max < 0 ? 0 : dy_max / 2 + 1, jw = dx_max < 0 ? 0 : dx_max / 2 + 1;
+            const S2Class k = s2_class(p->kh, p->kw, p->pad, py, px);
             const int Hs = (p->Hi - py + 1) / 2, Ws = (p->Wi - px + 1) / 2;
-            const size_t wcount = (size_t)p->Cout * jh * jw * p->Cin;
-            if (jh > 0 && jw > 0 && Hs > 0 && Ws > 0) {
+            if (k.jh > 0 && k.jw > 0 && Hs > 0 && Ws > 0) {
                 ScsfmConv r = q;
                 r.w = p->w + woff;
                 r.w_lo = p->w_lo ? p->w_lo + woff : nullptr;
-                r.Ho = Hs; r.Wo = Ws; r.kh = jh; r.kw = jw;
+                r.Ho = Hs; r.Wo = Ws; r.kh = k.jh; r.kw = k.jw;
                 // input (dout) row of output hy and tap jy: hy + (py + pad - dy_max)/2 + jy
-                TcView v{jh, jw, (py + p->pad - dy_max) / 2, (px + p->pad - dx_max) / 2, 1, 2, py, 2, px, p->Hi, p->Wi};
+                TcView v{k.jh, k.jw, (py + p->pad - k.dy_max) / 2, (px + p->pad - k.dx_max) / 2, 1, 2, py, 2, px, p->Hi, p->Wi};
                 if (int rc = tc_dispatch(r, v, st)) return rc;
             }
-            woff += wcount;
+            woff += (size_t)p->Cout * k.jh * k.jw * p->Cin;
         }
     return SCSFM_OK;
 }

@@ -37,15 +37,6 @@ struct TcCfg {
 // kernel that writes a tensor later consumed by a convolution takes the SCSFM_ROUND_TF32 flag, and the weights are
 // rounded per optimizer step (scsfm_round_tf32).  The loaders below therefore copy bits unchanged.
 
-__device__ __forceinline__ float tc_act(float v, int act) {
-    switch (act & 0xff) {
-        case ACT_RELU: return fmaxf(v, 0.f);
-        case ACT_ELU: return v > 0.f ? v : expm1f(v);
-        case ACT_DISP: return 10.0f * (1.0f / (1.0f + expf(-v))) + 0.01f;
-        default: return v;
-    }
-}
-
 // Geometry of one (sub-)convolution as the kernel sees it.  A plain convolution uses the identity output map; a
 // stride-2 data gradient is run as four parity-class stride-1 sub-convolutions (output pixels 2h+py, 2w+px) whose
 // taps are the kernel rows/columns of matching parity -- no multiplications by inserted zeros.
@@ -71,6 +62,15 @@ __host__ __device__ __forceinline__ int border_count(int Ho, int Wo) { return 2 
 CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, cuuint32_t rank, void* gaddr, const cuuint64_t* gdim,
                       const cuuint64_t* gstride, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapInterleave il,
                       CUtensorMapSwizzle sw, CUtensorMapL2promotion l2, CUtensorMapFloatOOBfill oob);
+// fp32 NHWC activations seen as [B][rows][cols][C]: element (c, x, y, b) at base + c + x col_step + y row_step + b img_step
+// (in elements: a parity view doubles a step), box = box_c x box_w x box_h x 1, zero fill out of bounds
+int encode_nhwc(CUtensorMap* map, const float* base, int B, int rows, int cols, int C, long long col_step, long long row_step,
+                long long img_step, int box_c, int box_w, int box_h, CUtensorMapSwizzle sw);
+// weights [Cout][K] (K contiguous): box = 32 columns x box_rows rows, 128B swizzle (rows past Cout are zero-filled)
+int encode_weights(CUtensorMap* map, const float* w, int Cout, int K, int box_rows);
+
+// multiprocessors of the current device (132 if the query fails), looked up once
+int sm_count();
 
 // conv_tma.cu: zero-padded stride-1 (sub-)convolutions and stride-2 convolutions with kh, kw <= 3 through the TMA
 // halo-patch kernel (stride 2: parity views of the input)

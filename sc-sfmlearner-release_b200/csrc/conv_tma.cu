@@ -285,7 +285,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMap
                             const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + off + c));
                             x.x += a.x; x.y += a.y;
                         }
-                        if (act != ACT_NONE) { x.x = tc_act(x.x, act); x.y = tc_act(x.y, act); }
+                        if (act != ACT_NONE) { x.x = apply_act(x.x, act); x.y = apply_act(x.y, act); }
                         if (round) { x.x = tf32_round(x.x); x.y = tf32_round(x.y); }
                         *reinterpret_cast<float2*>(p.out + off + c) = x;
                         if (p.out_lo != nullptr) *reinterpret_cast<float2*>(p.out_lo + off + c) = make_float2(tf32_lo(x.x), tf32_lo(x.y));
@@ -348,15 +348,6 @@ bool conv_tma_eligible(const ScsfmConv& p, const TcView& v) {
 }
 
 bool conv_tma_forced(const ScsfmConv& p) { return tune_mt(p) != 0 || tune_bn(p) != 0 || tune_tw(p) != 0; }
-
-static int sm_count() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    }
-    return n;
-}
 
 template <int BNW, int MT>
 static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cudaStream_t st) {
@@ -431,43 +422,19 @@ static int launch_tma_cfg(const ScsfmConv& p, const TcView& v, int tw_log2, cuda
         if (base == nullptr) continue;
         for (int i = 0; i < g.nbox; ++i)
             for (int dx = 0; dx < v.kw; ++dx) {
-                // activations [B][Hi][Wi][Cin] (Cin contiguous), seen through the (py, px) parity view at stride 2: every
-                // S-th row and column from row py, column px; box = 32 channels x TW x box_rows x 1, 128B swizzle
+                // the (py, px) parity view at stride 2: every S-th row and column from row py, column px; box = 32
+                // channels x TW x box_rows, 128B swizzle
                 const int py = g.box_py[i], px = g.col_px[dx];
-                CUtensorMap& m = (lo ? maps.a_lo : maps.a)[py * 2 + px];
-                const cuuint64_t gdim[4] = {(cuuint64_t)p.Cin, (cuuint64_t)((p.Wi - px + S - 1) / S), (cuuint64_t)((p.Hi - py + S - 1) / S),
-                                            (cuuint64_t)p.B};
-                const cuuint64_t gstride[3] = {(cuuint64_t)S * p.Cin * 4, (cuuint64_t)S * p.Wi * p.Cin * 4, (cuuint64_t)p.Hi * p.Wi * p.Cin * 4};
-                const cuuint32_t box[4] = {(cuuint32_t)TBK, (cuuint32_t)TW, (cuuint32_t)g.box_rows[i], 1};
-                const cuuint32_t estr[4] = {1, 1, 1, 1};
-                const CUresult r = encode_tiled(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base + ((size_t)py * p.Wi + px) * p.Cin),
-                                                gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-                if (r != CUDA_SUCCESS) {
-                    set_error("cuTensorMapEncodeTiled(activations %d x %d x %d x %d, view %d/%d) failed with CUresult %d", p.B, p.Hi, p.Wi,
-                              p.Cin, py, px, (int)r);
-                    return SCSFM_ERR_CUDA;
-                }
+                if (int rc = encode_nhwc(&(lo ? maps.a_lo : maps.a)[py * 2 + px], base + ((size_t)py * p.Wi + px) * p.Cin, p.B,
+                                         (p.Hi - py + S - 1) / S, (p.Wi - px + S - 1) / S, p.Cin, (long long)S * p.Cin,
+                                         (long long)S * p.Wi * p.Cin, (long long)p.Hi * p.Wi * p.Cin, TBK, TW, g.box_rows[i],
+                                         CU_TENSOR_MAP_SWIZZLE_128B))
+                    return rc;
             }
     }
-    for (int lo = 0; lo < 2; ++lo) {
-        const float* base = lo ? p.w_lo : p.w;
-        CUtensorMap& wmap_ = lo ? maps.w_lo : maps.w;
-        if (base == nullptr) continue;
-        // weights [Cout][K] (K contiguous); box = 32 columns x BNW rows (rows past Cout are zero-filled)
-        const int K = v.kh * v.kw * p.Cin;
-        const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)p.Cout};
-        const cuuint64_t gstride[1] = {(cuuint64_t)K * sizeof(float)};
-        const cuuint32_t box[2] = {(cuuint32_t)TBK, (cuuint32_t)BNW};
-        const cuuint32_t estr[2] = {1, 1};
-        const CUresult r = encode_tiled(&wmap_, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-                                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            set_error("cuTensorMapEncodeTiled(weights %d x %d) failed with CUresult %d", p.Cout, K, (int)r);
-            return SCSFM_ERR_CUDA;
-        }
-    }
+    const int K = v.kh * v.kw * p.Cin;
+    if (int rc = encode_weights(&maps.w, p.w, p.Cout, K, BNW)) return rc;
+    if (int rc = p.w_lo != nullptr ? encode_weights(&maps.w_lo, p.w_lo, p.Cout, K, BNW) : SCSFM_OK) return rc;
     int ctas = sm_count();
     if (ctas > g.num_work) ctas = g.num_work;
     conv_tma_kernel<BNW, MT><<<ctas, TMA_THREADS, smem, st>>>(p, v, g, maps);

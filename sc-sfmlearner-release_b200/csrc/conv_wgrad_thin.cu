@@ -198,12 +198,7 @@ static int launch_thin(const ScsfmConv& p, cudaStream_t st) {
     const int tiles_x = (p.Wo + TW - 1) / TW, tiles_y = (p.Ho + Cfg::TH - 1) / Cfg::TH;
     const long long total = (long long)p.B * tiles_y * tiles_x;
     SCSFM_CHECK_ARG(total < (1LL << 31), "conv_wgrad_thin: too many tiles");
-    int nsm = 132;
-    {
-        int dev = 0, v = 0;
-        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) nsm = v;
-    }
-    int ctas = nsm * MINB;
+    int ctas = sm_count() * MINB;
     if (ctas > total) ctas = (int)total;
     const int per = (int)((total + ctas - 1) / ctas);
     ctas = (int)((total + per - 1) / per);

@@ -307,32 +307,6 @@ bool conv_wgrad_tma_eligible(const ScsfmConv& p) {
     return true;
 }
 
-static int sm_count() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    }
-    return n;
-}
-
-// rows: rows of the view; row_step: image rows per view row (2: a parity-row view based on base's row), H: image rows
-static int encode_nhwc(CUtensorMap* map, const float* base, int B, int H, int W, int C, int box_w, int box_h, int rows, int row_step,
-                       int box_c = TBK, CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B) {
-    const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)rows, (cuuint64_t)B};
-    const cuuint64_t gstride[3] = {(cuuint64_t)C * 4, (cuuint64_t)row_step * W * C * 4, (cuuint64_t)H * W * C * 4};
-    const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstride, box, estr,
-                                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(%d x %d x %d x %d) failed with CUresult %d", B, H, W, C, (int)r);
-        return SCSFM_ERR_CUDA;
-    }
-    return SCSFM_OK;
-}
-
 template <int BN, bool SPLIT, int KW, int S>
 static int launch_wgrad_tma_cfg(const ScsfmConv& p, cudaStream_t st) {
     using Cfg = WtCfg<BN, SPLIT, KW, S>;
@@ -340,18 +314,21 @@ static int launch_wgrad_tma_cfg(const ScsfmConv& p, cudaStream_t st) {
         cudaFuncSetAttribute(conv_wgrad_tma_kernel<BN, SPLIT, KW, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     SCSFM_CHECK_CUDA(attr_rc);
     CUtensorMap amap, amap_odd, dmap;
+    const long long row = (long long)p.Wi * p.Cin, img = row * p.Hi;
     if (S == 1) {
-        if (int rc = encode_nhwc(&amap, p.in, p.B, p.Hi, p.Wi, p.Cin, Cfg::PW, WT_TH, p.Hi, 1)) return rc;
+        if (int rc = encode_nhwc(&amap, p.in, p.B, p.Hi, p.Wi, p.Cin, p.Cin, row, img, TBK, Cfg::PW, WT_TH, CU_TENSOR_MAP_SWIZZLE_128B))
+            return rc;
         amap_odd = amap;
     } else {
-        // the stem's box is all Cin (<= 8) channels, unswizzled
+        // the even and the odd input rows; the stem's box is all Cin (<= 8) channels, unswizzled
         const int box_c = Cfg::STEM ? p.Cin : TBK;
         const CUtensorMapSwizzle sw = Cfg::STEM ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
-        if (int rc = encode_nhwc(&amap, p.in, p.B, p.Hi, p.Wi, p.Cin, Cfg::PW, WT_TH, (p.Hi + 1) / 2, 2, box_c, sw)) return rc;
-        if (int rc = encode_nhwc(&amap_odd, p.in + (size_t)p.Wi * p.Cin, p.B, p.Hi, p.Wi, p.Cin, Cfg::PW, WT_TH, p.Hi / 2, 2, box_c, sw))
-            return rc;
+        if (int rc = encode_nhwc(&amap, p.in, p.B, (p.Hi + 1) / 2, p.Wi, p.Cin, p.Cin, 2 * row, img, box_c, Cfg::PW, WT_TH, sw)) return rc;
+        if (int rc = encode_nhwc(&amap_odd, p.in + row, p.B, p.Hi / 2, p.Wi, p.Cin, p.Cin, 2 * row, img, box_c, Cfg::PW, WT_TH, sw)) return rc;
     }
-    if (int rc = encode_nhwc(&dmap, p.dout, p.B, p.Ho, p.Wo, p.Cout, WT_TW, WT_TH, p.Ho, 1)) return rc;
+    if (int rc = encode_nhwc(&dmap, p.dout, p.B, p.Ho, p.Wo, p.Cout, p.Cout, (long long)p.Wo * p.Cout, (long long)p.Ho * p.Wo * p.Cout, TBK,
+                             WT_TW, WT_TH, CU_TENSOR_MAP_SWIZZLE_128B))
+        return rc;
     WtGeom g;
     g.tiles_x = (p.Wo + WT_TW - 1) / WT_TW;
     g.tiles_y = (p.Ho + WT_TH - 1) / WT_TH;

@@ -47,7 +47,7 @@ head_fwd_kernel(const float* __restrict__ in, const float* __restrict__ w, const
         for (int o = TPP / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
         if (c4 == 0 && ok) {
             acc += b0;
-            if ((act & 0xff) == ACT_DISP) acc = 10.0f * (1.0f / (1.0f + expf(-acc))) + 0.01f;
+            if ((act & 0xff) == ACT_DISP) acc = apply_act(acc, ACT_DISP);
             out[p] = acc;
         }
     }

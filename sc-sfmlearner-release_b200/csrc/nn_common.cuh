@@ -24,4 +24,14 @@ __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__
 __device__ __forceinline__ float tf32_lo(float x) { return tf32_round(x - tf32_trunc(x)); }
 // SCSFM_OPERAND_*: 0 = rounded TF32, 1 = raw bits, 2 = low part
 __device__ __forceinline__ float tc_operand(float x, int kind) { return kind == 0 ? tf32_round(x) : (kind == 1 ? x : tf32_lo(x)); }
+
+// SCSFM_ACT_* in the low byte of act
+__device__ __forceinline__ float apply_act(float v, int act) {
+    switch (act & 0xff) {
+        case ACT_RELU: return fmaxf(v, 0.f);
+        case ACT_ELU: return v > 0.f ? v : expm1f(v);
+        case ACT_DISP: return 10.0f * (1.0f / (1.0f + expf(-v))) + 0.01f;   // alpha*sigmoid+beta, DispResNet.py:98
+        default: return v;
+    }
+}
 }  // namespace scsfm
