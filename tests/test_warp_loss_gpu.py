@@ -122,7 +122,7 @@ def test_tiny_image_hits_the_10000_threshold(golden_warp):
     np.testing.assert_allclose(float(s), golden_warp["tiny_smooth"][0], rtol=1e-4)
 
 
-@pytest.mark.parametrize("shape", [(1, 50, 70), (3, 33, 97)])
+@pytest.mark.parametrize("shape", [(1, 50, 70), (3, 33, 97), (2, 52, 76)])
 @pytest.mark.parametrize("pm", ["zeros", "border"])
 def test_ragged_sizes_maps_and_grads_vs_oracle(shape, pm):
     """Sizes that are not multiples of the 32x16 tile; per-pixel maps + inverse_warp2 autograd."""
