@@ -58,7 +58,9 @@ def _conv(O, mode, knobs, x, w, act=0, sums=None, groups=1, **kw):
 @pytest.mark.parametrize("case", CASES)
 def test_stem_fwd_vs_fp64(case, cin, mode):
     O = _O()
-    tol = 1e-5 if mode == "tf32x3" else 1e-3
+    # fp64 reference from the operands the kernel reads (tf32: products of TF32 operands are exact in fp32); worst tf32
+    # relative L2 of these shapes on an H100: 9.5e-7
+    tol = 1e-5
     x, w = _inputs(*case, cin, mode, 3 + sum(case) + cin)
     want = _ref(x, w)
     got = {}
@@ -85,7 +87,7 @@ def test_stem_fwd_bn_sums(groups, cin, mode):
     for name, knobs in WAYS:
         sums = torch.zeros(O.BN_SLOTS, groups, C, 2, dtype=torch.float64, device=DEV)
         y = _conv(O, mode, knobs, x, w, sums=sums, groups=groups)
-        assert rel_l2(y.cpu(), want) < (1e-5 if mode == "tf32x3" else 1e-3), name
+        assert rel_l2(y.cpu(), want) < 1e-5, name
         s = sums.sum(0).cpu()
         yd = y.double().cpu().reshape(groups, B // groups, -1, C)
         s1, s2 = yd.sum((1, 2)), (yd * yd).sum((1, 2))

@@ -61,7 +61,9 @@ def _ref(x, w, bias, k):
 def test_conv_fwd_stride2_vs_fp64(case, mode):
     O = _O()
     k = case[5]
-    tol = 1e-5 if mode == "tf32x3" else 1e-3
+    # fp64 reference from the operands the kernel reads.  tf32: products of TF32 operands are exact in fp32, but the wgmma
+    # accumulator adds with truncation over a whole K loop (worst on an H100: 1.04e-5, the 512 -> 512 3x3 layer, K = 4608)
+    tol = 1e-5 if mode == "tf32x3" else 5e-5
     x, w, bias = _inputs(case, mode, 11 + sum(case))
     want = _ref(x, w, bias, k)
     got = {}
@@ -93,7 +95,9 @@ def test_conv_fwd_stride2_epilogues(case, mode):
     gather kernel."""
     O = _O()
     B, k = case[0], case[5]
-    tol = 1e-5 if mode == "tf32x3" else 1e-3
+    # fp64 reference from the operands the kernel reads.  tf32: products of TF32 operands are exact in fp32, but the wgmma
+    # accumulator adds with truncation over a whole K loop (worst on an H100: 1.04e-5, the 512 -> 512 3x3 layer, K = 4608)
+    tol = 1e-5 if mode == "tf32x3" else 5e-5
     x, w, bias = _inputs(case, mode, 7 + sum(case))
     lin = _ref(x, w, bias, k)
     g = torch.Generator().manual_seed(3)
@@ -107,7 +111,8 @@ def test_conv_fwd_stride2_epilogues(case, mode):
             assert rel_l2(y.cpu(), fn(lin)) < tol, (name, act)
         y = cx.conv_fwd(x, w, bias, 2, k // 2, O.PAD_ZERO, O.ACT_RELU | O.ROUND_TF32, None, 1, w_lo, addend=addend.to(DEV))
         want = torch.relu(lin + addend.double())
-        assert rel_l2(y.cpu(), want) < 1e-3, name                 # the stored result is rounded to TF32
+        # the stored result is rounded to TF32 (relative error up to 2^-11): compared with unrounded values, 1e-3 is the bound
+        assert rel_l2(y.cpu(), want) < 1e-3, name
         assert rel_l2(y, cx.conv_fwd(x, w, bias, 2, k // 2, O.PAD_ZERO, O.ACT_RELU, None, 1, w_lo, addend=addend.to(DEV))) < 1e-3, name
         assert torch.equal(y.view(torch.int32) & 0x1FFF, torch.zeros_like(y.view(torch.int32))), name   # TF32 mantissa
         sums = torch.zeros(O.BN_SLOTS, 3, case[4], 2, dtype=torch.float64, device=DEV)

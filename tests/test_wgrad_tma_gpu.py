@@ -38,7 +38,9 @@ def test_wgrad_tma_vs_fp64(case, mode):
     from scsfm import nnops as O
     B, H, W, Cin, Cout, k, pad_mode = case
     pad = k // 2
-    tol = 1e-5 if mode == "tf32x3" else 1e-3
+    # fp64 reference from the operands the kernel reads (tf32: products of TF32 operands are exact in fp32); worst tf32
+    # relative L2 of these shapes on an H100: 2.4e-6
+    tol = 1e-5
     g = torch.Generator().manual_seed(3)
     x = torch.randn(B, Cin, H, W, generator=g, dtype=torch.float64)
     dpre = torch.randn(B, Cout, H, W, generator=g, dtype=torch.float64)

@@ -34,7 +34,9 @@ def test_wgrad_tma_stride2_vs_fp64(case, mode):
     B, H, W, Cin, Cout, k = case
     pad = k // 2
     Ho, Wo = (H + 2 * pad - k) // 2 + 1, (W + 2 * pad - k) // 2 + 1
-    tol = 1e-5 if mode == "tf32x3" else 1e-3
+    # fp64 reference from the operands the kernel reads (tf32: products of TF32 operands are exact in fp32); worst tf32
+    # relative L2 of these shapes on an H100: 2.4e-6
+    tol = 1e-5
     g = torch.Generator().manual_seed(5)
     xc = torch.randn(B, H, W, Cin, generator=g).to(DEV)
     dc = torch.randn(B, Ho, Wo, Cout, generator=g).to(DEV)
@@ -80,7 +82,9 @@ def test_wgrad_tma_stem_vs_fp64(case, mode):
     from scsfm import nnops as O
     B, H, W, Cin, Cout = case
     Ho, Wo = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
-    tol = 1e-5 if mode == "tf32x3" else 1e-3
+    # fp64 reference from the operands the kernel reads (tf32: products of TF32 operands are exact in fp32); worst tf32
+    # relative L2 of these shapes on an H100: 2.4e-6
+    tol = 1e-5
     g = torch.Generator().manual_seed(9)
     xc = torch.randn(B, H, W, Cin, generator=g)
     xc[..., -1] = 0
