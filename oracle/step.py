@@ -14,9 +14,13 @@ def compute_depth(disp_net, tgt_img, ref_imgs):
 
 
 def compute_pose_with_inv(pose_net, tgt_img, ref_imgs):
-    """Forward and backward relative poses, two separate network calls per reference (train.py:437-444)."""
-    poses = [pose_net(tgt_img, r) for r in ref_imgs]
-    poses_inv = [pose_net(r, tgt_img) for r in ref_imgs]
+    """Forward and backward relative poses, two separate network calls per reference (train.py:437-444), in the reference's
+    order (tgt,ref0), (ref0,tgt), (tgt,ref1), ...: each call moves the BatchNorm running statistics, so with two or more
+    references the order shows in them."""
+    poses, poses_inv = [], []
+    for r in ref_imgs:
+        poses.append(pose_net(tgt_img, r))
+        poses_inv.append(pose_net(r, tgt_img))
     return poses, poses_inv
 
 

@@ -49,6 +49,76 @@ def rel_l2(a, b):
     return float((a - b).norm() / (b.norm() + 1e-30))
 
 
+def oracle_train_step(tgt, refs, K, *, disp_layers=18, pose_layers=18, lr=1e-4, betas=(0.9, 0.999), weight_decay=0.0,
+                      gpu="cuda", **step_cfg):
+    """One step of the oracle's training loop (oracle/step.py:train_step; step_cfg = its loss switches, padding and w1..w3)
+    from det_weights on the given inputs, evaluated three ways: "f32" and "f64" on the CPU, "f32gpu" through stock PyTorch /
+    cuDNN on `gpu` (the caller turns cuDNN / matmul TF32 off).  Each gives (the four losses, every gradient autograd produced
+    keyed "disp.*" / "pose.*" -- parameters left with grad None are absent --, the BatchNorm buffers after the step)."""
+    from golden_util import det_weights
+    from oracle import nets as N
+    from oracle import step as OS
+    assert not (torch.backends.cudnn.allow_tf32 or torch.backends.cuda.matmul.allow_tf32), "the fp32 GPU oracle needs TF32 off"
+    out = {}
+    for name, dt, dev in (("f32", torch.float32, "cpu"), ("f64", torch.float64, "cpu"), ("f32gpu", torch.float32, gpu)):
+        d, p = N.DispResNet(disp_layers).to(dt).to(dev), N.PoseResNet(pose_layers).to(dt).to(dev)
+        for net in (d, p):
+            net.load_state_dict({k: v.to(dt).to(dev) for k, v in det_weights(net.state_dict()).items()})
+            net.train()
+        losses = OS.train_step(d, p, OS.make_optimizer(d, p, lr=lr, betas=betas, weight_decay=weight_decay), tgt.to(dt).to(dev),
+                               [r.to(dt).to(dev) for r in refs], K.to(dt).to(dev), **step_cfg)
+        out[name] = ([float(v) for v in losses],
+                     {"disp." + k: q.grad.clone().cpu() for k, q in d.named_parameters() if q.grad is not None} |
+                     {"pose." + k: q.grad.clone().cpu() for k, q in p.named_parameters() if q.grad is not None},
+                     {"disp." + k: b.clone().cpu() for k, b in d.named_buffers()} |
+                     {"pose." + k: b.clone().cpu() for k, b in p.named_buffers()})
+    return out
+
+
+class Adam64:
+    """torch.optim.Adam in fp64 on one flat vector, as the reference of an fp32 Adam kernel compared per step on the parameter
+    CHANGE.  The hyper-parameters are the fp32 values the kernel receives.  step(g) continues the fp64 trajectory from p0;
+    step(g, before) starts the step from the parameters the kernel under test started from instead.  m and v carry over from
+    step to step in fp64 either way."""
+
+    def __init__(self, p0, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+        f = lambda v: float(np.float32(v))  # noqa: E731
+        self.lr, self.b1, self.b2, self.eps, self.wd = f(lr), f(betas[0]), f(betas[1]), f(eps), f(weight_decay)
+        self.p = p0.detach().double().clone().requires_grad_(True)
+        self.opt = torch.optim.Adam([self.p], lr=self.lr, betas=(self.b1, self.b2), eps=self.eps, weight_decay=self.wd,
+                                    foreach=False)
+        self.t = 0
+
+    def step(self, grad, before=None):
+        """Returns (change, size): the fp64 change of this step and the update's size, taken before m = b1 m + (1-b1) g
+        cancels (where g undoes the previous steps the change itself is tiny, but the fp32 rounding of the two terms is not)."""
+        self.t += 1
+        with torch.no_grad():
+            if before is not None:
+                self.p.copy_(before.double())
+            before = self.p.detach().clone()
+        state = self.opt.state[self.p]
+        m_prev = state["exp_avg"].clone() if state else torch.zeros_like(before)
+        grad = grad.double().to(before.device)
+        g_eff = grad + self.wd * before
+        self.p.grad = grad
+        self.opt.step()
+        den = state["exp_avg_sq"].sqrt() / (1 - self.b2 ** self.t) ** 0.5 + self.eps
+        size = self.lr / (1 - self.b1 ** self.t) * (self.b1 * m_prev.abs() + (1 - self.b1) * g_eff.abs()) / den
+        return self.p.detach() - before, size
+
+
+def assert_adam_change(got, want, size, after, grad, what=""):
+    """An fp32 Adam step's parameter change `got` against the fp64 change `want`: within 1e-5 of the update's size, plus the
+    rounding of the new fp32 parameter `after` (at most 2^-24 of its magnitude)."""
+    got, want, size, after, grad = (torch.as_tensor(x).double() for x in (got, want, size, after, grad))
+    err = (got - want).abs()
+    bound = 1e-5 * size + 2.0 ** -24 * after.abs()
+    worst = int(torch.argmax(err / bound.clamp_min(1e-300)))
+    assert bool((err <= bound).all()), "%s: change %.9g vs fp64 %.9g at %d (g = %.3g, error %.3g of the update size)" % (
+        what, float(got[worst]), float(want[worst]), worst, float(grad[worst]), float(err[worst] / size[worst]))
+
+
 def frac_within(a, b, tol):
     """Fraction of elements with |a-b| <= tol * max|b|."""
     a = torch.as_tensor(a, dtype=torch.float64).cpu()

@@ -507,10 +507,12 @@ def test_forward_multi_equals_separate_calls(mode):
 
 
 @pytest.mark.parametrize("mode", ["fp32", "tf32", "tf32x3"])
-@pytest.mark.parametrize("shape", [(6, 4, 6, 64, 3), (6, 8, 12, 64, 3), (8, 16, 24, 128, 4), (3, 5, 7, 32, 3)])
+@pytest.mark.parametrize("shape", [(6, 4, 6, 64, 3), (6, 8, 12, 64, 3), (8, 16, 24, 128, 4), (3, 5, 7, 32, 3),
+                                   (10, 8, 26, 64, 5), (16, 4, 13, 512, 8)])
 def test_fused_batchnorm_sums_per_group(mode, shape):
     """Per-group BatchNorm partial sums out of the conv epilogue when several calls are stacked: groups whose
-    row ranges straddle the 128-row (tensor-core) / 64-row (CUDA-core) tiles."""
+    row ranges straddle the 128-row (tensor-core) / 64-row (CUDA-core) tiles.  G=5 and G=8 are the DispResNet and PoseResNet
+    group counts of a five-frame sequence (--sequence-length 5)."""
     O = _ops()
     B, H, W, C, G = shape
     cx = O.ConvCtx(mode)

@@ -13,7 +13,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import rel_l2
+from helpers import Adam64, assert_adam_change, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -662,8 +662,7 @@ def test_adam_vs_torch_optim_fp64(wd):
         gr[zero] = 0.0
         grads.append(gr)
 
-    p64 = p0.double().requires_grad_(True)
-    opt = torch.optim.Adam([p64], lr=lr, betas=(b1, b2), eps=eps, weight_decay=wdf, foreach=False)
+    adam64 = Adam64(p0, lr, (b1, b2), eps, wdf)
     p = p0.to(DEV)
     m, v = torch.zeros_like(p), torch.zeros_like(p)
     # the same steps with the step count on the device and an operand mirror (TF32, then LO)
@@ -671,28 +670,12 @@ def test_adam_vs_torch_optim_fp64(wd):
             for op in (O.OPERAND_TF32, O.OPERAND_LO)]
     step_dev = torch.zeros(1, dtype=torch.int32, device=DEV)
     for step, gr in enumerate(grads, 1):
-        before64 = p64.detach().clone()
-        state = opt.state[p64]
-        m_prev = state["exp_avg"].clone() if state else torch.zeros(n, dtype=torch.float64)
-        g_eff = gr.double() + wdf * before64
-        p64.grad = gr.double()
-        opt.step()
-        want = p64.detach() - before64
+        want, size = adam64.step(gr)
         before = p.double().cpu()
         grc = gr.to(DEV)
         O.adam_step(p, grc, m, v, lr, b1, b2, eps, wdf, step)
         after = p.double().cpu()
-        got = after - before
-        # 1e-5 of the update's size, plus the rounding of the new fp32 parameter (at most 2^-24 of its magnitude).  The size
-        # is taken before m = b1 m + (1-b1) g cancels: where g undoes the previous steps the change itself is tiny, but the
-        # fp32 rounding of the two terms is not (that is fp32 noise, not a kernel error).
-        den = state["exp_avg_sq"].sqrt() / (1 - b2 ** step) ** 0.5 + eps
-        size = lr / (1 - b1 ** step) * (b1 * m_prev.abs() + (1 - b1) * g_eff.abs()) / den
-        err = (got - want).abs()
-        bound = 1e-5 * size + 2.0 ** -24 * after.abs()
-        worst = int(torch.argmax(err / bound))
-        assert bool((err <= bound).all()), "step %d: change %.9g vs fp64 %.9g (g = %.3g, error %.3g of the update size)" % (
-            step, float(got[worst]), float(want[worst]), float(gr[worst]), float(err[worst] / size[worst]))
+        assert_adam_change(after - before, want, size, after, gr, "step %d" % step)
         if wd == 0.0:
             _same_bits(p.cpu()[zero], p0[zero], "zero gradient leaves the parameter")
             assert float(m.cpu()[zero].abs().max()) == 0.0 and float(v.cpu()[zero].abs().max()) == 0.0

@@ -5,7 +5,7 @@ import pytest
 import torch
 
 from golden_util import det_weights
-from helpers import rel_l2
+from helpers import oracle_train_step, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -83,50 +83,45 @@ def test_two_training_steps_match_the_oracle(mode):
 
 
 _FULL = {}
-# benchmarked shapes: BASELINE config 2 (KITTI 256x832, 2 refs, 4 frames per GPU) and config 5 (NYU 256x320, `--folder-type pair`:
-# ONE reference frame, 8 frames per GPU)
-FULL_SHAPES = {"kitti": (4, 256, 832, 2, "kitti"), "nyu": (8, 256, 320, 1, "nyu")}
+# benchmarked shapes, (B, H, W, n_ref, intrinsics, DispResNet layers, PoseResNet layers): BASELINE config 2 (KITTI 256x832, 2 refs,
+# 4 frames per GPU), config 5 (NYU 256x320, `--folder-type pair`: ONE reference frame, 8 frames per GPU), bench.py's kitti_r50
+# (both networks ResNet-50, 2 frames per GPU) and what train.py --resnet-layers 50 builds for the reference's ResNet-50 scripts
+# (DispResNet-50 with PoseResNet-18, 4 frames per GPU)
+FULL_SHAPES = {"kitti": (4, 256, 832, 2, "kitti", 18, 18), "nyu": (8, 256, 320, 1, "nyu", 18, 18),
+               "kitti_r50": (2, 256, 832, 2, "kitti", 50, 50), "kitti_r50d": (4, 256, 832, 2, "kitti", 50, 18)}
 
 
 def _full_size_oracle(shape="kitti"):
     """One oracle step (fp32 and fp64 on the CPU, fp32 through stock PyTorch on the GPU) on a BENCHMARKED configuration, ssim +
-    mask + auto-mask.  Computed once per test session (~1 minute)."""
+    mask + auto-mask.  Computed once per test session (~1 minute per shape for ResNet-18)."""
     if shape not in _FULL:
-        from oracle import nets as N
-        from oracle import step as OS
         from scsfm import synth
-        B, H, W, n_ref, kind = FULL_SHAPES[shape]
+        B, H, W, n_ref, kind, dl, pl = FULL_SHAPES[shape]
         tgt, refs, K = synth.triplet(1234, B, H, W, n_ref, kind)
-        out = {"inputs": (tgt, refs, K)}
         torch.backends.cudnn.allow_tf32 = False
         torch.backends.cuda.matmul.allow_tf32 = False
-        for name, dt, dev in (("f32", torch.float32, "cpu"), ("f64", torch.float64, "cpu"), ("f32gpu", torch.float32, DEV)):
-            d, p = N.DispResNet(18).to(dt).to(dev), N.PoseResNet(18).to(dt).to(dev)
-            for net in (d, p):
-                net.load_state_dict({k: v.to(dt).to(dev) for k, v in det_weights(net.state_dict()).items()})
-                net.train()
-            losses = OS.train_step(d, p, OS.make_optimizer(d, p, lr=1e-4), tgt.to(dt).to(dev), [r.to(dt).to(dev) for r in refs],
-                                   K.to(dt).to(dev), num_scales=1, with_ssim=1, with_mask=1, with_auto_mask=1)
-            out[name] = ([float(v) for v in losses],
-                         {"disp." + k: q.grad.clone().cpu() for k, q in d.named_parameters() if q.grad is not None} |
-                         {"pose." + k: q.grad.clone().cpu() for k, q in p.named_parameters() if q.grad is not None})
-        _FULL[shape] = out
+        out = oracle_train_step(tgt, refs, K, disp_layers=dl, pose_layers=pl, lr=1e-4, gpu=DEV, num_scales=1, with_ssim=1,
+                                with_mask=1, with_auto_mask=1)
+        _FULL[shape] = {"inputs": (tgt, refs, K)} | {k: v[:2] for k, v in out.items()}
     return _FULL[shape]
 
 
-@pytest.mark.parametrize("mode,shape", [("tf32x3", "kitti"), ("tf32", "kitti"), ("fp32", "kitti"), ("tf32x3", "nyu")])
+@pytest.mark.parametrize("mode,shape", [("tf32x3", "kitti"), ("tf32", "kitti"), ("fp32", "kitti"), ("tf32x3", "nyu"),
+                                        ("tf32x3", "kitti_r50"), ("fp32", "kitti_r50"), ("tf32x3", "kitti_r50d")])
 def test_full_size_benchmarked_step_vs_oracle(mode, shape):
     """The step bench.py times (B=4, 256x832, auto-mask on) against the oracle, in every convolution mode: the four
     scalar losses and EVERY parameter gradient of both networks.  Yardstick for the gradients = the fp32 CPU oracle's own
     error against the fp64 oracle (kink pixels and ReLU gates flip between any two evaluations).  tf32x3 and fp32 are the
     parity modes (bound: 3x the larger error of two independent fp32 evaluations -- the CPU oracle and stock PyTorch / cuDNN with
     TF32 off on this GPU); tf32 (single product, cuDNN's default arithmetic) is only
-    required to stay within 1e-2 on the losses and is reported."""
+    required to stay within 1e-2 on the losses and is reported.  The ResNet-50 shapes run the bottleneck encoders through the
+    whole step at the benchmarked size."""
     import models
     from scsfm.trainer import Trainer
     o = _full_size_oracle(shape)
     tgt, refs, K = o["inputs"]
-    disp, pose = models.DispResNet(18, False), models.PoseResNet(18, False)
+    dl, pl = FULL_SHAPES[shape][5:]
+    disp, pose = models.DispResNet(dl, False), models.PoseResNet(pl, False)
     for net in (disp, pose):
         net.load_state_dict(det_weights(net.state_dict()))
     tr = Trainer(disp.to(DEV).train(), pose.to(DEV).train(), lr=1e-4, with_auto_mask=1, distributed=False, conv_mode=mode)
