@@ -1035,3 +1035,22 @@ class ArenaAdam:
         self._ensure_state()
         return {"step": self.step_count, "exp_avg": [self.state[id(n)][0] for n in self.nets],
                 "exp_avg_sq": [self.state[id(n)][1] for n in self.nets]}
+
+    def load_state_dict(self, sd):
+        """Load what state_dict() returns, in place: the moments and the device step counter keep their addresses (a captured
+        step and the camera's Adam hold them).  A different number of networks, or a moment arena whose length is not its
+        network's parameter arena's, raises ValueError before anything is copied."""
+        self._ensure_state()
+        for what in ("exp_avg", "exp_avg_sq"):
+            if len(sd[what]) != len(self.nets):
+                raise ValueError("optimizer state: %s holds %d networks, this ArenaAdam updates %d"
+                                 % (what, len(sd[what]), len(self.nets)))
+            for i, (n, src) in enumerate(zip(self.nets, sd[what])):
+                if tuple(src.shape) != tuple(n._flat.shape):
+                    raise ValueError("optimizer state: %s of network %d (%s) has shape %s, its parameter arena %s"
+                                     % (what, i, type(n).__name__, tuple(src.shape), tuple(n._flat.shape)))
+        for n, m0, v0 in zip(self.nets, sd["exp_avg"], sd["exp_avg_sq"]):
+            m, v, _ = self.state[id(n)]
+            m.copy_(m0)
+            v.copy_(v0)
+        self._step.fill_(int(sd["step"]))

@@ -234,6 +234,49 @@ class Trainer:
         m, v, step = self._cam_state
         return {"step": int(step.item()), "exp_avg": m, "exp_avg_sq": v}
 
+    def state_dict(self):
+        """CPU copies of everything training continues from: both networks' state_dict() (parameters, BatchNorm running
+        statistics, num_batches_tracked), the ArenaAdam state and, with a camera, its state_dict() and Adam state."""
+        cpu = lambda t: t.detach().contiguous().cpu()  # noqa: E731
+        opt = self.optimizer.state_dict()
+        sd = {"disp_net": {k: cpu(v) for k, v in self.disp_net.state_dict().items()},
+              "pose_net": {k: cpu(v) for k, v in self.pose_net.state_dict().items()},
+              "optimizer": {"step": opt["step"], "exp_avg": [cpu(t) for t in opt["exp_avg"]],
+                            "exp_avg_sq": [cpu(t) for t in opt["exp_avg_sq"]]}}
+        if self.camera is not None:
+            sd["camera"] = {k: cpu(v) for k, v in self.camera.state_dict().items()}
+            sd["camera_optimizer"] = {k: v if k == "step" else cpu(v) for k, v in self.camera_state_dict().items()}
+        return sd
+
+    def load_state_dict(self, sd):
+        """Load what state_dict() returns, in place, before or after capture(): a captured step and the gradient exchange keep
+        working on the same tensors.  A camera in `sd` but not in this Trainer, or the reverse, or a different number of cameras
+        raises ValueError.  Data parallel: every rank loads the same state, and rank 0's parameters are broadcast once more."""
+        has = "camera" in sd
+        if has != (self.camera is not None):
+            raise ValueError("the training state %s a learned camera and this Trainer %s" % (("holds", "has none") if has else
+                                                                                              ("holds no", "has one")))
+        if has and tuple(sd["camera"]["theta"].shape) != tuple(self.camera.theta.shape):
+            raise ValueError("the training state's camera theta is %s, this Trainer's %s: a different number of cameras"
+                             % (tuple(sd["camera"]["theta"].shape), tuple(self.camera.theta.shape)))
+        self.optimizer.load_state_dict(sd["optimizer"])          # (packs the arenas first: the networks load into them)
+        self.disp_net.load_state_dict(sd["disp_net"])
+        self.pose_net.load_state_dict(sd["pose_net"])
+        if has:
+            self.camera.load_state_dict(sd["camera"])
+            m, v, step = self._cam_state
+            m.copy_(sd["camera_optimizer"]["exp_avg"])
+            v.copy_(sd["camera_optimizer"]["exp_avg_sq"])
+            step.fill_(int(sd["camera_optimizer"]["step"]))
+        if self.exchange is not None:
+            self.exchange.broadcast_params([self.disp_net.flat_params(), self.pose_net.flat_params()] +
+                                           ([self.camera.theta.data] if has else []))
+        # the operand mirror: during replays only the Adam kernel writes it and no network call runs Python, so it is brought
+        # up to date here from the loaded arena (as capture() does after undoing the warm-up step)
+        for n in self.optimizer.nets:
+            n._tf32_version = None
+            n.refresh_operand_weights()
+
     def _check_intrinsics(self, intrinsics, capturing=False):
         """Learned intrinsics are supported by the eager single-GPU step only; elsewhere their gradient would be lost."""
         if intrinsics is None or not (torch.is_grad_enabled() and intrinsics.requires_grad):

@@ -22,11 +22,16 @@ networks' files (camera_model_best.pth.tar with the same best-copy rule).
 --camera-groups calibration | scene learns a bank of cameras instead: one per distinct cam.txt (KITTI raw's recording days,
 Cityscapes' sequences) or one per training scene (uncalibrated video), each sample seeing its own group's camera.  The
 checkpoint then holds theta [C,4] and a top-level 'groups' list of the cameras' labels.
+
+At the end of every epoch rank 0 also writes training_state.pth.tar beside the checkpoints: the networks, both Adams, the camera,
+the epoch, n_iter, best_error, the command line, the logs' row counts and every rank's random streams.  --resume RUN_DIR continues
+that run in RUN_DIR at the next epoch, as if it had not stopped.
 """
 import argparse
 import csv
 import datetime
 import os
+import random
 import shutil
 import time
 
@@ -101,6 +106,10 @@ parser.add_argument("--camera-groups", choices=["one", "calibration", "scene"], 
                          "matrix, per sample's intrinsics file with --folder-type pair (calibration: KITTI raw's recording days, "
                          "Cityscapes' sequences); one camera per training scene (scene: uncalibrated video).  Each camera starts from "
                          "its group's cam.txt, or every one from --intrinsics-init")
+parser.add_argument("--resume", default=None, metavar="RUN_DIR",
+                    help="continue the run saved in RUN_DIR (its training_state.pth.tar) at the epoch after the last one it finished, "
+                         "in RUN_DIR.  The other flags come from this command line; --resnet-layers, --learn-intrinsics, "
+                         "--camera-groups and the number of processes must be the run's")
 
 best_error = -1
 n_iter = 0
@@ -395,6 +404,95 @@ def save_camera_checkpoint(save_path, camera_state, is_best, filename="checkpoin
         shutil.copyfile(os.path.join(save_path, "camera_{}".format(filename)), os.path.join(save_path, "camera_model_best.pth.tar"))
 
 
+TRAINING_STATE = "training_state.pth.tar"
+
+
+def rng_state(device):
+    """This process's random streams: Python's `random` and numpy's (the augmentation draws), torch's CPU generator (the loaders'
+    shuffle) and, on a CUDA device, its generator."""
+    return {"python": random.getstate(), "numpy": np.random.get_state(), "torch": torch.get_rng_state(),
+            "cuda": torch.cuda.get_rng_state(device) if device.type == "cuda" else None}
+
+
+def set_rng_state(state, device):
+    random.setstate(state["python"])
+    np.random.set_state(state["numpy"])
+    torch.set_rng_state(state["torch"])
+    if state["cuda"] is not None:
+        torch.cuda.set_rng_state(state["cuda"], device)
+
+
+def gather_rng_states(world, device):
+    """Every rank's rng_state, in RANK order.  A collective with world > 1: every rank calls it."""
+    mine = rng_state(device)
+    if world == 1:
+        return [mine]
+    states = [None] * world
+    dist.all_gather_object(states, mine)
+    return states
+
+
+def log_rows(path):
+    """The number of data rows of a CSV log (its lines after the header)."""
+    with open(path, "rb") as f:
+        return sum(1 for _ in f) - 1
+
+
+def truncate_log(path, rows):
+    """Keep the header and the first `rows` data rows of a CSV log: the rows of an epoch that was cut off go."""
+    with open(path, "rb+") as f:
+        for i in range(rows + 1):
+            if not f.readline():
+                raise SystemExit("--resume: %s has %d data rows, fewer than the %d the training state counts" % (path, max(i - 1, 0), rows))
+        f.truncate(f.tell())
+
+
+def save_training_state(save_path, state):
+    """torch.save into a temporary file beside TRAINING_STATE, flushed to disk, then renamed over it: a run killed while
+    saving keeps its previous state whole."""
+    path = os.path.join(save_path, TRAINING_STATE)
+    tmp = path + ".tmp"
+    try:
+        with open(tmp, "wb") as f:
+            torch.save(state, f)
+            f.flush()
+            os.fsync(f.fileno())
+        os.replace(tmp, path)
+    except BaseException:
+        if os.path.exists(tmp):
+            os.remove(tmp)
+        raise
+
+
+def check_resume(args, cameras, world):
+    """--resume RUN_DIR: the training state saved in RUN_DIR (on the CPU), once this command line is known to continue it; None
+    without --resume.  SystemExit naming the flag otherwise.  Resuming with a different number of processes is not supported,
+    and the flags that set the shapes of the state must be the run's."""
+    if args.resume is None:
+        return None
+    if args.pretrained_disp or args.pretrained_pose:
+        raise SystemExit("--resume continues a run from its own training state; it does not take --pretrained-disp / --pretrained-pose")
+    path = os.path.join(args.resume, TRAINING_STATE)
+    if not os.path.isfile(path):
+        raise SystemExit("--resume %s: there is no %s in that directory (train.py writes it at the end of every epoch)"
+                         % (args.resume, TRAINING_STATE))
+    state = torch.load(path, map_location="cpu", weights_only=False)     # (the random streams and the command line are not tensors)
+    if state["world_size"] != world:
+        raise SystemExit("--resume: the run was trained by %d processes (WORLD_SIZE), this one has %d; resuming with a different "
+                         "number of GPUs is not supported" % (state["world_size"], world))
+    for name in ("resnet_layers", "learn_intrinsics", "camera_groups"):
+        if getattr(args, name) != state["args"][name]:
+            flag = "--" + name.replace("_", "-")
+            raise SystemExit("--resume: %s %s, the run was trained with %s %s (it sets the shapes of the saved state)"
+                             % (flag, getattr(args, name), flag, state["args"][name]))
+    if cameras is not None:
+        saved = state["trainer"]["camera"]["theta"].reshape(-1, 4).shape[0]
+        if saved != len(cameras):
+            raise SystemExit("--resume: the run learned %d cameras, the training scenes now give %d (--camera-groups %s)"
+                             % (saved, len(cameras), args.camera_groups))
+    return state
+
+
 def training_size(args, train_loader):
     if args.data == "synthetic":
         return tuple(args.synthetic_size)
@@ -409,6 +507,7 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
+    resume = check_resume(args, cameras, world)
     if not torch.cuda.is_available():
         raise SystemExit("train.py drives the H100 kernels: a CUDA device is required (no CPU fallback)")
     torch.cuda.set_device(local)
@@ -416,11 +515,20 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=device)
 
-    timestamp = datetime.datetime.now().strftime("%m-%d-%H:%M")
-    args.save_path = os.path.join("checkpoints", args.name, timestamp)
-    if rank == 0:
-        print("=> will save everything to {}".format(args.save_path))
-        os.makedirs(args.save_path, exist_ok=True)
+    if resume is None:
+        timestamp = datetime.datetime.now().strftime("%m-%d-%H:%M")
+        args.save_path = os.path.join("checkpoints", args.name, timestamp)
+        if rank == 0:
+            print("=> will save everything to {}".format(args.save_path))
+            os.makedirs(args.save_path, exist_ok=True)
+    else:
+        args.save_path = args.resume
+        if rank == 0:
+            print("=> resuming {} at epoch {}".format(args.save_path, resume["epoch"]))
+    # the reference's dataset classes seed Python's and numpy's streams with --seed as well (datasets/sequence_folders.py); seeding
+    # them here makes the augmentation draws of DIR = synthetic repeatable too
+    random.seed(args.seed)
+    np.random.seed(args.seed)
     torch.manual_seed(args.seed)
 
     bank = cameras is not None and cameras.mode != "one"          # every sample then carries its camera index
@@ -450,13 +558,25 @@ def main():
                       with_auto_mask=args.with_auto_mask, padding_mode=args.padding_mode, w1=args.photo_loss_weight,
                       w2=args.smooth_loss_weight, w3=args.geometry_consistency_weight, distributed=world > 1, conv_mode=args.conv_mode, overlap_nets=bool(args.overlap), overlap_wgrad=bool(args.overlap),
                       camera=camera, camera_lr=args.intrinsics_lr)
-    if rank == 0:
-        with open(os.path.join(args.save_path, args.log_summary), "w") as f:
-            csv.writer(f, delimiter="\t").writerow(["train_loss", "validation_loss"])
-        with open(os.path.join(args.save_path, args.log_full), "w") as f:
-            csv.writer(f, delimiter="\t").writerow(["train_loss", "photo_loss", "smooth_loss", "geometry_consistency_loss"])
+    logs = {"summary": os.path.join(args.save_path, args.log_summary), "full": os.path.join(args.save_path, args.log_full)}
+    if resume is None:
+        start_epoch, n_iter, best_error = 0, 0, -1
+        if rank == 0:
+            with open(logs["summary"], "w") as f:
+                csv.writer(f, delimiter="\t").writerow(["train_loss", "validation_loss"])
+            with open(logs["full"], "w") as f:
+                csv.writer(f, delimiter="\t").writerow(["train_loss", "photo_loss", "smooth_loss", "geometry_consistency_loss"])
+    else:
+        trainer.load_state_dict(resume["trainer"])
+        start_epoch, n_iter, best_error = resume["epoch"], resume["n_iter"], resume["best_error"]
+        if rank == 0:
+            for k, path in logs.items():
+                truncate_log(path, resume["log_rows"][k])
+        # last: building the datasets reseeds Python's and numpy's streams, and building the networks draws from torch's
+        set_rng_state(resume["rng"][rank], device)
+        resume = None                          # (the host copy of the state)
 
-    for epoch in range(args.epochs):
+    for epoch in range(start_epoch, args.epochs):
         sampler = getattr(train_loader, "sampler", None)
         if hasattr(sampler, "set_epoch"):
             sampler.set_epoch(epoch)           # DistributedSampler: a different shuffle every epoch
@@ -488,8 +608,13 @@ def main():
                 if camera.groups is not None:
                     state["groups"] = list(camera.groups)
                 save_camera_checkpoint(args.save_path, state, is_best)
-            with open(os.path.join(args.save_path, args.log_summary), "a") as f:
+            with open(logs["summary"], "a") as f:
                 csv.writer(f, delimiter="\t").writerow([train_loss, decisive])
+        rng = gather_rng_states(world, device)
+        if rank == 0:
+            save_training_state(args.save_path, {
+                "trainer": trainer.state_dict(), "epoch": epoch + 1, "n_iter": n_iter, "best_error": best_error, "args": vars(args),
+                "log_rows": {k: log_rows(path) for k, path in logs.items()}, "world_size": world, "rng": rng})
     if world > 1:
         dist.destroy_process_group()
 
@@ -509,8 +634,9 @@ def train(args, train_loader, trainer, device, rank, world):
         inputs = dict(intrinsics=intrinsics) if trainer.camera is None else dict(aug=batch[4])    # a learned camera builds K itself
         if len(batch) > 5:
             inputs["camera_index"] = batch[5]        # a bank of cameras: each sample's
-        if args.cuda_graph and world == 1 and trainer._graph is None and i == 0 and n_iter == 0:
+        if args.cuda_graph and world == 1 and trainer._graph is None:        # the first batch of the process
             trainer.capture(tgt_img, ref_imgs, **inputs)
+            print("=> captured the training step in a CUDA graph ({} kernel launches per step)".format(trainer.launches_per_step))
         out = trainer.step(tgt_img, ref_imgs, **inputs)
         rows.append(torch.stack(out))
         if i % args.print_freq == 0 or i >= args.epoch_size - 1:
