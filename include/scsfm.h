@@ -187,7 +187,7 @@ typedef struct ScsfmConv {
     double* bn_sums;
     int bn_groups;
     int B, Hi, Wi, Cin, Ho, Wo, Cout, kh, kw, stride, pad, pad_mode, act;
-    /* Split-accumulate ("3xTF32") operands of the tensor-core entry points, each optional (NULL = plain TF32):
+    /* Split-accumulate ("3xTF32") operands of the tensor-core kernels in SCSFM_MODE_TF32X3 (ignored in the other modes):
      * X_lo = tf32(X - trunc_tf32(X)) of the matching tensor (scsfm_split_tf32).  kind::tf32 reads only the upper 19 bits
      * of an fp32 operand, so the raw tensor IS the high part; with the low parts given the kernel accumulates
      * hi*hi + lo*hi + hi*lo into short fp32 accumulation chains (the dropped lo*lo term is 2^-22 relative), which restores
@@ -209,11 +209,8 @@ typedef struct ScsfmConv {
     /* forward only (NULL = off, 16-byte aligned, Cout % 4 == 0): also write tf32_lo(out) here, the split-accumulate low part a following tf32x3
      * convolution reads as in_lo (what scsfm_split_tf32 of the output would produce) */
     float* out_lo;
-    /* 1: split-accumulate (tf32x3) arithmetic.  With it, in_lo / dout_lo may be NULL where scsfm_conv_reads_lo() says the
-     * kernel chosen for the call computes them from the operands itself (w_lo is still required in the forward); a kernel
-     * that reads a low part which was not passed makes the call fail with SCSFM_ERR_ARG.  0: split mode as implied by the
-     * low parts passed. */
-    int split;
+    /* arithmetic, SCSFM_MODE_*: which kernels a call may run and which operands they read (scsfm_conv_plan) */
+    int mode;
 } ScsfmConv;
 
 /* ScsfmConv.tune */
@@ -223,49 +220,54 @@ typedef struct ScsfmConv {
 #define SCSFM_TUNE_BN(bn) (((bn) == 16 ? 1u : (bn) == 32 ? 2u : (bn) == 64 ? 3u : (bn) == 128 ? 4u : 0u) << 8)  /* weight rows in smem; TMA wgrad: Cout tile 32|64 */
 #define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 gather kernel, 2 TMA kernel, 3 thin-layer fp32 kernel */
 
-/* Exact-fp32 implicit-GEMM convolution on CUDA cores (every shape). */
-int scsfm_conv2d_fwd_simt(const ScsfmConv* p, void* stream);
-int scsfm_conv2d_dgrad_simt(const ScsfmConv* p, void* stream);
-int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream);
+/* ScsfmConv.mode */
+#define SCSFM_MODE_FP32 0     /* exact CUDA-core kernels */
+#define SCSFM_MODE_TF32 1     /* tensor cores, single TF32 product (operands rounded to TF32 by their producers) */
+#define SCSFM_MODE_TF32X3 2   /* tensor cores, split-accumulate products (the X_lo operands) */
 
-/* wgmma (tf32 operands, fp32 accumulation in registers) implicit-GEMM convolution; needs Cin % 4 == 0.
- * dgrad_tc: stride 1 or 2; p->w must hold the flipped/transposed weights [Cin,kh,kw,Cout] produced by
- * scsfm_weight_flip (the data gradient is the forward kernel run on dout). */
-/* Stride-1 (sub-)convolutions with kh, kw <= 3 run the TMA halo-patch kernel (conv_tma.cu: one 4-D tiled TMA load
- * per (channel chunk, dx) brings the input patch of a 2-D output tile, the kh vertical taps reuse it); reflection-
- * padded layers run it zero-padded and recompute the border ring with the gather kernel; so do the zero-padded stride-2
- * forwards with kh, kw <= 3, and the 7x7 stems run conv_stem_fwd.cu (below).  Other shapes use the cp.async gather
- * kernel.  wgrad_tc: stride-1 and zero-padded stride-2 layers with
- * kh, kw <= 3 and the 7x7 stride-2 stems (4 or 8 channels) run the TMA weight-gradient kernel (conv_wgrad_tma.cu). */
-int scsfm_conv2d_fwd_tc(const ScsfmConv* p, void* stream);
-int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream);
-int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream);
-/* The 7x7 stride-2 pad-3 zero-padded stems with Cin = 4 or 8 (padded) and Cout = 64 run a forward
- * kernel of their own (conv_stem_fwd.cu): a TMA box of the tile's input rows, the im2col operand fed to wgmma from
- * registers, and lo(in) computed from that operand. */
-/* Whether the kernel scsfm_conv2d_{fwd,dgrad,wgrad}_tc would pick for *p in split mode (tune knobs included) reads the
- * low parts of its activation operands: in_lo (SCSFM_PASS_FWD), dout_lo (SCSFM_PASS_DGRAD), in_lo and dout_lo
- * (SCSFM_PASS_WGRAD).  1 yes, 0 no (the kernel computes them itself), SCSFM_ERR_ARG for a bad descriptor or pass.  Only
- * the geometry, padding mode, epilogue pointers and tune of *p are looked at; nothing is launched. */
+/* Implicit-GEMM convolution, one entry per pass: forward with its epilogue, data gradient, weight gradient (+ bias gradient).
+ * The library picks the kernel (scsfm_conv_plan).  SCSFM_MODE_FP32 runs the exact CUDA-core kernels (conv_simt.cu).  The
+ * tf32 modes run the wgmma kernels (tf32 operands, fp32 accumulation) on the forwards with Cin % 4 == 0 and Cout >= 16, the
+ * data gradients of stride 1 or 2 with Cout % 4 == 0 and Cin >= 16 (the forward kernels on dout with the flipped weights of
+ * scsfm_weight_flip in w / w_lo; stride 2 as four parity-class sub-convolutions) and the weight gradients with Cin % 4 == 0,
+ * Cout % 4 == 0 and Cout >= 16: the 7x7 stem forward kernel (conv_stem_fwd.cu), the TMA halo-patch kernels (conv_tma.cu,
+ * conv_wgrad_tma.cu; reflection padding: zero-padded, plus the gather kernel over the border ring), the thin-layer fp32
+ * weight gradient (conv_wgrad_thin.cu) or the cp.async gather kernels (conv_tc.cu); everything else the CUDA-core kernels. */
+int scsfm_conv2d_fwd(const ScsfmConv* p, void* stream);
+int scsfm_conv2d_dgrad(const ScsfmConv* p, void* stream);
+int scsfm_conv2d_wgrad(const ScsfmConv* p, void* stream);
+/* The plan of call *p of pass SCSFM_PASS_*: the kernel that will run it (SCSFM_KERNEL_*, the low byte) OR-ed with
+ * SCSFM_PLAN_* flags naming what it reads beyond the plain operands; SCSFM_ERR_ARG for a bad descriptor or pass.  Only the
+ * geometry, mode, padding mode, BatchNorm sums and tune of *p are looked at; nothing is launched and no GPU is needed.  In
+ * tf32x3 mode a call whose kernel reads a low part that was not passed fails with SCSFM_ERR_ARG; low parts the kernel does not
+ * read are ignored.  A stride-2 data gradient reports the kernel of its parity class with the most taps. */
 #define SCSFM_PASS_FWD 0
 #define SCSFM_PASS_DGRAD 1
 #define SCSFM_PASS_WGRAD 2
-int scsfm_conv_reads_lo(const ScsfmConv* p, int pass);
+#define SCSFM_KERNEL_SIMT 0       /* CUDA-core implicit GEMM (conv_simt.cu) */
+#define SCSFM_KERNEL_GATHER 1     /* cp.async gather kernel (conv_tc.cu) */
+#define SCSFM_KERNEL_TMA 2        /* TMA halo-patch kernel (conv_tma.cu; weight gradient: conv_wgrad_tma.cu) */
+#define SCSFM_KERNEL_TMA_RING 3   /* the TMA kernel zero-padded, then the gather kernel over the reflection-padded border ring */
+#define SCSFM_KERNEL_STEM 4       /* 7x7 stem forward (conv_stem_fwd.cu) */
+#define SCSFM_KERNEL_THIN 5       /* thin-layer fp32 weight gradient (conv_wgrad_thin.cu) */
+#define SCSFM_PLAN_IN_LO 0x100    /* reads in_lo */
+#define SCSFM_PLAN_DOUT_LO 0x200  /* reads dout_lo */
+#define SCSFM_PLAN_W_LO 0x400     /* reads w_lo */
+#define SCSFM_PLAN_FLIPPED 0x800  /* w and w_lo are the flipped weights of scsfm_weight_flip (stride and pad of the call) */
+int scsfm_conv_plan(const ScsfmConv* p, int pass);
 /* Operand copies of a tensor for the tensor-core kernels: */
 #define SCSFM_OPERAND_TF32 0     /* round-to-nearest TF32 (plain TF32 mode) */
 #define SCSFM_OPERAND_RAW 1      /* bits unchanged (split mode: the MMA truncates, i.e. reads the high part) */
 #define SCSFM_OPERAND_LO 2       /* tf32(x - trunc_tf32(x)) (split mode: the low part) */
-/* flipped / transposed weights of the data gradient, `operand` = one of the above */
-int scsfm_weight_flip(const float* w, int Cout, int kh, int kw, int Cin, float* wt, int operand, void* stream);
-/* stride-2 data gradient: four parity-class weight sets back to back (Cin*kh*kw*Cout floats in total); p->w of
- * scsfm_conv2d_dgrad_tc must point to them when p->stride == 2 */
-int scsfm_weight_flip_s2(const float* w, int Cout, int kh, int kw, int Cin, int pad, float* wt4, int operand, void* stream);
+/* Flipped / transposed weights of the data gradient of a layer with weights w [Cout,kh,kw,Cin], stride 1 or 2 and padding
+ * pad, as operand kind `operand` (Cin*kh*kw*Cout floats): stride 1: [Cin,kh,kw,Cout] with reversed taps; stride 2: the four
+ * parity-class tap subsets back to back. */
+int scsfm_weight_flip(const float* w, int Cout, int kh, int kw, int Cin, int stride, int pad, float* wt, int operand, void* stream);
 
 /* Every flip of a network in one launch (the weights change once per optimizer step).  table: device array of
- * (n_rows + 1) x 12 int64 {src pointer, dst pointer, Cout, kh, kw, Cin, jh, jw, dy_max, dx_max, tap step | operand << 8, first block};
- * one row per scsfm_weight_flip job / per stride-2 parity class with taps (jh x jw taps kept, starting at (dy_max, dx_max)
- * and walking backwards by `tap step`); a row owns ceil(Cout/32) * ceil(Cin/32) * jh * jw blocks (one 32 x 32 tile
- * of one tap each) starting at its first block; the last row is a sentinel whose first block is total_blocks. */
+ * (n_rows + 1) x 10 int64 {src pointer, dst pointer, Cout, kh, kw, Cin, stride, pad, operand, first block}, one row per
+ * scsfm_weight_flip job; a row owns ceil(Cout/32) * ceil(Cin/32) * kh * kw blocks (one 32 x 32 tile of one tap each) starting
+ * at its first block; the last row is a sentinel whose first block is total_blocks. */
 int scsfm_weight_flip_batched(const long long* table, int n_rows, int total_blocks, void* stream);
 
 /* Disparity heads (DispResNet.py:79-82,98): 3x3 reflection-padded conv with one output channel, exact fp32.

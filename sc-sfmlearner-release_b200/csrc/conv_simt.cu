@@ -460,10 +460,7 @@ bias_grad_kernel(const float* __restrict__ dout, int rows, int C, float* __restr
     }
 }
 
-bool conv_wgrad_thin_eligible(const ScsfmConv& p);                       // conv_wgrad_thin.cu
-int launch_conv_wgrad_thin(const ScsfmConv& p, cudaStream_t st);
-
-// host-side launcher shared with the tensor-core weight gradient (conv_tc.cu)
+// bias gradient of every weight-gradient kernel (scsfm_conv2d_wgrad, conv_tc.cu)
 int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStream_t st) {
     const int gpr = C / 4;
     if ((C & 3) == 0 && gpr <= 64 && (gpr & (gpr - 1)) == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0) {
@@ -483,58 +480,27 @@ int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStrea
     return SCSFM_OK;
 }
 
-}  // namespace scsfm
-
-using namespace scsfm;
-
-static int check_conv(const ScsfmConv* p, const char* who) {
-    SCSFM_CHECK_ARG(p != nullptr, "%s: null descriptor", who);
-    SCSFM_CHECK_ARG(p->B > 0 && p->Hi > 0 && p->Wi > 0 && p->Cin > 0 && p->Ho > 0 && p->Wo > 0 && p->Cout > 0 && p->kh > 0 &&
-                        p->kw > 0 && p->stride > 0 && p->pad >= 0, "%s: bad geometry", who);
-    SCSFM_CHECK_ARG((long long)p->B * p->Hi * p->Wi * (long long)p->Cin < (1LL << 40), "%s: tensor too large", who);
-    return SCSFM_OK;
-}
-
-extern "C" int scsfm_conv2d_fwd_simt(const ScsfmConv* p, void* stream) {
-    if (int rc = check_conv(p, "conv2d_fwd")) return rc;
-    SCSFM_CHECK_ARG(p->in && p->w && p->out, "conv2d_fwd: null tensor");
-    SCSFM_CHECK_ARG(p->Ho == (p->Hi + 2 * p->pad - p->kh) / p->stride + 1 && p->Wo == (p->Wi + 2 * p->pad - p->kw) / p->stride + 1,
-                    "conv2d_fwd: output size does not match geometry");
-    SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || (p->pad < p->Hi && p->pad < p->Wi && p->pad <= 1), "conv2d_fwd: reflect pad must be 1");
-    SCSFM_CHECK_ARG((p->bn_scale == nullptr) == (p->bn_shift == nullptr), "conv2d_fwd: bn_scale and bn_shift go together");
-    SCSFM_CHECK_ARG(p->bn_scale == nullptr || (p->bias == nullptr && p->bn_sums == nullptr),
-                    "conv2d_fwd: the eval-mode BatchNorm epilogue excludes bias and bn_sums");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int M = p->B * p->Ho * p->Wo, N = p->Cout;
-    if (N <= 16) conv_fwd_simt_kernel<256, 16><<<dim3((M + 255) / 256, (N + 15) / 16), CT, 0, st>>>(*p);
-    else if (N <= 32) conv_fwd_simt_kernel<128, 32><<<dim3((M + 127) / 128, (N + 31) / 32), CT, 0, st>>>(*p);
-    else conv_fwd_simt_kernel<64, 64><<<dim3((M + 63) / 64, (N + 63) / 64), CT, 0, st>>>(*p);
+// Launchers of the kernels above for scsfm_conv2d_{fwd,dgrad,wgrad} (conv_tc.cu), which validate the call.
+int launch_fwd_simt(const ScsfmConv& p, cudaStream_t st) {
+    const int M = p.B * p.Ho * p.Wo, N = p.Cout;
+    if (N <= 16) conv_fwd_simt_kernel<256, 16><<<dim3((M + 255) / 256, (N + 15) / 16), CT, 0, st>>>(p);
+    else if (N <= 32) conv_fwd_simt_kernel<128, 32><<<dim3((M + 127) / 128, (N + 31) / 32), CT, 0, st>>>(p);
+    else conv_fwd_simt_kernel<64, 64><<<dim3((M + 63) / 64, (N + 63) / 64), CT, 0, st>>>(p);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
 
-extern "C" int scsfm_conv2d_dgrad_simt(const ScsfmConv* p, void* stream) {
-    if (int rc = check_conv(p, "conv2d_dgrad")) return rc;
-    SCSFM_CHECK_ARG(p->dout && p->w && p->din, "conv2d_dgrad: null tensor");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int M = p->B * p->Hi * p->Wi, N = p->Cin;
-    if (N <= 16) conv_dgrad_simt_kernel<256, 16><<<dim3((M + 255) / 256, (N + 15) / 16), CT, 0, st>>>(*p);
-    else if (N <= 32) conv_dgrad_simt_kernel<128, 32><<<dim3((M + 127) / 128, (N + 31) / 32), CT, 0, st>>>(*p);
-    else conv_dgrad_simt_kernel<64, 64><<<dim3((M + 63) / 64, (N + 63) / 64), CT, 0, st>>>(*p);
+int launch_dgrad_simt(const ScsfmConv& p, cudaStream_t st) {
+    const int M = p.B * p.Hi * p.Wi, N = p.Cin;
+    if (N <= 16) conv_dgrad_simt_kernel<256, 16><<<dim3((M + 255) / 256, (N + 15) / 16), CT, 0, st>>>(p);
+    else if (N <= 32) conv_dgrad_simt_kernel<128, 32><<<dim3((M + 127) / 128, (N + 31) / 32), CT, 0, st>>>(p);
+    else conv_dgrad_simt_kernel<64, 64><<<dim3((M + 63) / 64, (N + 63) / 64), CT, 0, st>>>(p);
     SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }
 
-extern "C" int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream) {
-    if (int rc = check_conv(p, "conv2d_wgrad")) return rc;
-    SCSFM_CHECK_ARG(p->dout && p->in && p->dw, "conv2d_wgrad: null tensor");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int M = p->Cout, N = p->kh * p->kw * p->Cin, Kall = p->B * p->Ho * p->Wo;
-    if (conv_wgrad_thin_eligible(*p) && ((p->tune >> 12) & 3u) != 1u) {       // thin decoder layers: direct kernel (conv_wgrad_thin.cu)
-        if (int rc = launch_conv_wgrad_thin(*p, st)) return rc;
-        if (p->dbias) return launch_bias_grad(p->dout, Kall, M, p->dbias, st);
-        return SCSFM_OK;
-    }
+int launch_wgrad_simt(const ScsfmConv& p, cudaStream_t st) {
+    const int M = p.Cout, N = p.kh * p.kw * p.Cin, Kall = p.B * p.Ho * p.Wo;
     auto plan = [&](int bm, int bn, dim3& grid, int& kps) {
         const int tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
         int splits = (132 * 4 + tiles - 1) / tiles;
@@ -546,10 +512,11 @@ extern "C" int scsfm_conv2d_wgrad_simt(const ScsfmConv* p, void* stream) {
     };
     dim3 grid;
     int kps;
-    if (M <= 16) { plan(16, 256, grid, kps); conv_wgrad_simt_kernel<16, 256><<<grid, CT, 0, st>>>(*p, kps); }
-    else if (M <= 32) { plan(32, 128, grid, kps); conv_wgrad_simt_kernel<32, 128><<<grid, CT, 0, st>>>(*p, kps); }
-    else { plan(64, 64, grid, kps); conv_wgrad_simt_kernel<64, 64><<<grid, CT, 0, st>>>(*p, kps); }
+    if (M <= 16) { plan(16, 256, grid, kps); conv_wgrad_simt_kernel<16, 256><<<grid, CT, 0, st>>>(p, kps); }
+    else if (M <= 32) { plan(32, 128, grid, kps); conv_wgrad_simt_kernel<32, 128><<<grid, CT, 0, st>>>(p, kps); }
+    else { plan(64, 64, grid, kps); conv_wgrad_simt_kernel<64, 64><<<grid, CT, 0, st>>>(p, kps); }
     SCSFM_CHECK_LAUNCH();
-    if (p->dbias) return launch_bias_grad(p->dout, Kall, M, p->dbias, st);
     return SCSFM_OK;
 }
+
+}  // namespace scsfm

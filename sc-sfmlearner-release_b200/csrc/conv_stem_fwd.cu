@@ -275,7 +275,6 @@ bool conv_stem_eligible(const ScsfmConv& p) {
     if (p.stride != 2 || p.kh != 7 || p.kw != 7 || p.pad != 3 || p.pad_mode != PADMODE_ZERO) return false;
     if ((p.Cin != 4 && p.Cin != 8) || p.Cout != 64) return false;
     if (p.Cin == 8 && p.Wi < 2) return false;                       // the odd-column view needs one column
-    if (p.in_lo != nullptr && p.w_lo == nullptr) return false;      // lo(x) x W alone is no mode of this kernel
     if (p.bn_sums && p.B % (p.bn_groups > 0 ? p.bn_groups : 1) != 0) return false;
     return true;
 }
@@ -319,7 +318,7 @@ static int launch_stem_cfg(const ScsfmConv& p, cudaStream_t st) {
 }
 
 int launch_conv_stem_fwd(const ScsfmConv& p, cudaStream_t st) {
-    const bool split = p.split || p.w_lo != nullptr;
+    const bool split = p.mode == SCSFM_MODE_TF32X3;
     if (p.Cin == 8) return split ? launch_stem_cfg<8, true>(p, st) : launch_stem_cfg<8, false>(p, st);
     return split ? launch_stem_cfg<4, true>(p, st) : launch_stem_cfg<4, false>(p, st);
 }

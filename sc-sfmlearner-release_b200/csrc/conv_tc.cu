@@ -13,7 +13,7 @@
 // A software gather is used instead of TMA-im2col because the same loader folds in reflection padding and the
 // transposed-convolution view used for the data gradient.
 //
-// dgrad (stride 1) is the same kernel run on dout with flipped/transposed weights (weight_flip_kernel below);
+// dgrad (stride 1) is the same kernel run on dout with flipped/transposed weights (weight_flip_tiles_kernel below);
 // for reflection-padded layers it returns the gradient of the padded tensor (pad' = 2), folded afterwards.
 //
 // Replaces cuDNN implicit-GEMM fwd/dgrad (SURVEY.md row K1) for every layer with Cin % 4 == 0.
@@ -319,24 +319,6 @@ conv_fwd_tc_kernel(ScsfmConv p, TcView v, const __grid_constant__ CUtensorMap wm
     }
 }
 
-// w [Co][kh][kw][Ci] -> wt [Ci][jh][jw][Co] with wt[c][jy][jx][o] = w[o][dy_max - step*jy][dx_max - step*jx][c]:
-// the (TF32-rounded) weights of the transposed conv.  step 1, d*_max = k-1: the full flipped kernel (stride-1 dgrad);
-// step 2: the taps of one output-parity class of a stride-2 dgrad.
-__global__ void weight_flip_kernel(const float* __restrict__ w, int Co, int kh, int kw, int Ci, int jh, int jw, int dy_max,
-                                   int dx_max, int step, float* __restrict__ wt, int operand) {
-    const long long total = (long long)Co * jh * jw * Ci;
-    for (long long i = blockIdx.x * 256LL + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-        const int o = (int)(i % Co);
-        long long t2 = i / Co;
-        const int jx = (int)(t2 % jw); t2 /= jw;
-        const int jy = (int)(t2 % jh);
-        const int c = (int)(t2 / jh);
-        const int dy = dy_max - step * jy, dx = dx_max - step * jx;
-        wt[i] = tc_operand(__ldg(w + (((size_t)o * kh + dy) * kw + dx) * Ci + c), operand);
-    }
-}
-
-
 // ---------------------------------------------------------------------------------------------------------
 // weight gradient on the tensor cores:  dW^T[(tap,c), o] += sum_pix  in[pix (+) tap, c] * dout[pix, o]
 //   GEMM  M = kh*kw*Cin (gathered input),  N = Cout (dout),  K = B*Ho*Wo pixels, split over gridDim.z; partial tiles are
@@ -571,8 +553,6 @@ int sm_count() {
     return n;
 }
 
-int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStream_t st);   // conv_simt.cu
-
 template <int BN, bool STACK = false>
 static int launch_wgrad_tc(const ScsfmConv& p, int border, cudaStream_t st) {
     using Cfg = WgCfg<BN>;
@@ -620,45 +600,10 @@ static int launch_fwd_tc(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
 
 using namespace scsfm;
 
-// Weight-gradient kernel for *p: 1 the gather kernel, 2 the TMA kernel (and the gather kernel on the ring of a reflection-
-// padded layer), 3 the thin-layer fp32 kernel.  SCSFM_TUNE_WGRAD: 0 auto, 1 the gather kernel, 2 the TMA kernel (the
-// gather kernel where it does not apply), 3 the thin-layer kernel.
-static int wgrad_kernel(const ScsfmConv& p) {
-    const bool split = p.split || (p.in_lo != nullptr && p.dout_lo != nullptr);
-    int kernel = (int)((p.tune >> 12) & 3u);
-    if (kernel == 3 && !conv_wgrad_thin_eligible(p)) kernel = 0;
-    // the 16-output-channel decoder layers in split mode read four tensors and use 16 of the MMA's columns: the fp32 FMA
-    // kernel reads two and is exact per product (conv_wgrad_thin.cu)
-    if (kernel == 0 && (split || p.in_lo != nullptr || p.dout_lo != nullptr) && conv_wgrad_thin_eligible(p)) kernel = 3;
-    if ((kernel == 0 || kernel == 2) && conv_wgrad_tma_eligible(p) && (split || (p.in_lo == nullptr && p.dout_lo == nullptr))) return 2;
-    return kernel == 3 ? 3 : 1;
-}
-
-// split mode: does the kernel the dispatcher picks for *p read the low parts of its activation operands?  The stem forward
-// kernel and the TMA / thin weight-gradient kernels compute or do not need them; the gather kernels and the TMA forward
-// read them, as does the gather pass over the ring of a reflection-padded weight gradient.
-static bool conv_reads_lo(const ScsfmConv& p, int pass) {
-    if (pass == SCSFM_PASS_FWD) return !conv_stem_eligible(p);
-    if (pass == SCSFM_PASS_WGRAD) {
-        ScsfmConv q = p;
-        q.split = 1;
-        const int k = wgrad_kernel(q);
-        return k == 1 || (k == 2 && p.pad_mode == PADMODE_REFLECT);
-    }
-    return true;
-}
-
-extern "C" int scsfm_conv_reads_lo(const ScsfmConv* p, int pass) {
-    SCSFM_CHECK_ARG(p != nullptr && pass >= SCSFM_PASS_FWD && pass <= SCSFM_PASS_WGRAD, "conv_reads_lo: bad arguments");
-    SCSFM_CHECK_ARG(p->B > 0 && p->Hi > 0 && p->Wi > 0 && p->Cin > 0 && p->Cout > 0 && p->kh > 0 && p->kw > 0 && p->stride > 0 && p->pad >= 0,
-                    "conv_reads_lo: bad geometry");
-    return conv_reads_lo(*p, pass) ? 1 : 0;
-}
-
 // cp.async gather kernel: any stride / padding mode / border-only rows
-static int tc_dispatch_gather(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
+static int launch_gather(const ScsfmConv& p, const TcView& v, bool stacked, cudaStream_t st) {
     const int N = p.Cout;
-    if (p.in_lo != nullptr && p.w_lo != nullptr && N <= 64) {       // split mode, thin: W / lo(W) stacked on the N side
+    if (stacked) {                                                  // split mode, thin: W / lo(W) stacked on the N side
         if (N <= 16) return launch_fwd_tc<32, true>(p, v, st);
         if (N <= 32) return launch_fwd_tc<64, true>(p, v, st);
         return launch_fwd_tc<128, true>(p, v, st);
@@ -672,133 +617,26 @@ static int tc_dispatch_gather(const ScsfmConv& p, const TcView& v, cudaStream_t 
     return launch_fwd_tc<128>(p, v, st);
 }
 
-// Stride-2 forwards the gather kernel runs faster than the TMA kernel (tools/conv_layers.py --only s2 --tune mt=1
-// --compare no_tma=1, H100): in split mode, Cin >= 512 into output planes of at most 8 x 26 pixels (the ResNet-50 layer4
-// 3x3 512 -> 512 and 1x1 1024 -> 2048).  Two 128-pixel tiles per image leave most SMs idle through a long K loop, where
-// the gather kernel's 64-pixel tiles give twice the CTAs.  The ResNet-18 layer4 (Cin 256) and every tf32 shape are at
-// least as fast on the TMA kernel.
-static bool s2_prefers_gather(const ScsfmConv& p, const TcView& v) {
-    return v.in_stride == 2 && p.in_lo != nullptr && p.Cin >= 512 && p.Ho * p.Wo <= 8 * 26 && !conv_tma_forced(p);
-}
-
-static int tc_dispatch(const ScsfmConv& p, const TcView& v, cudaStream_t st) {
-    if (conv_stem_eligible(p)) return launch_conv_stem_fwd(p, st);      // (a data gradient's sub-convolutions have stride 1)
-    if (p.pad_mode == PADMODE_ZERO && conv_tma_eligible(p, v) && !s2_prefers_gather(p, v)) return launch_conv_tma(p, v, st);
-    if (p.pad_mode == PADMODE_REFLECT && v.in_stride == 1 && p.bn_sums == nullptr && p.Ho >= 3 && p.Wo >= 3 &&
-        (p.Ho * p.Wo >= 64 * 208 || conv_tma_forced(p)) && conv_tma_eligible(p, v)) {
-        // reflection padding only changes the outermost ring of output pixels: run the TMA kernel with zero padding
-        // (interior exact), then recompute the 2*(Ho+Wo)-4 border pixels per image with the reflecting gather kernel.
-        // Measured on H100 (tools/conv_layers.py --only dec --compare mt=1, tf32x3): pays off from 64x208 upwards; below
-        // that the ring is too large a share of the image and the gather kernel alone is as fast or faster (8x26:
-        // x0.63, 16x52: x0.95; at 32x104 the split was x1.14, not yet taken: tf32 unmeasured).
-        ScsfmConv q = p;
-        q.pad_mode = PADMODE_ZERO;
-        if (int rc = launch_conv_tma(q, v, st)) return rc;
-        TcView bv = v;
-        bv.border = 1;
-        return tc_dispatch_gather(p, bv, st);
+// cp.async gather weight-gradient kernel: any stride / padding mode (whatever the TMA kernel does not take); border = 1:
+// the image-border ring pixels only
+static int launch_wgrad_gather(const ScsfmConv& p, bool stacked, int border, cudaStream_t st) {
+    if (stacked) {                                                  // split mode, thin: dout / lo(dout) stacked on the N side
+        if (p.Cout <= 16) return launch_wgrad_tc<32, true>(p, border, st);
+        if (p.Cout <= 32) return launch_wgrad_tc<64, true>(p, border, st);
+        return launch_wgrad_tc<128, true>(p, border, st);
     }
-    return tc_dispatch_gather(p, v, st);
-}
-
-static int check_tc(const ScsfmConv* p, const char* who) {
-    SCSFM_CHECK_ARG(p != nullptr && p->in && p->w && p->out, "%s: null tensor", who);
-    SCSFM_CHECK_ARG(p->B > 0 && p->Hi > 0 && p->Wi > 0 && p->Cin > 0 && p->Cout > 0 && p->kh > 0 && p->kw > 0 && p->stride > 0 && p->pad >= 0,
-                    "%s: bad geometry", who);
-    SCSFM_CHECK_ARG((p->Cin & 3) == 0, "%s: the tensor-core kernel needs Cin %% 4 == 0 (got %d); use the CUDA-core kernel", who, p->Cin);
-    SCSFM_CHECK_ARG(p->Ho == (p->Hi + 2 * p->pad - p->kh) / p->stride + 1 && p->Wo == (p->Wi + 2 * p->pad - p->kw) / p->stride + 1,
-                    "%s: output size does not match geometry", who);
-    SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || p->pad == 1, "%s: reflect pad must be 1", who);
-    if (p->bn_sums) {
-        const int g = p->bn_groups > 0 ? p->bn_groups : 1;
-        SCSFM_CHECK_ARG(p->B % g == 0, "%s: batch not divisible by the number of BatchNorm groups", who);
-    }
-    SCSFM_CHECK_ARG((p->bn_scale == nullptr) == (p->bn_shift == nullptr), "%s: bn_scale and bn_shift go together", who);
-    SCSFM_CHECK_ARG(p->bn_scale == nullptr || (p->bias == nullptr && p->bn_sums == nullptr),
-                    "%s: the eval-mode BatchNorm epilogue excludes bias and bn_sums", who);
-    SCSFM_CHECK_ARG(p->out_lo == nullptr || ((p->Cout & 3) == 0 && (reinterpret_cast<uintptr_t>(p->out_lo) & 15) == 0),
-                    "%s: out_lo needs Cout %% 4 == 0 and 16-byte alignment", who);
-    SCSFM_CHECK_ARG(((reinterpret_cast<uintptr_t>(p->bn_scale) | reinterpret_cast<uintptr_t>(p->bn_shift)) & 7) == 0,
-                    "%s: bn_scale / bn_shift must be 8-byte aligned", who);
-    return SCSFM_OK;
-}
-
-extern "C" int scsfm_conv2d_fwd_tc(const ScsfmConv* p, void* stream) {
-    if (int rc = check_tc(p, "conv2d_fwd_tc")) return rc;
-    if (p->split) {
-        SCSFM_CHECK_ARG(p->w_lo != nullptr, "conv2d_fwd_tc: split mode needs w_lo");
-        SCSFM_CHECK_ARG(p->in_lo != nullptr || !conv_reads_lo(*p, SCSFM_PASS_FWD),
-                        "conv2d_fwd_tc: the kernel chosen for this call reads in_lo, which was not passed (scsfm_conv_reads_lo)");
-    }
-    return tc_dispatch(*p, plain_view(*p), (cudaStream_t)stream);
-}
-
-extern "C" int scsfm_weight_flip(const float* w, int Cout, int kh, int kw, int Cin, float* wt, int operand, void* stream) {
-    SCSFM_CHECK_ARG(w && wt && Cout > 0 && kh > 0 && kw > 0 && Cin > 0 && operand >= 0 && operand <= 2, "weight_flip: bad arguments");
-    const long long total = (long long)Cout * kh * kw * Cin;
-    int grid = (int)((total + 255) / 256);
-    if (grid > sm_count() * 16) grid = sm_count() * 16;
-    weight_flip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, Cout, kh, kw, Cin, kh, kw, kh - 1, kw - 1, 1, wt, operand);
-    SCSFM_CHECK_LAUNCH();
-    return SCSFM_OK;
-}
-
-// All flips of a network in ONE launch.  table = n rows of 12 int64: {src pointer, dst pointer, Co, kh, kw, Ci, jh, jw,
-// dy_max, dx_max, step, first block}; a row is one weight_flip_kernel job (a stride-2 layer contributes one row per parity
-// class with taps) and owns blocks [first block, next row's first block); row n is a sentinel holding the total.
-// Each block transposes one 32 (Cout) x 32 (Cin) tile of one tap through shared memory: reads coalesced along Cin, writes
-// coalesced along Cout.  A row owns ceil(Co/32) * ceil(Ci/32) * jh * jw blocks.
-__global__ void __launch_bounds__(256)
-weight_flip_batched_kernel(const long long* __restrict__ table, int n) {
-    __shared__ int s_row;
-    __shared__ float tile[32][33];
-    if (threadIdx.x == 0) {
-        int lo = 0, hi = n;                       // last row with first block <= blockIdx.x
-        while (hi - lo > 1) {
-            const int mid = (lo + hi) >> 1;
-            if (table[mid * 12 + 11] <= (long long)blockIdx.x) lo = mid; else hi = mid;
-        }
-        s_row = lo;
-    }
-    __syncthreads();
-    const long long* e = table + s_row * 12;
-    const float* w = reinterpret_cast<const float*>(e[0]);
-    float* wt = reinterpret_cast<float*>(e[1]);
-    const int Co = (int)e[2], kh = (int)e[3], kw = (int)e[4], Ci = (int)e[5], jh = (int)e[6], jw = (int)e[7];
-    const int dy_max = (int)e[8], dx_max = (int)e[9], step = (int)(e[10] & 0xff), operand = (int)(e[10] >> 8);
-    const int tco = (Co + 31) >> 5, tci = (Ci + 31) >> 5;
-    int t = (int)((long long)blockIdx.x - e[11]);
-    const int to = t % tco; t /= tco;
-    const int tc = t % tci; t /= tci;
-    const int jy = t / jw, jx = t - jy * jw;
-    const int dy = dy_max - step * jy, dx = dx_max - step * jx;
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int o = to * 32 + ty + 8 * k, c = tc * 32 + tx;
-        if (o < Co && c < Ci) tile[ty + 8 * k][tx] = tc_operand(__ldg(w + (((size_t)o * kh + dy) * kw + dx) * Ci + c), operand);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int c = tc * 32 + ty + 8 * k, o = to * 32 + tx;
-        if (c < Ci && o < Co) wt[(((size_t)c * jh + jy) * jw + jx) * Co + o] = tile[tx][ty + 8 * k];
-    }
-}
-
-extern "C" int scsfm_weight_flip_batched(const long long* table, int n_rows, int total_blocks, void* stream) {
-    SCSFM_CHECK_ARG(table != nullptr && n_rows > 0 && total_blocks > 0, "weight_flip_batched: bad arguments");
-    weight_flip_batched_kernel<<<total_blocks, 256, 0, (cudaStream_t)stream>>>(table, n_rows);
-    SCSFM_CHECK_LAUNCH();
-    return SCSFM_OK;
+    if (p.Cout <= 16) return launch_wgrad_tc<16>(p, border, st);
+    if (p.Cout <= 32) return launch_wgrad_tc<32>(p, border, st);
+    if (p.Cout <= 64) return launch_wgrad_tc<64>(p, border, st);
+    return launch_wgrad_tc<128>(p, border, st);
 }
 
 // Output-parity class (py, px) of a stride-2 data gradient: the kernel rows dy_max, dy_max - 2, ... (jh of them) and
-// columns dx_max, dx_max - 2, ... (jw) reach it; jh or jw = 0: no tap does.
+// columns dx_max, dx_max - 2, ... (jw) reach it; jh or jw = 0: no tap does.  The four classes partition the taps.
 struct S2Class {
     int jh, jw, dy_max, dx_max;
 };
-static S2Class s2_class(int kh, int kw, int pad, int py, int px) {
+__host__ __device__ static S2Class s2_class(int kh, int kw, int pad, int py, int px) {
     S2Class k{0, 0, kh - 1, kw - 1};
     while (k.dy_max >= 0 && ((py + pad - k.dy_max) & 1)) --k.dy_max;
     while (k.dx_max >= 0 && ((px + pad - k.dx_max) & 1)) --k.dx_max;
@@ -807,119 +645,334 @@ static S2Class s2_class(int kh, int kw, int pad, int py, int px) {
     return k;
 }
 
-// Stride-2 data gradient: wt4 receives the four parity-class weight sets back to back (class order (py,px) =
-// (0,0),(0,1),(1,0),(1,1)); total size = Cin*kh*kw*Cout floats, the same as the full flipped kernel.
-extern "C" int scsfm_weight_flip_s2(const float* w, int Cout, int kh, int kw, int Cin, int pad, float* wt4, int operand, void* stream) {
-    SCSFM_CHECK_ARG(w && wt4 && Cout > 0 && kh > 0 && kw > 0 && Cin > 0 && pad >= 0 && operand >= 0 && operand <= 2, "weight_flip_s2: bad arguments");
-    size_t off = 0;
-    for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-            const S2Class k = s2_class(kh, kw, pad, py, px);
-            const long long total = (long long)Cout * k.jh * k.jw * Cin;
-            if (total > 0) {
-                int grid = (int)((total + 255) / 256);
-                if (grid > sm_count() * 16) grid = sm_count() * 16;
-                weight_flip_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, Cout, kh, kw, Cin, k.jh, k.jw, k.dy_max, k.dx_max, 2, wt4 + off,
-                                                                           operand);
-                SCSFM_CHECK_LAUNCH();
-            }
-            off += (size_t)total;
-        }
-    return SCSFM_OK;
-}
-
-// stride-1 data gradient = forward kernel on dout with the flipped weights `wt` ([Cin][kh][kw][Cout], from
-// scsfm_weight_flip) passed in p->w; p->din [B,Hi,Wi,Cin] (+ p->addend).
-extern "C" int scsfm_conv2d_dgrad_tc(const ScsfmConv* p, void* stream) {
-    SCSFM_CHECK_ARG(p != nullptr && p->dout && p->w && p->din, "conv2d_dgrad_tc: null tensor");
-    SCSFM_CHECK_ARG(p->stride == 1 || p->stride == 2, "conv2d_dgrad_tc: stride must be 1 or 2");
-    SCSFM_CHECK_ARG(!p->split || (p->dout_lo != nullptr && p->w_lo != nullptr), "conv2d_dgrad_tc: split mode needs dout_lo and w_lo");
-    SCSFM_CHECK_ARG(p->kh == p->kw && p->kh - 1 - p->pad >= 0, "conv2d_dgrad_tc: square kernels only");
-    cudaStream_t st = (cudaStream_t)stream;
-    ScsfmConv q = *p;
-    q.in = p->dout; q.in_lo = p->dout_lo; q.out = p->din; q.bias = nullptr; q.bn_sums = nullptr; q.act = SCSFM_ACT_NONE;
-    q.bn_scale = nullptr; q.bn_shift = nullptr; q.out_lo = nullptr;
-    q.dout_lo = nullptr;                       // (w_lo: the flipped low-part weights, laid out like w)
-    q.Hi = p->Ho; q.Wi = p->Wo; q.Cin = p->Cout;
-    q.Cout = p->Cin; q.pad_mode = SCSFM_PADMODE_ZERO;
-    if (p->stride == 1) {
-        q.Ho = p->Hi; q.Wo = p->Wi;
-        q.pad = p->kh - 1 - p->pad;
-        if (int rc = check_tc(&q, "conv2d_dgrad_tc")) return rc;
-        return tc_dispatch(q, plain_view(q), st);
+// The data gradient of p as forward convolutions on dout with the flipped weights (p.w / p.w_lo from scsfm_weight_flip)
+// into din, part cls seen through v: at stride 1 one convolution (cls 0), at stride 2 the stride-1 sub-convolution of
+// output-parity class cls = 2 py + px (its weights follow the earlier classes' in the flipped set).  r.kh * r.kw = 0: no tap
+// reaches the part; r.Ho * r.Wo = 0: din has no pixel in it.
+static void dgrad_part(const ScsfmConv& p, int cls, ScsfmConv& r, TcView& v) {
+    r = p;
+    r.in = p.dout; r.in_lo = p.dout_lo; r.out = p.din; r.bias = nullptr; r.bn_sums = nullptr; r.act = SCSFM_ACT_NONE;
+    r.bn_scale = nullptr; r.bn_shift = nullptr; r.out_lo = nullptr; r.dout_lo = nullptr;     // w_lo: laid out like w
+    r.Hi = p.Ho; r.Wi = p.Wo; r.Cin = p.Cout; r.Cout = p.Cin; r.pad_mode = SCSFM_PADMODE_ZERO; r.stride = 1;
+    if (p.stride == 1) {
+        r.Ho = cls == 0 ? p.Hi : 0; r.Wo = p.Wi; r.pad = p.kh - 1 - p.pad;
+        v = plain_view(r);
+        return;
     }
-    // stride 2: p->w holds the four parity-class weight sets of scsfm_weight_flip_s2
-    SCSFM_CHECK_ARG((q.Cin & 3) == 0, "conv2d_dgrad_tc: needs Cout %% 4 == 0");
-    q.stride = 1;
-    bool covered_all = true;
-    for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-            const S2Class k = s2_class(p->kh, p->kw, p->pad, py, px);
-            const int Hs = (p->Hi - py + 1) / 2, Ws = (p->Wi - px + 1) / 2;
-            if ((k.jh == 0 || k.jw == 0) && Hs > 0 && Ws > 0) covered_all = false;
-        }
-    if (!covered_all) {
-        // parity classes without taps (1x1 stride 2): their gradient is the addend alone (or zero).  Enqueued before the
-        // sub-convolutions, which write the other classes' pixels of din.
-        const size_t bytes = (size_t)p->B * p->Hi * p->Wi * p->Cin * sizeof(float);
-        if (p->addend) SCSFM_CHECK_CUDA(cudaMemcpyAsync(p->din, p->addend, bytes, cudaMemcpyDeviceToDevice, st));
-        else SCSFM_CHECK_CUDA(cudaMemsetAsync(p->din, 0, bytes, st));
-    }
+    const int py = cls >> 1, px = cls & 1;
     size_t woff = 0;
-    for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-            const S2Class k = s2_class(p->kh, p->kw, p->pad, py, px);
-            const int Hs = (p->Hi - py + 1) / 2, Ws = (p->Wi - px + 1) / 2;
-            if (k.jh > 0 && k.jw > 0 && Hs > 0 && Ws > 0) {
-                ScsfmConv r = q;
-                r.w = p->w + woff;
-                r.w_lo = p->w_lo ? p->w_lo + woff : nullptr;
-                r.Ho = Hs; r.Wo = Ws; r.kh = k.jh; r.kw = k.jw;
-                // input (dout) row of output hy and tap jy: hy + (py + pad - dy_max)/2 + jy
-                TcView v{k.jh, k.jw, (py + p->pad - k.dy_max) / 2, (px + p->pad - k.dx_max) / 2, 1, 2, py, 2, px, p->Hi, p->Wi};
-                if (int rc = tc_dispatch(r, v, st)) return rc;
+    for (int c = 0; c < cls; ++c) {
+        const S2Class k = s2_class(p.kh, p.kw, p.pad, c >> 1, c & 1);
+        woff += (size_t)p.Cout * k.jh * k.jw * p.Cin;
+    }
+    const S2Class k = s2_class(p.kh, p.kw, p.pad, py, px);
+    r.w = p.w != nullptr ? p.w + woff : nullptr;
+    r.w_lo = p.w_lo != nullptr ? p.w_lo + woff : nullptr;
+    r.Ho = (p.Hi - py + 1) / 2; r.Wo = (p.Wi - px + 1) / 2; r.kh = k.jh; r.kw = k.jw;
+    // input (dout) row of output hy and tap jy: hy + (py + pad - dy_max)/2 + jy
+    v = TcView{k.jh, k.jw, (py + p.pad - k.dy_max) / 2, (px + p.pad - k.dx_max) / 2, 1, 2, py, 2, px, p.Hi, p.Wi};
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Routing: which kernel runs a call and which operands it reads.  conv_plan is the only place these rules live; the
+// entry points below validate for, and launch, what it picks.
+// ---------------------------------------------------------------------------------------------------------
+struct ConvPlan {
+    int kernel;          // SCSFM_KERNEL_*
+    unsigned reads;      // SCSFM_PLAN_* operand flags
+    bool stacked;        // split mode, Cout <= 64: the gather kernel (and the ring pass) stacks W and lo(W) (weight
+                         // gradient: dout and lo(dout)) on the N side of one tile, 2 passes instead of 3
+};
+
+// Stride-2 forwards the gather kernel runs faster than the TMA kernel (tools/conv_layers.py --only s2 --tune mt=1
+// --compare no_tma=1, H100): in split mode, Cin >= 512 into output planes of at most 8 x 26 pixels (the ResNet-50 layer4
+// 3x3 512 -> 512 and 1x1 1024 -> 2048).  Two 128-pixel tiles per image leave most SMs idle through a long K loop, where
+// the gather kernel's 64-pixel tiles give twice the CTAs.  The ResNet-18 layer4 (Cin 256) and every tf32 shape are at
+// least as fast on the TMA kernel.
+static bool s2_prefers_gather(const ScsfmConv& p, const TcView& v) {
+    return v.in_stride == 2 && p.mode == SCSFM_MODE_TF32X3 && p.Cin >= 512 && p.Ho * p.Wo <= 8 * 26 && !conv_tma_forced(p);
+}
+
+// Tensor-core forward (sub-)convolution p seen through v: the stem kernel, the TMA kernel, the TMA kernel plus the gather
+// kernel over the border ring, or the gather kernel.
+static ConvPlan route_tc(const ScsfmConv& p, const TcView& v) {
+    const bool split = p.mode == SCSFM_MODE_TF32X3;
+    ConvPlan r{SCSFM_KERNEL_GATHER, split ? SCSFM_PLAN_IN_LO | SCSFM_PLAN_W_LO : 0u, split && p.Cout <= 64};
+    if (conv_stem_eligible(p)) {                    // (a data gradient's sub-convolutions have stride 1)
+        r.kernel = SCSFM_KERNEL_STEM;
+        r.reads &= ~(unsigned)SCSFM_PLAN_IN_LO;     // lo(in) comes from the A fragment
+    } else if (p.pad_mode == PADMODE_ZERO && conv_tma_eligible(p, v) && !s2_prefers_gather(p, v)) {
+        r.kernel = SCSFM_KERNEL_TMA;
+    } else if (p.pad_mode == PADMODE_REFLECT && v.in_stride == 1 && p.bn_sums == nullptr && p.Ho >= 3 && p.Wo >= 3 &&
+               (p.Ho * p.Wo >= 64 * 208 || conv_tma_forced(p)) && conv_tma_eligible(p, v)) {
+        // reflection padding only changes the outermost ring of output pixels: run the TMA kernel with zero padding
+        // (interior exact), then recompute the 2*(Ho+Wo)-4 border pixels per image with the reflecting gather kernel.
+        // Measured on H100 (tools/conv_layers.py --only dec --compare mt=1, tf32x3): pays off from 64x208 upwards; below
+        // that the ring is too large a share of the image and the gather kernel alone is as fast or faster (8x26:
+        // x0.63, 16x52: x0.95; at 32x104 the split was x1.14, not yet taken: tf32 unmeasured).
+        r.kernel = SCSFM_KERNEL_TMA_RING;
+    }
+    return r;
+}
+
+// The kernel that runs call p of `pass` and the operands it reads (include/scsfm.h, scsfm_conv_plan).
+static ConvPlan conv_plan(const ScsfmConv& p, int pass) {
+    const bool tc = p.mode != SCSFM_MODE_FP32, split = p.mode == SCSFM_MODE_TF32X3;
+    const ConvPlan simt{SCSFM_KERNEL_SIMT, 0u, false};
+    if (pass == SCSFM_PASS_FWD) {
+        if (!tc || (p.Cin & 3) != 0 || p.Cout < 16) return simt;
+        return route_tc(p, plain_view(p));
+    }
+    if (pass == SCSFM_PASS_DGRAD) {
+        // the forward routing on dout, per part (dgrad_part); reported: the part with the most taps (at stride 2 the others
+        // take the same kernel unless kh or kw > 3)
+        if (!tc || (p.stride != 1 && p.stride != 2) || (p.Cout & 3) != 0 || p.Cin < 16) return simt;
+        ConvPlan r{SCSFM_KERNEL_GATHER, 0u, false};
+        for (int cls = 0, taps = 0; cls < 4; ++cls) {
+            ScsfmConv q;
+            TcView v;
+            dgrad_part(p, cls, q, v);
+            if (q.kh * q.kw > taps && q.Ho > 0 && q.Wo > 0) {
+                taps = q.kh * q.kw;
+                r = route_tc(q, v);
             }
-            woff += (size_t)p->Cout * k.jh * k.jw * p->Cin;
         }
+        r.reads = (split ? SCSFM_PLAN_DOUT_LO | SCSFM_PLAN_W_LO : 0u) | SCSFM_PLAN_FLIPPED;
+        return r;
+    }
+    // weight gradient.  SCSFM_TUNE_WGRAD: 0 auto, 1 the gather kernel (CUDA cores: the generic kernel), 2 the TMA kernel
+    // (the gather kernel where it does not apply), 3 the thin-layer kernel (auto where it does not apply)
+    const unsigned knob = (p.tune >> 12) & 3u;
+    const bool thin = conv_wgrad_thin_eligible(p);
+    const ConvPlan thin_plan{SCSFM_KERNEL_THIN, 0u, false};
+    if (!tc || (p.Cin & 3) != 0 || (p.Cout & 3) != 0 || p.Cout < 16) return thin && knob != 1u ? thin_plan : simt;
+    // the 16-output-channel decoder layers in split mode read four tensors and use 16 of the MMA's columns: the fp32 FMA
+    // kernel reads two and is exact per product (conv_wgrad_thin.cu)
+    if (thin && (knob == 3u || (knob == 0u && split))) return thin_plan;
+    const unsigned lo = split ? SCSFM_PLAN_IN_LO | SCSFM_PLAN_DOUT_LO : 0u;
+    if (knob != 1u && conv_wgrad_tma_eligible(p)) {
+        // the TMA kernel computes the low parts itself; under reflection padding it takes the interior pixels with zero
+        // padding and the gather kernel, which reads them, the border ring
+        if (p.pad_mode == PADMODE_REFLECT) return ConvPlan{SCSFM_KERNEL_TMA_RING, lo, split && p.Cout <= 64};
+        return ConvPlan{SCSFM_KERNEL_TMA, 0u, false};
+    }
+    return ConvPlan{SCSFM_KERNEL_GATHER, lo, split && p.Cout <= 64};
+}
+
+// Launches the kernel route_tc picked for the forward (sub-)convolution p seen through v.
+static int launch_route(const ScsfmConv& p, const TcView& v, const ConvPlan& r, cudaStream_t st) {
+    switch (r.kernel) {
+        case SCSFM_KERNEL_STEM: return launch_conv_stem_fwd(p, st);
+        case SCSFM_KERNEL_TMA: return launch_conv_tma(p, v, st);
+        case SCSFM_KERNEL_TMA_RING: {
+            ScsfmConv q = p;                        // the interior: zero padding
+            q.pad_mode = PADMODE_ZERO;
+            if (int rc = launch_conv_tma(q, v, st)) return rc;
+            TcView ring = v;
+            ring.border = 1;
+            return launch_gather(p, ring, r.stacked, st);
+        }
+        default: return launch_gather(p, v, r.stacked, st);
+    }
+}
+
+static int check_desc(const ScsfmConv* p, const char* who) {
+    SCSFM_CHECK_ARG(p != nullptr, "%s: null descriptor", who);
+    SCSFM_CHECK_ARG(p->B > 0 && p->Hi > 0 && p->Wi > 0 && p->Cin > 0 && p->Ho > 0 && p->Wo > 0 && p->Cout > 0 && p->kh > 0 &&
+                        p->kw > 0 && p->stride > 0 && p->pad >= 0, "%s: bad geometry", who);
+    SCSFM_CHECK_ARG(p->mode >= SCSFM_MODE_FP32 && p->mode <= SCSFM_MODE_TF32X3, "%s: bad mode %d", who, p->mode);
     return SCSFM_OK;
 }
 
-// cp.async gather weight-gradient kernel: any stride / padding mode (whatever the TMA kernel does not take); border = 1:
-// the image-border ring pixels only
-static int wgrad_gather(const ScsfmConv& p, int border, cudaStream_t st) {
-    const bool split = p.in_lo != nullptr && p.dout_lo != nullptr;
-    if (split && p.Cout <= 16) return launch_wgrad_tc<32, true>(p, border, st);
-    if (split && p.Cout <= 32) return launch_wgrad_tc<64, true>(p, border, st);
-    if (split && p.Cout <= 64) return launch_wgrad_tc<128, true>(p, border, st);
-    if (p.Cout <= 16) return launch_wgrad_tc<16>(p, border, st);
-    if (p.Cout <= 32) return launch_wgrad_tc<32>(p, border, st);
-    if (p.Cout <= 64) return launch_wgrad_tc<64>(p, border, st);
-    return launch_wgrad_tc<128>(p, border, st);
+// Plans call *p of `pass` and validates it for the kernel picked; q receives the descriptor the kernels see (the low parts
+// the kernel does not read dropped: the tensor-core kernels count their passes from the low-part pointers).
+static int plan_call(const ScsfmConv* p, int pass, const char* who, ConvPlan& r, ScsfmConv& q) {
+    if (int rc = check_desc(p, who)) return rc;
+    r = conv_plan(*p, pass);
+    const bool simt = r.kernel == SCSFM_KERNEL_SIMT;
+    SCSFM_CHECK_ARG(pass == SCSFM_PASS_FWD ? p->in && p->w && p->out : pass == SCSFM_PASS_DGRAD ? p->dout && p->w && p->din : p->in && p->dout && p->dw,
+                    "%s: null tensor", who);
+    SCSFM_CHECK_ARG((long long)p->B * p->Hi * p->Wi * (long long)p->Cin < (1LL << 40), "%s: tensor too large", who);
+    SCSFM_CHECK_ARG(p->Ho == (p->Hi + 2 * p->pad - p->kh) / p->stride + 1 && p->Wo == (p->Wi + 2 * p->pad - p->kw) / p->stride + 1,
+                    "%s: output size does not match geometry", who);
+    if (pass == SCSFM_PASS_FWD) {
+        SCSFM_CHECK_ARG((p->bn_scale == nullptr) == (p->bn_shift == nullptr), "%s: bn_scale and bn_shift go together", who);
+        SCSFM_CHECK_ARG(p->bn_scale == nullptr || (p->bias == nullptr && p->bn_sums == nullptr),
+                        "%s: the eval-mode BatchNorm epilogue excludes bias and bn_sums", who);
+        if (simt) {
+            SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || (p->pad < p->Hi && p->pad < p->Wi && p->pad <= 1), "%s: reflect pad must be 1", who);
+        } else {
+            SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || p->pad == 1, "%s: reflect pad must be 1", who);
+            SCSFM_CHECK_ARG(p->bn_sums == nullptr || p->B % (p->bn_groups > 0 ? p->bn_groups : 1) == 0,
+                            "%s: batch not divisible by the number of BatchNorm groups", who);
+            SCSFM_CHECK_ARG(p->out_lo == nullptr || ((p->Cout & 3) == 0 && (reinterpret_cast<uintptr_t>(p->out_lo) & 15) == 0),
+                            "%s: out_lo needs Cout %% 4 == 0 and 16-byte alignment", who);
+            SCSFM_CHECK_ARG(((reinterpret_cast<uintptr_t>(p->bn_scale) | reinterpret_cast<uintptr_t>(p->bn_shift)) & 7) == 0,
+                            "%s: bn_scale / bn_shift must be 8-byte aligned", who);
+        }
+    }
+    if (pass == SCSFM_PASS_DGRAD && !simt)
+        SCSFM_CHECK_ARG(p->kh == p->kw && p->kh - 1 - p->pad >= 0, "%s: square kernels only", who);
+    if (pass == SCSFM_PASS_WGRAD && !simt) {
+        SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || p->pad == 1, "%s: reflect pad must be 1", who);
+        SCSFM_CHECK_ARG((long long)p->B * p->Ho * p->Wo < (1LL << 31), "%s: too many pixels", who);
+    }
+    const unsigned missing = r.reads & ~((p->in_lo ? SCSFM_PLAN_IN_LO : 0u) | (p->dout_lo ? SCSFM_PLAN_DOUT_LO : 0u) |
+                                         (p->w_lo ? SCSFM_PLAN_W_LO : 0u) | SCSFM_PLAN_FLIPPED);
+    SCSFM_CHECK_ARG(missing == 0, "%s: the kernel chosen for this call reads low parts that were not passed:%s%s%s (scsfm_conv_plan)", who,
+                    (missing & SCSFM_PLAN_W_LO) ? " w_lo" : "", (missing & SCSFM_PLAN_IN_LO) ? " in_lo" : "",
+                    (missing & SCSFM_PLAN_DOUT_LO) ? " dout_lo" : "");
+    q = *p;
+    if (!(r.reads & SCSFM_PLAN_IN_LO)) q.in_lo = nullptr;
+    if (!(r.reads & SCSFM_PLAN_DOUT_LO)) q.dout_lo = nullptr;
+    if (!(r.reads & SCSFM_PLAN_W_LO)) q.w_lo = nullptr;
+    return SCSFM_OK;
 }
 
-// dw [Cout,kh,kw,Cin] += dout^T x gather(in); dbias += column sums of dout.  Needs Cin % 4 == 0 and Cout % 4 == 0.
-extern "C" int scsfm_conv2d_wgrad_tc(const ScsfmConv* p, void* stream) {
-    SCSFM_CHECK_ARG(p != nullptr && p->in && p->dout && p->dw, "conv2d_wgrad_tc: null tensor");
-    SCSFM_CHECK_ARG(p->B > 0 && p->Hi > 0 && p->Wi > 0 && p->Cin > 0 && p->Cout > 0 && p->kh > 0 && p->kw > 0 && p->stride > 0 && p->pad >= 0,
-                    "conv2d_wgrad_tc: bad geometry");
-    SCSFM_CHECK_ARG((p->Cin & 3) == 0 && (p->Cout & 3) == 0, "conv2d_wgrad_tc: needs Cin %% 4 == 0 and Cout %% 4 == 0");
-    SCSFM_CHECK_ARG(p->pad_mode != PADMODE_REFLECT || p->pad == 1, "conv2d_wgrad_tc: reflect pad must be 1");
-    SCSFM_CHECK_ARG((long long)p->B * p->Ho * p->Wo < (1LL << 31), "conv2d_wgrad_tc: too many pixels");
-    SCSFM_CHECK_ARG(!p->split || (p->in_lo != nullptr && p->dout_lo != nullptr) || !conv_reads_lo(*p, SCSFM_PASS_WGRAD),
-                    "conv2d_wgrad_tc: the kernel chosen for this call reads in_lo and dout_lo, which were not passed (scsfm_conv_reads_lo)");
+extern "C" int scsfm_conv_plan(const ScsfmConv* p, int pass) {
+    SCSFM_CHECK_ARG(pass >= SCSFM_PASS_FWD && pass <= SCSFM_PASS_WGRAD, "conv_plan: bad pass %d", pass);
+    if (int rc = check_desc(p, "conv_plan")) return rc;
+    const ConvPlan r = conv_plan(*p, pass);
+    return r.kernel | (int)r.reads;
+}
+
+extern "C" int scsfm_conv2d_fwd(const ScsfmConv* p, void* stream) {
+    ConvPlan r;
+    ScsfmConv q;
+    if (int rc = plan_call(p, SCSFM_PASS_FWD, "conv2d_fwd", r, q)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    return r.kernel == SCSFM_KERNEL_SIMT ? launch_fwd_simt(q, st) : launch_route(q, plain_view(q), r, st);
+}
+
+// Tensor cores: the forward kernels on dout with the flipped weights in p->w / p->w_lo; p->din [B,Hi,Wi,Cin] (+ p->addend).
+extern "C" int scsfm_conv2d_dgrad(const ScsfmConv* p, void* stream) {
+    ConvPlan r;
+    ScsfmConv q;
+    if (int rc = plan_call(p, SCSFM_PASS_DGRAD, "conv2d_dgrad", r, q)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (r.kernel == SCSFM_KERNEL_SIMT) return launch_dgrad_simt(q, st);
+    ScsfmConv f;
+    TcView v;
+    bool covered_all = true;
+    for (int cls = 0; cls < 4; ++cls) {
+        dgrad_part(q, cls, f, v);
+        if (f.kh * f.kw == 0 && f.Ho > 0 && f.Wo > 0) covered_all = false;
+    }
+    if (!covered_all) {
+        // stride-2 parity classes without taps (1x1 stride 2): their gradient is the addend alone (or zero).  Enqueued
+        // before the sub-convolutions, which write the other classes' pixels of din.
+        const size_t bytes = (size_t)q.B * q.Hi * q.Wi * q.Cin * sizeof(float);
+        if (q.addend) SCSFM_CHECK_CUDA(cudaMemcpyAsync(q.din, q.addend, bytes, cudaMemcpyDeviceToDevice, st));
+        else SCSFM_CHECK_CUDA(cudaMemsetAsync(q.din, 0, bytes, st));
+    }
+    for (int cls = 0; cls < 4; ++cls) {
+        dgrad_part(q, cls, f, v);
+        if (f.kh * f.kw > 0 && f.Ho > 0 && f.Wo > 0)
+            if (int rc = launch_route(f, v, route_tc(f, v), st)) return rc;
+    }
+    return SCSFM_OK;
+}
+
+// dw [Cout,kh,kw,Cin] += dout^T x gather(in); dbias += column sums of dout.
+extern "C" int scsfm_conv2d_wgrad(const ScsfmConv* p, void* stream) {
+    ConvPlan r;
+    ScsfmConv q;
+    if (int rc = plan_call(p, SCSFM_PASS_WGRAD, "conv2d_wgrad", r, q)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    const int kernel = wgrad_kernel(*p);
-    if (kernel == 2) {
-        // reflection padding: the TMA kernel takes the interior with zero padding, the gather kernel the border ring
-        if ((rc = launch_conv_wgrad_tma(*p, st))) return rc;
-        rc = p->pad_mode == PADMODE_REFLECT ? wgrad_gather(*p, 1, st) : SCSFM_OK;
-    } else if (kernel == 3) {
-        rc = launch_conv_wgrad_thin(*p, st);
-    } else {
-        rc = wgrad_gather(*p, 0, st);
-    }
+    if (r.kernel == SCSFM_KERNEL_SIMT) rc = launch_wgrad_simt(q, st);
+    else if (r.kernel == SCSFM_KERNEL_THIN) rc = launch_conv_wgrad_thin(q, st);
+    else if (r.kernel == SCSFM_KERNEL_GATHER) rc = launch_wgrad_gather(q, r.stacked, 0, st);
+    else if ((rc = launch_conv_wgrad_tma(q, st)) == SCSFM_OK && r.kernel == SCSFM_KERNEL_TMA_RING)
+        rc = launch_wgrad_gather(q, r.stacked, 1, st);
     if (rc) return rc;
-    if (p->dbias) return launch_bias_grad(p->dout, p->B * p->Ho * p->Wo, p->Cout, p->dbias, st);
+    if (q.dbias) return launch_bias_grad(q.dout, q.B * q.Ho * q.Wo, q.Cout, q.dbias, st);
+    return SCSFM_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Flipped / transposed weights of the tensor-core data gradient: w [Co][kh][kw][Ci] -> the weights of the transposed
+// convolution, as operand kind `operand`.  Stride 1: wt[c][jy][jx][o] = w[o][kh-1-jy][kw-1-jx][c].  Stride 2: the four
+// parity classes back to back in the order (py,px) = (0,0),(0,1),(1,0),(1,1), class k as [Ci][jh][jw][Co] with
+// wt[c][jy][jx][o] = w[o][dy_max - 2 jy][dx_max - 2 jx][c]; Ci*kh*kw*Co floats in total either way.
+// A job owns ceil(Co/32) * ceil(Ci/32) * kh * kw blocks; each transposes one 32 (Cout) x 32 (Cin) tile of one tap through
+// shared memory: reads coalesced along Cin, writes coalesced along Cout.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int FLIP_ROW = 10;         // table row: {src, dst, Co, kh, kw, Ci, stride, pad, operand, first block}
+
+struct FlipJob {
+    const float* w;
+    float* wt;
+    int Co, kh, kw, Ci, stride, pad, operand;
+};
+
+// table == nullptr: the blocks of `job`; else the job of each block is the table row whose first block is the last one
+// <= blockIdx.x (row n: a sentinel holding the total).
+__global__ void __launch_bounds__(256)
+weight_flip_tiles_kernel(FlipJob job, const long long* __restrict__ table, int n) {
+    __shared__ int s_row;
+    __shared__ float tile[32][33];
+    long long t = blockIdx.x;
+    if (table != nullptr) {
+        if (threadIdx.x == 0) {
+            int lo = 0, hi = n;
+            while (hi - lo > 1) {
+                const int mid = (lo + hi) >> 1;
+                if (table[mid * FLIP_ROW + 9] <= t) lo = mid; else hi = mid;
+            }
+            s_row = lo;
+        }
+        __syncthreads();
+        const long long* e = table + s_row * FLIP_ROW;
+        job = FlipJob{reinterpret_cast<const float*>(e[0]), reinterpret_cast<float*>(e[1]), (int)e[2], (int)e[3], (int)e[4],
+                      (int)e[5], (int)e[6], (int)e[7], (int)e[8]};
+        t -= e[9];
+    }
+    const int Co = job.Co, kh = job.kh, kw = job.kw, Ci = job.Ci;
+    const int tco = (Co + 31) >> 5, tci = (Ci + 31) >> 5;
+    const int to = (int)(t % tco), tc = (int)(t / tco % tci);
+    int u = (int)(t / tco / tci);                 // tap of the block, counted over the classes in order
+    S2Class k{kh, kw, kh - 1, kw - 1};
+    size_t off = 0;                               // the class's offset in wt
+    if (job.stride == 2) {
+        for (int cls = 0;; ++cls) {
+            k = s2_class(kh, kw, job.pad, cls >> 1, cls & 1);
+            if (u < k.jh * k.jw) break;
+            u -= k.jh * k.jw;
+            off += (size_t)Co * k.jh * k.jw * Ci;
+        }
+    }
+    const int jy = u / k.jw, jx = u - jy * k.jw;
+    const int dy = k.dy_max - job.stride * jy, dx = k.dx_max - job.stride * jx;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int o = to * 32 + ty + 8 * i, c = tc * 32 + tx;
+        if (o < Co && c < Ci) tile[ty + 8 * i][tx] = tc_operand(__ldg(job.w + (((size_t)o * kh + dy) * kw + dx) * Ci + c), job.operand);
+    }
+    __syncthreads();
+    float* wt = job.wt + off;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int c = tc * 32 + ty + 8 * i, o = to * 32 + tx;
+        if (c < Ci && o < Co) wt[(((size_t)c * k.jh + jy) * k.jw + jx) * Co + o] = tile[tx][ty + 8 * i];
+    }
+}
+
+extern "C" int scsfm_weight_flip(const float* w, int Cout, int kh, int kw, int Cin, int stride, int pad, float* wt, int operand,
+                                 void* stream) {
+    SCSFM_CHECK_ARG(w && wt && Cout > 0 && kh > 0 && kw > 0 && Cin > 0 && (stride == 1 || stride == 2) && pad >= 0 && operand >= 0 &&
+                        operand <= 2, "weight_flip: bad arguments");
+    const long long blocks = (long long)((Cout + 31) / 32) * ((Cin + 31) / 32) * kh * kw;
+    SCSFM_CHECK_ARG(blocks < (1LL << 31), "weight_flip: too large");
+    weight_flip_tiles_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(FlipJob{w, wt, Cout, kh, kw, Cin, stride, pad, operand}, nullptr, 0);
+    SCSFM_CHECK_LAUNCH();
+    return SCSFM_OK;
+}
+
+extern "C" int scsfm_weight_flip_batched(const long long* table, int n_rows, int total_blocks, void* stream) {
+    SCSFM_CHECK_ARG(table != nullptr && n_rows > 0 && total_blocks > 0, "weight_flip_batched: bad arguments");
+    weight_flip_tiles_kernel<<<total_blocks, 256, 0, (cudaStream_t)stream>>>(FlipJob{}, table, n_rows);
+    SCSFM_CHECK_LAUNCH();
     return SCSFM_OK;
 }

@@ -93,4 +93,10 @@ int launch_conv_wgrad_tma(const ScsfmConv& p, cudaStream_t st);
 bool conv_wgrad_thin_eligible(const ScsfmConv& p);
 int launch_conv_wgrad_thin(const ScsfmConv& p, cudaStream_t st);
 
+// conv_simt.cu: exact-fp32 implicit GEMM on the CUDA cores (every shape); the weight gradient without the bias gradient
+int launch_fwd_simt(const ScsfmConv& p, cudaStream_t st);
+int launch_dgrad_simt(const ScsfmConv& p, cudaStream_t st);
+int launch_wgrad_simt(const ScsfmConv& p, cudaStream_t st);
+int launch_bias_grad(const float* dout, int rows, int C, float* dbias, cudaStream_t st);
+
 }  // namespace scsfm

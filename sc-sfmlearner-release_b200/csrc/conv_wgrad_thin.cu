@@ -207,12 +207,8 @@ static int launch_thin(const ScsfmConv& p, cudaStream_t st) {
     return SCSFM_OK;
 }
 
+// for the layers conv_wgrad_thin_eligible takes (conv_plan routes no others here)
 int launch_conv_wgrad_thin(const ScsfmConv& p, cudaStream_t st) {
-    if (!conv_wgrad_thin_eligible(p)) {
-        set_error("conv_wgrad_thin: needs a 3x3 stride-1 pad-1 layer with Cout = 16 and Cin in {16, 32} (got %d -> %d, k%d s%d p%d)", p.Cin,
-                  p.Cout, p.kh, p.stride, p.pad);
-        return SCSFM_ERR_ARG;
-    }
     if (p.Cin == 16) return launch_thin<16, 16, 32, 2>(p, st);
     return launch_thin<32, 16, 16, 1>(p, st);
 }

@@ -356,11 +356,11 @@ static int launch_wgrad_tma_bn(const ScsfmConv& p, cudaStream_t st) {
     return p.kw == 1 ? launch_wgrad_tma_cfg<BN, SPLIT, 1, 1>(p, st) : launch_wgrad_tma_cfg<BN, SPLIT, 3, 1>(p, st);
 }
 
-// Zero-padded pass over every pixel (reflection padding: interior pixels only, the caller adds the ring).  Split mode is
-// taken from p.split or from p.in_lo / p.dout_lo being set; the kernel recomputes the low parts rather than reading them.
+// Zero-padded pass over every pixel (reflection padding: interior pixels only, the caller adds the ring).  In tf32x3 mode
+// the kernel recomputes the low parts rather than reading them.
 // SCSFM_TUNE_BN(32 | 64) picks the Cout tile (default: 32 for Cout <= 32, else 64).
 int launch_conv_wgrad_tma(const ScsfmConv& p, cudaStream_t st) {
-    const bool split = p.split || (p.in_lo != nullptr && p.dout_lo != nullptr);
+    const bool split = p.mode == SCSFM_MODE_TF32X3;
     const unsigned bn_knob = (p.tune >> 8) & 7u;
     const bool bn32 = bn_knob == 2 || (bn_knob != 3 && p.Cout <= 32);
     if (bn32) return split ? launch_wgrad_tma_bn<32, true>(p, st) : launch_wgrad_tma_bn<32, false>(p, st);

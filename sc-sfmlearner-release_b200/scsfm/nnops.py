@@ -4,6 +4,8 @@ Tensors are torch CUDA tensors used as typed device buffers: activations NHWC `[
 contiguous, conv weights `[Cout,kh,kw,Cin]`.  Every function enqueues on torch's current stream.
 """
 import ctypes
+import operator
+import struct
 
 import torch
 
@@ -42,9 +44,17 @@ class Conv(ctypes.Structure):
                 [(n, ctypes.c_void_p) for n in ("in_lo", "w_lo", "dout_lo")] +
                 [("tune", ctypes.c_uint), ("debug", ctypes.c_void_p)] +
                 [(n, ctypes.c_void_p) for n in ("bn_scale", "bn_shift", "out_lo")] +
-                [("split", ctypes.c_int)])
+                [("mode", ctypes.c_int)])
 
-PASS_FWD, PASS_DGRAD, PASS_WGRAD = 0, 1, 2        # SCSFM_PASS_* of scsfm_conv_reads_lo
+PASS_FWD, PASS_DGRAD, PASS_WGRAD = 0, 1, 2        # SCSFM_PASS_*
+# scsfm_conv_plan: SCSFM_KERNEL_* in the low byte, SCSFM_PLAN_* flags above it
+KERNEL_SIMT, KERNEL_GATHER, KERNEL_TMA, KERNEL_TMA_RING, KERNEL_STEM, KERNEL_THIN = range(6)
+PLAN_IN_LO, PLAN_DOUT_LO, PLAN_W_LO, PLAN_FLIPPED = 0x100, 0x200, 0x400, 0x800
+
+# the plan-cache key of a descriptor: its integer fields and which of its pointers are null
+_DESC = struct.Struct("@" + "".join("P" if t is ctypes.c_void_p else "I" if t is ctypes.c_uint else "i" for _, t in Conv._fields_))
+_DESC_INTS = operator.itemgetter(*[i for i, (_, t) in enumerate(Conv._fields_) if t is not ctypes.c_void_p])
+_DESC_PTRS = operator.itemgetter(*[i for i, (_, t) in enumerate(Conv._fields_) if t is ctypes.c_void_p])
 
 
 _bound = False
@@ -56,14 +66,12 @@ def _lib():
     if not _bound:
         I, P, LL, F = ctypes.c_int, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_float
         CP = ctypes.POINTER(Conv)
-        for name in ("scsfm_conv2d_fwd_simt", "scsfm_conv2d_dgrad_simt", "scsfm_conv2d_wgrad_simt",
-                     "scsfm_conv2d_fwd_tc", "scsfm_conv2d_dgrad_tc", "scsfm_conv2d_wgrad_tc"):
+        for name in ("scsfm_conv2d_fwd", "scsfm_conv2d_dgrad", "scsfm_conv2d_wgrad"):
             getattr(lib, name).argtypes = [CP, P]
-        lib.scsfm_conv_reads_lo.argtypes = [CP, I]
+        lib.scsfm_conv_plan.argtypes = [CP, I]
         lib.scsfm_round_tf32.argtypes = [P, P, LL, P]
         lib.scsfm_split_tf32.argtypes = [P, P, LL, P]
-        lib.scsfm_weight_flip.argtypes = [P, I, I, I, I, P, I, P]
-        lib.scsfm_weight_flip_s2.argtypes = [P, I, I, I, I, I, P, I, P]
+        lib.scsfm_weight_flip.argtypes = [P, I, I, I, I, I, I, P, I, P]
         lib.scsfm_weight_flip_batched.argtypes = [P, I, I, P]
         lib.scsfm_nchw_to_nhwc.argtypes = [P, P, I, I, I, I, P, P]
         lib.scsfm_nhwc_to_nchw.argtypes = [P, I, I, I, I, P, P]
@@ -123,51 +131,16 @@ def aligned64(n):
     return (n + 63) // 64 * 64
 
 
-def tc_supported(kind, Cin, Cout, kh, stride):
-    """Shapes the tensor-core kernels take; everything else runs the CUDA-core kernel."""
-    if kind == "fwd":
-        return Cin % 4 == 0 and Cout >= 16
-    if kind == "dgrad":                      # forward kernel on dout: its "Cin" is Cout, its "Cout" is Cin
-        return stride in (1, 2) and Cout % 4 == 0 and Cin >= 16
-    if kind == "wgrad":
-        return Cin % 4 == 0 and Cout % 4 == 0 and Cout >= 16
-    return False
-
-
-def _s2_classes(kh, kw, pad):
-    """Parity classes (py, px) of a stride-2 data gradient: taps kept = jh x jw starting at (dy_max, dx_max), step 2."""
-    out = []
-    for py in range(2):
-        for px in range(2):
-            dy_max, dx_max = kh - 1, kw - 1
-            while dy_max >= 0 and ((py + pad - dy_max) & 1):
-                dy_max -= 1
-            while dx_max >= 0 and ((px + pad - dx_max) & 1):
-                dx_max -= 1
-            jh = 0 if dy_max < 0 else dy_max // 2 + 1
-            jw = 0 if dx_max < 0 else dx_max // 2 + 1
-            out.append((jh, jw, dy_max, dx_max))
-    return out
-
-
 class FlipTable:
-    """Device job table of every cached flip of one context (one network's operand arena)."""
+    """Device job table of scsfm_weight_flip_batched: every cached flip of one context (one network's operand arena)."""
 
     def __init__(self, cache, device):
-        self.keys = sorted(cache)
         rows, blk = [], 0
-        for key in self.keys:
-            ptr, (Cout, kh, kw, Cin), stride, pad, operand = key
-            dst = cache[key][1].data_ptr()
-            jobs = [(kh, kw, kh - 1, kw - 1)] if stride == 1 else _s2_classes(kh, kw, pad)
-            for (jh, jw, dy_max, dx_max) in jobs:
-                total = Cout * jh * jw * Cin
-                if total > 0:
-                    rows.append([ptr, dst, Cout, kh, kw, Cin, jh, jw, dy_max, dx_max, stride | (operand << 8), blk])
-                    blk += ((Cout + 31) // 32) * ((Cin + 31) // 32) * jh * jw      # one block per 32x32 tile of one tap
-                dst += 4 * total
-        self.n_rows, self.total_blocks, self.bytes = len(rows), blk, 8.0 * sum(cache[k][1].numel() for k in self.keys)
-        rows.append([0] * 11 + [blk])
+        for (ptr, (Cout, kh, kw, Cin), stride, pad, operand), (_, wt) in sorted(cache.items()):
+            rows.append([ptr, wt.data_ptr(), Cout, kh, kw, Cin, stride, pad, operand, blk])
+            blk += ((Cout + 31) // 32) * ((Cin + 31) // 32) * kh * kw      # one block per 32x32 tile of one tap
+        self.n_rows, self.total_blocks, self.bytes = len(rows), blk, 8.0 * sum(wt.numel() for _, wt in cache.values())
+        rows.append([0] * 9 + [blk])
         self.table = torch.tensor(rows, dtype=torch.int64).to(device)
 
 
@@ -204,6 +177,7 @@ class ConvCtx:
         self.tune = 0                 # ScsfmConv.tune of every call made through this context (see tune())
         self.debug = None             # ScsfmConv.debug: uint64 tensor [8 * SMs] of per-role cycle counters, or None
         self._flips = {}              # (source pointer, shape, stride, pad, operand) -> (source tensor, flipped weights)
+        self._plans = {}              # (pass, descriptor key) -> scsfm_conv_plan
         self._table = None
         self.sums_pool = None         # fp64 scratch of the fused BatchNorm sums of this network's calls (scsfm.nets._pool)
         # Optional side stream for the weight gradients: a layer's wgrad is off the backward's critical path (only the
@@ -230,28 +204,39 @@ class ConvCtx:
         """SCSFM_OPERAND_* of tensors prepared for the tensor cores (padded stem input / weights)."""
         return OPERAND_TF32 if self.mode == "tf32" else OPERAND_RAW
 
-    def _use_tc(self, kind, Cin, Cout, kh, stride):
-        return self.tc and tc_supported(kind, Cin, Cout, kh, stride)
-
     def _finish(self, d):
         d.tune = self.tune
         d.debug = self.debug.data_ptr() if self.debug is not None else None
+        d.mode = MODES.index(self.mode)
 
-    def _reads_lo(self, d, pass_):
-        """tf32x3: does the kernel picked for descriptor d (its tune included) read the low parts of its activation
-        operands?  The stem forward and the TMA / thin-layer weight gradients compute them themselves."""
-        rc = _lib().scsfm_conv_reads_lo(ctypes.byref(d), pass_)
-        L.check(0 if rc >= 0 else rc, "scsfm_conv_reads_lo")
-        return rc == 1
+    def plan(self, d, pass_):
+        """scsfm_conv_plan of descriptor d (after _finish): the kernel (KERNEL_*, low byte) and the PLAN_* operands it reads.
+        Memoised on d's integer fields and which of its pointers are null, so that an eager call costs no query."""
+        v = _DESC.unpack_from(d)
+        key = (pass_, _DESC_INTS(v), tuple(map(bool, _DESC_PTRS(v))))
+        plan = self._plans.get(key)
+        if plan is None:
+            plan = _lib().scsfm_conv_plan(ctypes.byref(d), pass_)
+            L.check(0 if plan >= 0 else plan, "scsfm_conv_plan")
+            self._plans[key] = plan
+        return plan
+
+    def _use_tc(self, kind, Cin, Cout, kh, stride):
+        """Whether a "fwd" / "dgrad" / "wgrad" convolution of these channels, kernel size and stride runs on the tensor cores:
+        the plan of a descriptor of that shape (the plan takes the CUDA cores or not from these fields and the mode alone)."""
+        d = conv_desc((1, 2 * kh, 2 * kh, Cin), (Cout, kh, kh, Cin), stride, 0, PAD_ZERO, ACT_NONE)
+        self._finish(d)
+        return self.tc and self.plan(d, {"fwd": PASS_FWD, "dgrad": PASS_DGRAD, "wgrad": PASS_WGRAD}[kind]) & 0xff != KERNEL_SIMT
+
+    def _family(self, name, plan):
+        """Profiling family of a call: name + _tc for the tensor-core modes' kernels, _simt for the CUDA-core kernel."""
+        return name + ("_tc" if self.tc and plan & 0xff != KERNEL_SIMT else "_simt")
 
     def wgrad_reads_lo(self, x_shape, w_shape, stride, pad, pad_mode=PAD_ZERO):
-        """Whether conv_wgrad of this shape will read lo(x) and lo(dout): False outside tf32x3, and where its kernel
-        computes them itself (a producer of dout can then skip writing lo(dout))."""
-        if not (self.split and self._use_tc("wgrad", x_shape[-1], w_shape[0], w_shape[1], stride)):
-            return False
+        """Whether conv_wgrad of this shape will read lo(x) and lo(dout) (a producer of dout can skip writing lo(dout) if not)."""
         d = conv_desc(tuple(x_shape), tuple(w_shape), stride, pad, pad_mode, ACT_NONE)
         self._finish(d)
-        return self._reads_lo(d, PASS_WGRAD)
+        return bool(self.plan(d, PASS_WGRAD) & PLAN_DOUT_LO)
 
     # -- flipped weights of the data gradients -----------------------------------------------------------
     def flipped_weights(self, w, stride, pad, operand):
@@ -263,12 +248,8 @@ class ConvCtx:
         if hit is None:
             Cout, kh, kw, Cin = w.shape
             wt = empty((Cin, kh, kw, Cout), w)
-            if stride == 1:
-                L.launch(_lib().scsfm_weight_flip, "scsfm_weight_flip", "weight_flip", 1, 8.0 * w.numel(), L.ptr(w), Cout, kh, kw, Cin,
-                         L.ptr(wt), operand, L.stream())
-            else:
-                L.launch(_lib().scsfm_weight_flip_s2, "scsfm_weight_flip_s2", "weight_flip", 4, 8.0 * w.numel(), L.ptr(w), Cout, kh, kw,
-                         Cin, pad, L.ptr(wt), operand, L.stream())
+            L.launch(_lib().scsfm_weight_flip, "scsfm_weight_flip", "weight_flip", 1, 8.0 * w.numel(), L.ptr(w), Cout, kh, kw, Cin,
+                     stride, pad, L.ptr(wt), operand, L.stream())
             hit = self._flips[key] = (w, wt)
             self._table = None
         return hit[1]
@@ -307,17 +288,16 @@ class ConvCtx:
         if with_lo:
             y._scsfm_lo = empty(y.shape, y)
             d.out_lo = y._scsfm_lo.data_ptr()
-        tc = self._use_tc("fwd", d.Cin, d.Cout, d.kh, stride)
-        if tc and self.split:
+        self._finish(d)
+        plan = self.plan(d, PASS_FWD)
+        if plan & PLAN_W_LO:
             if w_lo is None:
                 raise RuntimeError("tf32x3 convolution called without the low part of its weights")
-            d.w_lo, d.split = w_lo.data_ptr(), 1
-        self._finish(d)
-        if tc and self.split and self._reads_lo(d, PASS_FWD):
+            d.w_lo = w_lo.data_ptr()
+        if plan & PLAN_IN_LO:
             d.in_lo = lo_of(x).data_ptr()
         _tag(d)
-        fn = lib.scsfm_conv2d_fwd_tc if tc else lib.scsfm_conv2d_fwd_simt
-        L.launch(fn, "scsfm_conv2d_fwd", "conv_fwd_tc" if tc else "conv_fwd_simt", 1, _flops(d), ctypes.byref(d), L.stream())
+        L.launch(lib.scsfm_conv2d_fwd, "scsfm_conv2d_fwd", self._family("conv_fwd", plan), 1, _flops(d), ctypes.byref(d), L.stream())
         return y
 
     def conv_dgrad(self, dout, w, x_shape, stride=1, pad=0, addend=None, padded_input=False, w_src=None):
@@ -332,19 +312,18 @@ class ConvCtx:
         assert (d.Ho, d.Wo, d.Cout) == tuple(dout.shape[1:]), (d.Ho, d.Wo, d.Cout, dout.shape)
         din = empty((B, Hi, Wi, Cin), dout)
         d.dout, d.din, d.addend = dout.data_ptr(), din.data_ptr(), addend.data_ptr() if addend is not None else None
-        tc = self._use_tc("dgrad", d.Cin, d.Cout, d.kh, stride)
-        if tc:
-            if self.split:
-                src = w if w_src is None else w_src
-                d.w = self.flipped_weights(src, stride, pad, OPERAND_RAW).data_ptr()
-                d.w_lo = self.flipped_weights(src, stride, pad, OPERAND_LO).data_ptr()
-                d.dout_lo, d.split = lo_of(dout).data_ptr(), 1
-            else:
-                d.w = self.flipped_weights(w, stride, pad, OPERAND_TF32).data_ptr()
         self._finish(d)
+        plan = self.plan(d, PASS_DGRAD)
+        if plan & PLAN_W_LO:                # flipped raw and low parts, both derived from the raw weights
+            src = w if w_src is None else w_src
+            d.w = self.flipped_weights(src, stride, pad, OPERAND_RAW).data_ptr()
+            d.w_lo = self.flipped_weights(src, stride, pad, OPERAND_LO).data_ptr()
+        elif plan & PLAN_FLIPPED:
+            d.w = self.flipped_weights(w, stride, pad, OPERAND_TF32).data_ptr()
+        if plan & PLAN_DOUT_LO:
+            d.dout_lo = lo_of(dout).data_ptr()
         _tag(d)
-        fn = lib.scsfm_conv2d_dgrad_tc if tc else lib.scsfm_conv2d_dgrad_simt
-        L.launch(fn, "scsfm_conv2d_dgrad", "conv_dgrad_tc" if tc else "conv_dgrad_simt", 1, _flops(d), ctypes.byref(d), L.stream())
+        L.launch(lib.scsfm_conv2d_dgrad, "scsfm_conv2d_dgrad", self._family("conv_dgrad", plan), 1, _flops(d), ctypes.byref(d), L.stream())
         return din
 
     def conv_wgrad(self, x, dout, dw, dbias=None, stride=1, pad=0, pad_mode=PAD_ZERO):
@@ -355,20 +334,17 @@ class ConvCtx:
         assert (d.Ho, d.Wo, d.Cout) == tuple(dout.shape[1:])
         d.inp, d.dout, d.dw, d.dbias = x.data_ptr(), dout.data_ptr(), dw.data_ptr(), dbias.data_ptr() if dbias is not None else None
         d.w = None
-        tc = self._use_tc("wgrad", d.Cin, d.Cout, d.kh, stride)
-        keep = [x, dout]
         self._finish(d)
-        if tc and self.split:
-            d.split = 1
-            if self._reads_lo(d, PASS_WGRAD):
-                x_lo, dout_lo = lo_of(x), lo_of(dout)      # (computed on the CURRENT stream: the data gradient reads them too)
-                d.in_lo, d.dout_lo = x_lo.data_ptr(), dout_lo.data_ptr()
-                keep += [x_lo, dout_lo]
+        plan = self.plan(d, PASS_WGRAD)
+        keep = [x, dout]
+        if plan & PLAN_IN_LO:                # (with PLAN_DOUT_LO: the weight-gradient kernels read both or neither)
+            x_lo, dout_lo = lo_of(x), lo_of(dout)      # (computed on the CURRENT stream: the data gradient reads them too)
+            d.in_lo, d.dout_lo = x_lo.data_ptr(), dout_lo.data_ptr()
+            keep += [x_lo, dout_lo]
         _tag(d)
-        fn = lib.scsfm_conv2d_wgrad_tc if tc else lib.scsfm_conv2d_wgrad_simt
         with self.on_wgrad_stream(keep):
-            L.launch(fn, "scsfm_conv2d_wgrad", "conv_wgrad_tc" if tc else "conv_wgrad_simt", 2 if dbias is not None else 1, _flops(d),
-                     ctypes.byref(d), L.stream())
+            L.launch(lib.scsfm_conv2d_wgrad, "scsfm_conv2d_wgrad", self._family("conv_wgrad", plan), 2 if dbias is not None else 1,
+                     _flops(d), ctypes.byref(d), L.stream())
 
     def on_wgrad_stream(self, keep=()):
         """Context: the weight-gradient side stream, ordered after the work already enqueued on the current stream (no-op

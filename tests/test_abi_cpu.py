@@ -60,18 +60,18 @@ def test_host_side_helpers():
         lib.dev_f32(torch.zeros(1, 3, 8, 8), "x")
 
 
-def test_network_entry_points_reject_bad_arguments_without_a_gpu():
+def test_network_operators_reject_bad_arguments_without_a_gpu():
     """Host-side checks of the network operators added for the tensor-core path (no launch happens on an error)."""
     from scsfm import lib
     from scsfm import nnops as O
     L = O._lib()
     n0 = lib.launch_count()
-    assert L.scsfm_weight_flip(None, 8, 3, 3, 8, None, 5, None) == -1 and b"weight_flip" in L.scsfm_last_error()
+    assert L.scsfm_weight_flip(None, 8, 3, 3, 8, 1, 1, None, 5, None) == -1 and b"weight_flip" in L.scsfm_last_error()
     assert L.scsfm_split_tf32(None, None, 16, None) == -1 and b"split_tf32" in L.scsfm_last_error()
     assert L.scsfm_adam_step(None, None, None, None, 0, 1e-4, 0.9, 0.999, 1e-8, 0.0, 1, None, None, 0, None) == -1
     assert L.scsfm_weight_flip_batched(None, 1, 1, None) == -1
     assert L.scsfm_head_conv_dgrad(None, None, None, 1, 8, 8, 16, None) == -1
-    assert L.scsfm_conv2d_fwd_tc(None, None) == -1
+    assert L.scsfm_conv2d_fwd(None, None) == -1
     assert lib.launch_count() == n0          # nothing was launched
 
 
@@ -85,8 +85,8 @@ def test_conv_descriptor_matches_the_c_struct_and_tune_word():
 #include <stddef.h>
 #include "scsfm.h"
 int main(void) {
-    printf("%zu %zu %zu %zu %zu %zu\n", sizeof(ScsfmConv), offsetof(ScsfmConv, bn_groups), offsetof(ScsfmConv, act),
-           offsetof(ScsfmConv, in_lo), offsetof(ScsfmConv, tune), offsetof(ScsfmConv, debug));
+    printf("%zu %zu %zu %zu %zu %zu %zu\n", sizeof(ScsfmConv), offsetof(ScsfmConv, bn_groups), offsetof(ScsfmConv, act),
+           offsetof(ScsfmConv, in_lo), offsetof(ScsfmConv, tune), offsetof(ScsfmConv, debug), offsetof(ScsfmConv, mode));
     printf("%u %u\n", SCSFM_TUNE_NO_TMA | SCSFM_TUNE_MT(2) | SCSFM_TUNE_TW(4) | SCSFM_TUNE_BN(64) | SCSFM_TUNE_WGRAD(2),
            SCSFM_TUNE_MT(1) | SCSFM_TUNE_TW(3) | SCSFM_TUNE_BN(128));
     return 0;
@@ -96,8 +96,9 @@ int main(void) {
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), os.path.join(d, "t.c"), "-o", os.path.join(d, "t")])
         out = subprocess.check_output([os.path.join(d, "t")], text=True).split()
     C = O.Conv
-    assert [int(v) for v in out[:6]] == [ctypes.sizeof(C), C.bn_groups.offset, C.act.offset, C.in_lo.offset, C.tune.offset, C.debug.offset]
-    assert int(out[6]) == O.tune(no_tma=1, mt=2, tw_log2=4, bn=64, wgrad=2) and int(out[7]) == O.tune(mt=1, tw_log2=3, bn=128)
+    assert [int(v) for v in out[:7]] == [ctypes.sizeof(C), C.bn_groups.offset, C.act.offset, C.in_lo.offset, C.tune.offset, C.debug.offset,
+                                         C.mode.offset]
+    assert int(out[7]) == O.tune(no_tma=1, mt=2, tw_log2=4, bn=64, wgrad=2) and int(out[8]) == O.tune(mt=1, tw_log2=3, bn=128)
 
 
 def test_conv_context_is_per_network_state():
@@ -113,23 +114,3 @@ def test_conv_context_is_per_network_state():
         a.set_conv_mode("bf16")
     assert not hasattr(O, "CONFIG")
 
-
-def test_stride2_parity_classes_partition_the_taps():
-    """A stride-2 data gradient runs as four parity-class sub-convolutions: every tap of the kernel must belong to exactly
-    one class (the tap rows dy_max, dy_max-2, ... of class py are those with (py + pad - dy) even)."""
-    from scsfm import nnops as O
-    for k in (1, 3, 7):
-        for pad in (0, 1, 3):
-            classes = O._s2_classes(k, k, pad)
-            assert len(classes) == 4
-            owners = {}
-            for cls, (jh, jw, dy_max, dx_max) in enumerate(classes):
-                py, px = divmod(cls, 2)
-                for jy in range(jh):
-                    for jx in range(jw):
-                        dy, dx = dy_max - 2 * jy, dx_max - 2 * jx
-                        assert 0 <= dy < k and 0 <= dx < k
-                        assert (py + pad - dy) % 2 == 0 and (px + pad - dx) % 2 == 0
-                        assert (dy, dx) not in owners
-                        owners[(dy, dx)] = cls
-            assert len(owners) == k * k

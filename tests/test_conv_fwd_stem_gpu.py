@@ -2,7 +2,7 @@
 wgmma from registers, lo(x) computed from it) against F.conv2d in fp64, with 4 and 8 (padded) input channels.  Each case
 runs three ways: the automatic choice, a forced TMA tile knob (which the stems ignore) and the cp.async gather kernel
 (SCSFM_TUNE_NO_TMA).  Also: BatchNorm sums over several groups, the fused eval-mode BatchNorm, the low part of the output,
-scsfm_conv_reads_lo, and that a tf32x3 training step no longer splits the stem inputs.  Needs a GPU."""
+the input low part in scsfm_conv_plan, and that a tf32x3 training step no longer splits the stem inputs.  Needs a GPU."""
 import ctypes
 
 import pytest
@@ -130,7 +130,7 @@ def test_stem_fwd_fused_bn(cin, mode):
         assert _bits(zf._scsfm_lo, O.split_tf32(zf)), name
 
 
-def test_stem_fwd_reads_no_input_low_part():
+def test_stem_fwd_plan_reads_no_input_low_part():
     """The stem kernel runs in split mode with in_lo NULL; the gather kernel forced by tune reads in_lo, so the same call
     is refused with an argument error (never a device fault)."""
     O = _O()
@@ -141,9 +141,9 @@ def test_stem_fwd_reads_no_input_low_part():
     for knobs, reads in ((dict(), 0), (dict(no_tma=1), 1)):
         d = O.conv_desc(x.shape, w, 2, 3, O.PAD_ZERO, O.ACT_NONE)
         y = torch.zeros(2, 19, 23, 64, device=DEV)
-        d.inp, d.out, d.w_lo, d.split, d.tune = x.data_ptr(), y.data_ptr(), w_lo.data_ptr(), 1, O.tune(**knobs)
-        assert lib.scsfm_conv_reads_lo(ctypes.byref(d), O.PASS_FWD) == reads
-        rc = lib.scsfm_conv2d_fwd_tc(ctypes.byref(d), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        d.inp, d.out, d.w_lo, d.mode, d.tune = x.data_ptr(), y.data_ptr(), w_lo.data_ptr(), O.MODES.index("tf32x3"), O.tune(**knobs)
+        assert (lib.scsfm_conv_plan(ctypes.byref(d), O.PASS_FWD) & O.PLAN_IN_LO) == (O.PLAN_IN_LO if reads else 0)
+        rc = lib.scsfm_conv2d_fwd(ctypes.byref(d), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
         torch.cuda.synchronize()
         if reads:
             assert rc == -1 and b"in_lo" in lib.scsfm_last_error()

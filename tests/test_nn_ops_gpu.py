@@ -130,6 +130,45 @@ def test_round_and_split_tf32_bitwise(n):
     assert (np.abs(hi + _np(lo).astype(np.float64) - x) <= 2.0 ** -21 * np.abs(x))[big].all()
 
 
+def _flip_ref(w, stride, pad, operand):
+    """Flipped weights of the data gradient restated: w [Cout,kh,kw,Cin] -> [Cin,kh,kw,Cout] with reversed taps at stride 1;
+    at stride 2 the four output-parity classes (py, px) back to back, class (py, px) holding the kernel rows dy with
+    py + pad - dy even (and columns likewise), each from the last one down, in the same layout."""
+    w = {0: rna_tf32, 1: lambda a: a, 2: lo_tf32}[operand](w)
+    kh, kw = w.shape[1:3]
+    if stride == 1:
+        return np.ascontiguousarray(w[:, ::-1, ::-1].transpose(3, 1, 2, 0)).ravel()
+    parts = []
+    for py in range(2):
+        for px in range(2):
+            rows = [dy for dy in range(kh - 1, -1, -1) if (py + pad - dy) % 2 == 0]
+            cols = [dx for dx in range(kw - 1, -1, -1) if (px + pad - dx) % 2 == 0]
+            parts.append(w[:, rows][:, :, cols].transpose(3, 1, 2, 0).ravel())
+    return np.concatenate(parts)
+
+
+def test_weight_flips_match_their_restatement():
+    """Every flipped layout bit for bit: strides 1 and 2, k = 1, 3, 7, pad 0, 1, 3, the three operand kinds, from the first
+    flip (one launch per weight) and from the batched refresh of all of them (one launch) after the weights changed.
+    Cout and Cin are not multiples of the 32 x 32 tiles."""
+    O = _ops()
+    cx = O.ConvCtx("tf32x3")
+    g = torch.Generator().manual_seed(3)
+    cases = [(s, k, pad, op) for s in (1, 2) for k in (1, 3, 7) for pad in (0, 1, 3) for op in (0, 1, 2)]
+    ws = {k: torch.randn(40, k, k, 36, generator=g).to(DEV) for k in (1, 3, 7)}
+    got = {c: cx.flipped_weights(ws[c[1]], c[0], c[2], c[3]) for c in cases}
+    for rnd in range(2):
+        torch.cuda.synchronize()
+        for (s, k, pad, op), wt in got.items():
+            want = _flip_ref(ws[k].cpu().numpy(), s, pad, op)
+            assert wt.shape == (36, k, k, 40)
+            _same_bits(wt.flatten(), want, "flip s%d k%d pad%d operand %d %s" % (s, k, pad, op, ("first", "refresh")[rnd]))
+        for w in ws.values():
+            w.copy_(torch.randn(w.shape, generator=g))
+        cx.refresh_flips(DEV)
+    assert len(cx._flips) == len(cases) and cx._table.n_rows == len(cases)
+
+
 def test_split_tf32_refuses_unaligned_buffers():
     """split_tf32 reads and writes float4: a buffer offset by one float is refused before any launch."""
     from scsfm import lib as L

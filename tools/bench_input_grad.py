@@ -9,7 +9,7 @@ Arms (images/s for DispResNet, pairs/s for PoseResNet; forward + backward of one
   eval_params        eval mode, parameter gradients (frozen BatchNorm statistics)
   eval_input_only    eval mode, every parameter frozen, gradient of the input image(s) only
   cudnn_*            the same three on stock PyTorch / cuDNN (oracle.nets; TF32 convolutions on in mode tf32, off otherwise)
-Stem: scsfm_stem_dgrad against conv2d_dgrad_simt + nhwc_to_nchw on the same dy (ms per call, CUDA events).
+Stem: scsfm_stem_dgrad against the CUDA-core conv2d_dgrad + nhwc_to_nchw on the same dy (ms per call, CUDA events).
 """
 import argparse
 import json
