@@ -326,12 +326,16 @@ int scsfm_maxpool_fwd(const float* x, int B, int H, int W, int C, float* y, unsi
 int scsfm_maxpool_bwd(const float* dy, const unsigned char* idx, int B, int H, int W, int C, float* dx, int accumulate,
                       void* stream);
 
-/* nearest x2 upsample of `lo` concatenated with `skip` on channels (DispResNet.py:92-95). skip may be NULL. */
+/* nearest x2 upsample of `lo` [B,H/2,W/2,C1] concatenated with `skip` [B,H,W,C2] on channels into out [B,H,W,C1+C2]
+ * (DispResNet.py:92-95). skip may be NULL.  H and W are even, and skip must be exactly [B,H,W,C2]: it is read at those
+ * strides and the library cannot see its real shape (a skip of another plane is read out of place and past its end;
+ * scsfm/nnops.py upcat_fwd refuses one).  DispResNet's skips have that shape for H, W = 0 or 31 mod 32, at least 63. */
 int scsfm_upcat_fwd(const float* lo, const float* skip, int B, int H, int W, int C1, int C2, float* out, void* stream);
 /* Backward of ReflectionPad2d(1) (+ optional upsample/concat): dpad is the gradient w.r.t. the padded tensor
  * [B,H+2,W+2,C1+C2].  d_lo [B,H/2,W/2,C1] (overwritten; multiplied by act'(lo_act) if act != NONE),
  * d_skip [B,H,W,C2] overwritten, or NULL when its gradient is not wanted (not computed).  With C2 == 0 and upsample == 0: plain fold into d_lo [B,H,W,C1]
- * (accumulate flag honoured, act applied after accumulation). */
+ * (accumulate flag honoured, act applied after accumulation).  With upsample, H and W are even and d_lo / lo_act are
+ * exactly [B,H/2,W/2,C1], as for scsfm_upcat_fwd (scsfm/nnops.py fold_upcat refuses other shapes). */
 int scsfm_fold_bwd(const float* dpad, int B, int H, int W, int C1, int C2, int upsample, float* d_lo,
                    const float* lo_act, int act, int accumulate, float* d_skip, void* stream);
 

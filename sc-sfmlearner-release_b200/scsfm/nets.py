@@ -765,6 +765,37 @@ def encoder_backward(cx, enc, rec, d_feats, plan):
 # ------------------------------------------------------------------------------------------------
 # networks
 # ------------------------------------------------------------------------------------------------
+def _disp_side_ok(n, training_step):
+    """Whether DispResNet takes an image side of n pixels.  Its encoder planes are ceil(n/2), ceil(n/4), ..., ceil(n/32), and
+    each decoder stage concatenates its x2 upsampled plane with the encoder plane one level up, so ceil(n/2) is a multiple
+    of 16; the first stage reflection-pads the ceil(n/32) plane by one, which needs 2 pixels: n = 0 or 31 mod 32, n >= 63,
+    the sizes the reference's module runs on.  A training step also needs the disparity (2 ceil(n/2)) at the image's size:
+    n a multiple of 32, n >= 64."""
+    if training_step:
+        return n % 32 == 0 and n >= 64
+    h = (n + 1) // 2
+    return h % 16 == 0 and h >= 32
+
+
+def check_image_size(H, W, training_step=False):
+    """Raises ValueError, naming the nearest accepted sizes, unless DispResNet takes an H x W image (its disparity is then
+    2 ceil(H/2) x 2 ceil(W/2)); training_step: unless a training step takes it (_disp_side_ok)."""
+    if _disp_side_ok(H, training_step) and _disp_side_ok(W, training_step):
+        return
+
+    def near(n):
+        if _disp_side_ok(n, training_step):
+            return [n]
+        lo = next((m for m in range(n - 1, 0, -1) if _disp_side_ok(m, training_step)), None)
+        hi = next(m for m in range(n + 1, n + 65) if _disp_side_ok(m, training_step))
+        return [m for m in (lo, hi) if m is not None]
+    sizes = sorted(((h, w) for h in near(H) for w in near(W)), key=lambda s: (abs(s[0] - H) + abs(s[1] - W), s))
+    rule = ("a training step takes H and W that are multiples of 32, at least 64" if training_step else
+            "DispResNet takes H and W = 0 or 31 mod 32, at least 63")
+    raise ValueError("image size %dx%d: %s (nearest accepted sizes: %s)"
+                     % (H, W, rule, ", ".join("%dx%d" % s for s in sizes[:4])))
+
+
 class DispResNet(ArenaNet):
     """models.DispResNet(num_layers=18, pretrained=True) (reference DispResNet.py:104-121)."""
 
@@ -777,6 +808,7 @@ class DispResNet(ArenaNet):
         pass
 
     def forward(self, x):
+        check_image_size(x.shape[-2], x.shape[-1])
         outs = self._call((x,))
         return list(outs) if self.training else outs[0]
 
@@ -785,6 +817,8 @@ class DispResNet(ArenaNet):
         returns one output per image, each exactly what `self(image)` would return.  The calls are stacked on
         the batch axis (more rows per GEMM, 1/len(images) of the kernel launches) while BatchNorm statistics
         and running-stat updates stay per call, in list order (train.py:427-434 semantics)."""
+        for x in images:
+            check_image_size(x.shape[-2], x.shape[-1])
         per = self._call((torch.cat(list(images), 0),), len(images))
         return per if self.training else [p[0] for p in per]
 

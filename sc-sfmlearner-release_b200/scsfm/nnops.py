@@ -530,7 +530,12 @@ def maxpool_bwd(dy, idx, x_shape, dx, accumulate):
 
 
 def upcat_fwd(lo, skip):
+    """[B,2h,2w,C1+C2]: lo [B,h,w,C1] upsampled x2 (nearest), then skip [B,2h,2w,C2] on channels.  The kernel reads skip at
+    the upsampled plane's strides, so a skip of any other shape raises ValueError before anything is allocated or launched."""
     B, h, w, C1 = lo.shape
+    if skip is not None and tuple(skip.shape[:3]) != (B, 2 * h, 2 * w):
+        raise ValueError("upcat_fwd: skip is %s, the x2 upsampled %s needs [%d,%d,%d,C]"
+                         % (list(skip.shape), list(lo.shape), B, 2 * h, 2 * w))
     C2 = skip.shape[-1] if skip is not None else 0
     out = empty((B, 2 * h, 2 * w, C1 + C2), lo)
     L.launch(_lib().scsfm_upcat_fwd, "scsfm_upcat_fwd", "upcat", 1, 8.0 * out.numel(), L.ptr(lo), L.ptr(skip), B, 2 * h, 2 * w, C1, C2, L.ptr(out), L.stream())
@@ -544,9 +549,15 @@ def fold_plain(dpad, d, act_out, act, accumulate):
 
 
 def fold_upcat(dpad, C1, lo_act, act, with_skip=True):
-    """Gradient of the upsampled part (d_lo) and, with_skip, of the skip part (d_skip; None without) of a concatenation."""
+    """Gradient of the upsampled part (d_lo) and, with_skip, of the skip part (d_skip; None without) of a concatenation.
+    The plane of dpad is the concatenation's [2h,2w] padded by one on each side, h x w that of lo_act [B,h,w,C1] (upcat_fwd's
+    contract): any other shape raises ValueError before anything is allocated or launched."""
     B, Hp, Wp, Ct = dpad.shape
     H, W, C2 = Hp - 2, Wp - 2, Ct - C1
+    if tuple(lo_act.shape) != (B, H // 2, W // 2, C1) or H % 2 or W % 2:
+        raise ValueError("fold_upcat: dpad is %s, the low-resolution part %s with C1 = %d needs [%d,%d,%d,C1+C2]"
+                         % (list(dpad.shape), list(lo_act.shape), C1, lo_act.shape[0], 2 * lo_act.shape[1] + 2,
+                            2 * lo_act.shape[2] + 2))
     d_lo = empty((B, H // 2, W // 2, C1), dpad)
     d_skip = empty((B, H, W, C2), dpad) if C2 > 0 and with_skip else None
     L.launch(_lib().scsfm_fold_bwd, "scsfm_fold_bwd", "fold", 2 if d_skip is not None else 1, 4.0 * dpad.numel(), L.ptr(dpad), B, H, W, C1,

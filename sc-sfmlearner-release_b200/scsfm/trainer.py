@@ -24,7 +24,14 @@ import loss_functions as LF
 from . import nnops as O
 from .camera import _check as _check_camera_inputs, _check_theta
 from .exchange import GradExchange
-from .nets import ArenaAdam
+from .nets import ArenaAdam, check_image_size
+
+
+def _check_sizes(tgt_img, ref_imgs):
+    """The losses compare each disparity with its image pixel by pixel: refuse a size whose disparity is not the image's, or
+    that DispResNet does not take, before PoseResNet is launched on the side stream."""
+    for img in [tgt_img] + list(ref_imgs):
+        check_image_size(img.shape[-2], img.shape[-1], training_step=True)
 
 
 def compute_depth(disp_net, tgt_img, ref_imgs):
@@ -136,7 +143,9 @@ class Trainer:
         Intrinsics that require a gradient (a learned / self-calibrated K) get it in an eager single-GPU step, accumulated
         into their .grad as in the reference loop; updating them is left to the caller's own optimizer.
         With a camera the step takes `aug`, the batch's augmentation records, and no intrinsics: K is built from the camera; a bank
-        of cameras also takes `camera_index`, each sample's camera (int32 or int64 [B] on the GPU)."""
+        of cameras also takes `camera_index`, each sample's camera (int32 or int64 [B] on the GPU).
+        The images' H and W are multiples of 32, at least 64 (nets.check_image_size): else ValueError before any launch."""
+        _check_sizes(tgt_img, ref_imgs)
         intrinsics = self._camera_inputs(tgt_img, intrinsics, aug, camera_index)
         self._check_intrinsics(intrinsics)
         if self._graph is not None:
@@ -161,6 +170,7 @@ class Trainer:
         place of intrinsics (as in step()); the records (and a bank's camera index) become static buffers and the camera's theta and
         Adam state are undone too."""
         from . import lib as L
+        _check_sizes(tgt_img, ref_imgs)
         if self.exchange is not None and not allow_distributed:
             raise RuntimeError("graph capture of the data-parallel step is opt-in (allow_distributed=True): capturing the NCCL "
                                "all-reduce on the side stream has not been validated on this pod yet")
