@@ -199,7 +199,9 @@ typedef struct ScsfmConv {
     /* per-call experiment knobs (0 = the heuristics) and per-call profiling buffer: nothing in the library is
      * process-global mutable state */
     unsigned tune;
-    unsigned long long* debug;   /* device array of 8 x (number of SMs) cycle counters written by the TMA conv kernel, or NULL */
+    unsigned long long* debug;   /* device array of 8 cycle counters per CTA written by the TMA conv kernels, or NULL (forward: one
+                                    CTA per SM; the chain-drain slot and the weight gradient, whose grid can exceed the SM
+                                    count, only in a build with -DSCSFM_DRAIN_COUNTERS) */
     /* Eval-mode BatchNorm in the forward epilogue (NULL = off): z = act(fmaf(acc, bn_scale[c], bn_shift[c]) + addend), then
      * SCSFM_ROUND_TF32 if flagged -- the arithmetic of scsfm_bn_apply without batch sums, so the fused result is bitwise the
      * conv output followed by scsfm_bn_apply.  Per-output-channel [Cout] arrays from scsfm_bn_eval_prepare_batched.  Refused

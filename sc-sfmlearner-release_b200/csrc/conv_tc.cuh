@@ -8,6 +8,15 @@
 
 namespace scsfm {
 
+// Chain-drain cycle counters of the TMA convolution kernels (ScsfmConv.debug slot 3, and slots 2, 4, 7 of the weight
+// gradient): compiled in only with NVCC_EXTRA=-DSCSFM_DRAIN_COUNTERS.  Predicated off by a NULL debug pointer they still
+// cost 1.2 % of the benchmarked step (H100, tf32x3; DESIGN.md §6), so the default build leaves them out.
+#ifdef SCSFM_DRAIN_COUNTERS
+constexpr bool DRAIN_COUNTERS = true;
+#else
+constexpr bool DRAIN_COUNTERS = false;
+#endif
+
 constexpr int TBM = 128;            // pixel tile of the TMA kernel (two consumer warpgroups of 64 rows)
 constexpr int GBM = 64;             // tile rows of the cp.async gather kernels (one wgmma M = 64 warpgroup)
 constexpr int TBK = 32;             // floats per k-block = one 128-byte swizzle row

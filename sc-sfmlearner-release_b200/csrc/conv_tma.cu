@@ -76,6 +76,26 @@ struct TmaMaps {
     CUtensorMap a[4], a_lo[4], w, w_lo;
 };
 
+// The wgmma of one stage with all four K8 slices of the channel chunk: NTAP taps x 4 slices x MT sub-tiles, in the order of
+// the generic loop in conv_tma_kernel, with compile-time trip counts.  ptxas then issues them back to back; behind a loop
+// with runtime bounds it puts a warpgroup.arrive before every wgmma and gives each its own scoreboard wait.
+template <int BNW, int MT, int NTAP>
+__device__ __forceinline__ void tma_stage_chain(float (&part)[MT][BNW / 2], uint32_t x_addr, uint32_t w_addr,
+                                                const int (&shift)[TMA_MAX_KH], int TW, int wg, uint32_t scale0) {
+#pragma unroll
+    for (int j = 0; j < NTAP; ++j) {
+#pragma unroll
+        for (int q8 = 0; q8 < TBK / 8; ++q8) {
+            const uint64_t dw = tc::make_desc_sw128(w_addr + (uint32_t)(j * BNW * 128 + q8 * 32));
+#pragma unroll
+            for (int mb = 0; mb < MT; ++mb) {
+                const uint32_t a = x_addr + (uint32_t)((shift[j] * TW + 64 * (wg * MT + mb)) * 128 + q8 * 32);
+                tc::wgmma_tf32<BNW>(part[mb], tc::make_desc_sw128(a), dw, j == 0 && q8 == 0 ? scale0 : 1u);
+            }
+        }
+    }
+}
+
 // BNW: Cout tile = weight rows kept in shared memory = N of the wgmma (16/32/64/128).
 // MT: 128-pixel sub-tiles stacked vertically; each consumer warpgroup runs MT wgmma of M = 64 per K8 slice.
 template <int BNW, int MT>
@@ -177,7 +197,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMap
         uint32_t ph = 0;
         int pend = -1;
         int items = 0;                                   // work items of this CTA (debug slot 7)
-        long long t_full = 0;
+        long long t_full = 0, t_drain = 0;
         const long long t_begin = clock64();
         for (int w = blockIdx.x; w < g.num_work; w += gridDim.x, ++items) {
             int tt = w / g.n_tiles;
@@ -206,7 +226,19 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMap
 #pragma unroll
                             for (int mb = 0; mb < MT; ++mb) tc::reg_fence(part[mb]);
                             tc::wgmma_fence();
-                            for (int j = 0; j < g.box_ntap[bx]; ++j) {
+                            const int ntap = g.box_ntap[bx];
+                            if (k8 == TBK / 8) {
+                                // a whole channel chunk (every layer but a partial last chunk): the unrolled chain
+                                int shift[TMA_MAX_KH];
+#pragma unroll
+                                for (int j = 0; j < TMA_MAX_KH; ++j) shift[j] = j < ntap ? g.tap_shift[g.box_tap0[bx] + j] : 0;
+                                const uint32_t scale0 = first ? 0u : 1u;
+                                if (ntap == 1) tma_stage_chain<BNW, MT, 1>(part, x_addr, w_addr, shift, TW, wg, scale0);
+                                else if (ntap == 2) tma_stage_chain<BNW, MT, 2>(part, x_addr, w_addr, shift, TW, wg, scale0);
+                                else tma_stage_chain<BNW, MT, 3>(part, x_addr, w_addr, shift, TW, wg, scale0);
+                                first = false;
+                            } else                       // a partial last chunk: its k8 < 4 slices holding real channels
+                            for (int j = 0; j < ntap; ++j) {
                                 const int shift = g.tap_shift[g.box_tap0[bx] + j];
                                 for (int q8 = 0; q8 < k8; ++q8) {
                                     const uint64_t dw = tc::make_desc_sw128(w_addr + (uint32_t)(j * W_TILE + q8 * 32));
@@ -221,6 +253,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMap
                             tc::wgmma_commit();
                             if (g.npass > 1) {
                                 // split mode: every stage is a chain of its own (kh * k8 <= 12 wgmma), added in fp32 registers
+                                const long long t1 = DRAIN_COUNTERS && g.dbg ? clock64() : 0;
                                 tc::wgmma_wait<0>();
 #pragma unroll
                                 for (int mb = 0; mb < MT; ++mb) {
@@ -228,6 +261,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMap
 #pragma unroll
                                     for (int i = 0; i < BNW / 2; ++i) acc[mb][i] += part[mb][i];
                                 }
+                                if (DRAIN_COUNTERS && g.dbg) t_drain += clock64() - t1;
                                 tc::mbar_arrive(bar_empty + s);
                                 first = true;
                             } else {
@@ -324,6 +358,7 @@ conv_tma_kernel(ScsfmConv p, TcView v, TmaGeom g, const __grid_constant__ TmaMap
         }
         if (g.dbg && tid == 0) {
             g.dbg[blockIdx.x * 8 + 2] = (unsigned long long)t_full;
+            if (DRAIN_COUNTERS) g.dbg[blockIdx.x * 8 + 3] = (unsigned long long)t_drain;
             g.dbg[blockIdx.x * 8 + 4] = (unsigned long long)(clock64() - t_begin);
             g.dbg[blockIdx.x * 8 + 7] = (unsigned long long)items;
         }

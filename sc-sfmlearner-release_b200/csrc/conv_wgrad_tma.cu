@@ -197,11 +197,16 @@ conv_wgrad_tma_kernel(ScsfmConv p, WtGeom g, const __grid_constant__ CUtensorMap
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[dx][i] = 0.f;
     float part[BN / 2];
+    unsigned long long* dbg = DRAIN_COUNTERS ? p.debug : nullptr;   // optional per-CTA cycle counters (ScsfmConv.debug)
+    long long t_full = 0, t_drain = 0;
+    const long long t_start = DRAIN_COUNTERS ? clock64() : 0;
     for (int it = 0; it < ntile; ++it) {
         const int s = it % WT_STAGES;
         const uint32_t ph = (it / WT_STAGES) & 1;
+        const long long t0 = dbg ? clock64() : 0;
         tc::mbar_wait(bar_full + s, ph);              // the input patch (read with ld.shared)
         tc::mbar_wait(bar_ready + s, ph);             // the transposed dout (read by wgmma)
+        if (dbg) t_full += clock64() - t0;
         const uint32_t st = ring + (uint32_t)(s * Cfg::STAGE);
         const uint32_t patch = st + (uint32_t)((w >> 1) * Cfg::PATCH);
         const uint32_t bhi = st + 2 * Cfg::PATCH + (BN / 32) * Cfg::RAW, blo = bhi + Cfg::BT;
@@ -248,10 +253,12 @@ conv_wgrad_tma_kernel(ScsfmConv p, WtGeom g, const __grid_constant__ CUtensorMap
                         tc::wgmma_tf32_rs<BN>(part, ahi[j], tc::make_desc_sw128(bhi + boff), 1u);
                     }
                     tc::wgmma_commit();
+                    const long long t1 = dbg ? clock64() : 0;
                     tc::wgmma_wait<0>();
                     tc::reg_fence(part);
 #pragma unroll
                     for (int i = 0; i < BN / 2; ++i) acc[dx][i] += part[i];
+                    if (dbg) t_drain += clock64() - t1;
                 } else {
                     tc::reg_fence(acc[dx]);
                     tc::wgmma_fence();
@@ -268,6 +275,15 @@ conv_wgrad_tma_kernel(ScsfmConv p, WtGeom g, const __grid_constant__ CUtensorMap
             }
         }
         tc::mbar_arrive(bar_empty + s);
+    }
+    if (dbg && tid == 0) {
+        // slots as in conv_tma_kernel: 2 wait for a full stage, 3 chain drains (wgmma_wait), 4 consumer
+        // total, 7 tiles; one row per CTA of the (possibly larger than one wave) grid
+        const size_t cta = blockIdx.x + (size_t)gridDim.x * (blockIdx.y + (size_t)gridDim.y * blockIdx.z);
+        dbg[cta * 8 + 2] = (unsigned long long)t_full;
+        dbg[cta * 8 + 3] = (unsigned long long)t_drain;
+        dbg[cta * 8 + 4] = (unsigned long long)(clock64() - t_start);
+        dbg[cta * 8 + 7] = (unsigned long long)ntile;
     }
     // dw[o][dy][dx][c] += acc[dx][4 i + e] (row 16 w + gq + 8 (e / 2) = channel, column 8 i + 2 tq + (e % 2) = o); the
     // stem's row m = dx * Cin + c is the same offset inside dw[o][dy]

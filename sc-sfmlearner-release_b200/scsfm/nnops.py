@@ -175,7 +175,7 @@ class ConvCtx:
             raise ValueError("conv mode must be one of %s, got %r" % (MODES, mode))
         self.mode = mode
         self.tune = 0                 # ScsfmConv.tune of every call made through this context (see tune())
-        self.debug = None             # ScsfmConv.debug: uint64 tensor [8 * SMs] of per-role cycle counters, or None
+        self.debug = None             # ScsfmConv.debug: uint64 tensor [8 * CTAs] of per-role cycle counters, or None
         self._flips = {}              # (source pointer, shape, stride, pad, operand) -> (source tensor, flipped weights)
         self._plans = {}              # (pass, descriptor key) -> scsfm_conv_plan
         self._table = None

@@ -6,7 +6,9 @@ the layer shapes of DispResNet18 / PoseResNet18 at 256x832 (B = 12 stacked DispR
 
 --tune / --compare: nnops.tune() keywords (no_tma, mt, tw_log2, bn, wgrad); with --compare every layer is run in both
 configurations and the second is checked against the first.  --roles prints the TMA kernel's per-role cycle counters
-(ScsfmConv.debug).  Errors are relative L2 against an fp64 torch reference.
+(ScsfmConv.debug).  The chain-drain counter (wgmma_wait of a split-accumulate chain; the weight gradient's consumer
+counters too) is compiled in only by a build with NVCC_EXTRA=-DSCSFM_DRAIN_COUNTERS; --roles then also prints its share
+of the consumer cycles.  Errors are relative L2 against an fp64 torch reference.
 """
 import argparse
 import os
@@ -100,8 +102,9 @@ def main():
     g = torch.Generator().manual_seed(0)
     bad = 0
     totals = {(c, p): 0.0 for c, _ in cfgs for p in passes}
-    # the counters conv_tma_kernel writes per CTA (slot: meaning, in cycles); slot 7 = tiles
-    names = {0: "producer wait-empty", 1: "producer total", 2: "consumer wait-full", 4: "consumer total"}
+    # the counters the TMA kernels write per CTA (slot: meaning, in cycles; consumer slots from warpgroup 0); slot 7 = tiles.
+    # The weight-gradient kernel writes the consumer slots only.
+    names = {0: "producer wait-empty", 1: "producer total", 2: "consumer wait-full", 3: "consumer drain", 4: "consumer total"}
     for (name, B, H, W, Cin, Cout, k, s, pad, reflect) in LAYERS:
         if args.only and args.only not in name:
             continue
@@ -174,7 +177,8 @@ def main():
                     if d_.shape[0]:
                         m = d_.mean(0)
                         print("      roles (%d CTAs, %.1f tiles/CTA): " % (d_.shape[0], m[7]) +
-                              "  ".join("%s=%.0f" % (n, float(m[k])) for k, n in names.items()), flush=True)
+                              "  ".join("%s=%.0f" % (n, float(m[k])) for k, n in names.items()) +
+                              "  drain share %.1f%%" % (100.0 * float(m[3]) / max(float(m[4]), 1.0)), flush=True)
     for (c, p), t in totals.items():
         print("total %-5s %-5s %.3f ms" % (c, p, t))
     print("MISMATCHES: %d" % bad)
