@@ -199,9 +199,9 @@ typedef struct ScsfmConv {
     /* per-call experiment knobs (0 = the heuristics) and per-call profiling buffer: nothing in the library is
      * process-global mutable state */
     unsigned tune;
-    unsigned long long* debug;   /* device array of 8 cycle counters per CTA written by the TMA conv kernels, or NULL (forward: one
-                                    CTA per SM; the chain-drain slot and the weight gradient, whose grid can exceed the SM
-                                    count, only in a build with -DSCSFM_DRAIN_COUNTERS) */
+    unsigned long long* debug;   /* device array of 8 cycle counters per CTA written by the TMA conv kernels, or NULL (one
+                                    CTA per SM, slot 7 = work items or tiles of the CTA; the chain-drain slot and the weight
+                                    gradient's cycle counters only in a build with -DSCSFM_DRAIN_COUNTERS) */
     /* Eval-mode BatchNorm in the forward epilogue (NULL = off): z = act(fmaf(acc, bn_scale[c], bn_shift[c]) + addend), then
      * SCSFM_ROUND_TF32 if flagged -- the arithmetic of scsfm_bn_apply without batch sums, so the fused result is bitwise the
      * conv output followed by scsfm_bn_apply.  Per-output-channel [Cout] arrays from scsfm_bn_eval_prepare_batched.  Refused
@@ -221,6 +221,8 @@ typedef struct ScsfmConv {
 #define SCSFM_TUNE_TW(l2) (((unsigned)((l2) ? (l2) - 2 : 0) & 3u) << 6)   /* TMA kernel: tile width log2 3|4 (0 = auto) */
 #define SCSFM_TUNE_BN(bn) (((bn) == 16 ? 1u : (bn) == 32 ? 2u : (bn) == 64 ? 3u : (bn) == 128 ? 4u : 0u) << 8)  /* weight rows in smem; TMA wgrad: Cout tile 32|64 */
 #define SCSFM_TUNE_WGRAD(k) (((unsigned)(k) & 3u) << 12)     /* weight gradient: 0 auto, 1 gather kernel, 2 TMA kernel, 3 thin-layer fp32 kernel */
+#define SCSFM_TUNE_WT_TILE(tw) (((tw) == 16 ? 1u : (tw) == 8 ? 2u : 0u) << 14)   /* TMA wgrad: pixel tile 4x16 | 8x8 (0 = auto) */
+#define SCSFM_TUNE_WT_SPLIT_GRID 0x10000u                   /* TMA wgrad: one CTA per (unit, pixel split) instead of stream-K */
 
 /* ScsfmConv.mode */
 #define SCSFM_MODE_FP32 0     /* exact CUDA-core kernels */

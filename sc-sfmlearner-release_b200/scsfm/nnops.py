@@ -26,13 +26,16 @@ OPERAND_TF32, OPERAND_RAW, OPERAND_LO = 0, 1, 2      # SCSFM_OPERAND_*
 MODES = ("fp32", "tf32", "tf32x3")
 
 
-def tune(no_tma=0, mt=0, tw_log2=0, bn=0, wgrad=0):
-    """ScsfmConv.tune word (include/scsfm.h): per-call experiment knobs of the tensor-core kernels."""
+def tune(no_tma=0, mt=0, tw_log2=0, bn=0, wgrad=0, wt_tile=0, wt_split_grid=0):
+    """ScsfmConv.tune word (include/scsfm.h): per-call experiment knobs of the tensor-core kernels.  wt_tile (16: 4x16,
+    8: 8x8) and wt_split_grid (1: the split grid instead of stream-K) shape the TMA weight gradient's schedule."""
     t = 1 if no_tma else 0
     t |= (mt & 3) << 4
     t |= ((tw_log2 - 2 if tw_log2 else 0) & 3) << 6
     t |= {0: 0, 16: 1, 32: 2, 64: 3, 128: 4}[bn] << 8
     t |= (wgrad & 3) << 12
+    t |= {0: 0, 16: 1, 8: 2}[wt_tile] << 14
+    t |= 0x10000 if wt_split_grid else 0
     return t
 
 

@@ -4,8 +4,9 @@ the layer shapes of DispResNet18 / PoseResNet18 at 256x832 (B = 12 stacked DispR
     python tools/conv_layers.py [--mode tf32|tf32x3] [--pass fwd,dgrad,wgrad] [--tune key=val,...] [--compare key=val,...]
                                 [--roles] [--only substring] [--reps N]
 
---tune / --compare: nnops.tune() keywords (no_tma, mt, tw_log2, bn, wgrad); with --compare every layer is run in both
-configurations and the second is checked against the first.  --roles prints the TMA kernel's per-role cycle counters
+--tune / --compare: nnops.tune() keywords (no_tma, mt, tw_log2, bn, wgrad, wt_tile, wt_split_grid); with --compare
+every layer is run in both configurations and the second is checked against the first.  The weight-gradient pass also
+prints the TMA kernel's schedule: CTAs, tiles per CTA and the fill (useful pixels over the SM time of the busiest SM).  --roles prints the TMA kernel's per-role cycle counters
 (ScsfmConv.debug).  The chain-drain counter (wgmma_wait of a split-accumulate chain; the weight gradient's consumer
 counters too) is compiled in only by a build with NVCC_EXTRA=-DSCSFM_DRAIN_COUNTERS; --roles then also prints its share
 of the consumer cycles.  Errors are relative L2 against an fp64 torch reference.
@@ -166,6 +167,24 @@ def main():
                     bad += 1
                 print("%-18s B%-2d %3dx%-3d C%4d->%-3d k%d s%d %-5s %-5s err %.1e  %8.3f ms %7.1f TF/s%s"
                       % (name, B, H, W, Cin, Cout, k, s, p, cname, err, t, flops / t / 1e9, msg), flush=True)
+                if p == "wgrad":
+                    # the TMA weight gradient's schedule: tiles per CTA (debug slot 7) and the share of SM time spent on
+                    # real pixels, units x B Ho Wo / 64 / SMs over the busiest SM's tile-steps
+                    dbg = torch.zeros(8192 * 8, dtype=torch.int64, device="cuda")
+                    cx.debug = dbg
+                    run(p)
+                    torch.cuda.synchronize()
+                    cx.debug = None
+                    tiles = dbg.view(-1, 8)[:, 7]
+                    tiles = tiles[tiles > 0]
+                    if tiles.numel():
+                        knob = (tw >> 8) & 7                 # the Cout tile launch_conv_wgrad_tma picks
+                        bn = 32 if knob == 2 or (knob != 3 and Cout <= 32) else 64
+                        units = -(-Cin // 64) * k * -(-Cout // bn)
+                        busiest = -(-tiles.numel() // nsm) * int(tiles.max())
+                        print("      schedule: %d CTAs, tiles per CTA %d..%d, fill %.2f"
+                              % (tiles.numel(), int(tiles.min()), int(tiles.max()), units * B * Ho * Wo / 64 / nsm / busiest),
+                              flush=True)
                 if args.roles:
                     dbg = torch.zeros(8192 * 8, dtype=torch.int64, device="cuda")
                     cx.debug = dbg
