@@ -461,6 +461,55 @@ int scsfm_camera_build_indexed(const float* theta, int n_cams, const double* aug
 int scsfm_camera_grad_indexed(const double* aug, const int* idx, const float* dK, int B, int n_cams, float* dtheta,
                               void* stream);
 
+/* Dense reconstruction (run_fusion.py, scsfm/fusion.py): a truncated signed distance field on a two-level grid.
+ * The volume's box starts at lo and holds nb[0] x nb[1] x nb[2] bricks of 8^3 voxels of size `voxel`; voxel (i, j, k) has its
+ * centre at lo + (ijk + 0.5) voxel.  index [nb2][nb1][nb0] (int32, cell = (bz nb1 + by) nb0 + bx) is each cell's brick id or
+ * -1; brick b is pool[b][5][512]: tsdf, w, r, g, b (fp32), voxel (x, y, z) of the brick at x + 8 y + 64 z.  The caller owns
+ * all of it; fewer than 2^31 cells.  lo_d / voxel_d are the same box in fp64 (mesh vertices).
+ * A frame: depth [H][W] fp32, optional colour [H][W][3] uint8, intrinsics, and the pose both ways (fp32 of the fp64 host
+ * inverse): camera = R_wc world + t_wc, world = R_cw camera + t_cw, row-major.
+ * Update of a voxel by a frame: p = R_wc centre + t_wc; nothing unless z > 0; pixel (floor(fx x / z + cx + 0.5),
+ * floor(fy y / z + cy + 0.5)) inside the image with a depth d, 0 < d <= max_depth; sdf = d - z, nothing unless |sdf| <= trunc;
+ * then tsdf = (tsdf w + sdf / trunc) / (w + 1), with colour rgb = (rgb w + c) / (w + 1), w = w + 1.
+ *   scsfm_fusion_alloc: gives a brick (ids from counters[0] upwards) to every cell that a voxel the batch can update lies
+ *     in (the box of each valid pixel's footprint between depths max(d - trunc, 0) and d + trunc), and lists each such cell
+ *     once in touched[] (counters[1] counts them, entries past touched_cap are dropped): stamp [cells] (int32, zero at first)
+ *     marks the cells listed under `epoch`, a positive number new for every call.  Bricks past the pool's end are only
+ *     numbered: the caller reads counters[0] and grows the pool before integrating.
+ *   scsfm_fusion_integrate: applies the F frames in order to every voxel of the n_touched listed cells (zero-initialised
+ *     new bricks); one pass over the voxels whatever F is.
+ *   scsfm_fusion_sample: out [n][5] = the five fields of voxels ijk [n][3] (int64), zeros for voxels in no brick.
+ *   scsfm_fusion_mesh_count / _emit: marching cubes over the cells of the n_bricks bricks cells[] (the cells of allocated
+ *     bricks); a cell (the cube whose lowest corner is a voxel) is meshed when its 8 corners have w > 0, corner c inside when
+ *     tsdf < 0, triangles from tri_table [256][16] (int8 edge numbers, -1 after the last; scsfm/mc_tables.py).  _count writes
+ *     counts [n_bricks][512] (triangles per cell); _emit writes cell q's triangles from offsets[q] (int64, the exclusive scan
+ *     of counts): per triangle corner the edge key (lower voxel's linear index (k ny + j) nx + i, times 3, plus the axis),
+ *     the vertex at t = tsdf0 / (tsdf0 - tsdf1) from the lower voxel (fp64, stored fp32) and its colour rint(rgb0 + t (rgb1 -
+ *     rgb0)) clamped to uint8. */
+#define SCSFM_FUSION_MAX_FRAMES 16
+typedef struct ScsfmFusionFrame {
+    const float* depth;
+    const unsigned char* color;
+    float R_wc[9], t_wc[3], R_cw[9], t_cw[3];
+    float fx, fy, cx, cy;
+} ScsfmFusionFrame;
+typedef struct ScsfmFusionVolume {
+    double lo_d[3], voxel_d;
+    float lo[3], voxel, trunc, max_depth;
+    int nb[3];
+} ScsfmFusionVolume;
+int scsfm_fusion_alloc(const ScsfmFusionFrame* frames_host, int F, int H, int W, const ScsfmFusionVolume* vol_host, int* index,
+                       int* stamp, int epoch, int* counters, int* touched, int touched_cap, void* stream);
+int scsfm_fusion_integrate(const ScsfmFusionFrame* frames_host, int F, int H, int W, const ScsfmFusionVolume* vol_host,
+                           const int* index, const int* touched, int n_touched, float* pool, void* stream);
+int scsfm_fusion_sample(const ScsfmFusionVolume* vol_host, const int* index, const float* pool, const long long* ijk, long long n,
+                        float* out, void* stream);
+int scsfm_fusion_mesh_count(const ScsfmFusionVolume* vol_host, const int* index, const float* pool, const int* cells,
+                            int n_bricks, const signed char* tri_table, int* counts, void* stream);
+int scsfm_fusion_mesh_emit(const ScsfmFusionVolume* vol_host, const int* index, const float* pool, const int* cells,
+                           int n_bricks, const signed char* tri_table, const long long* offsets, long long* keys, float* verts,
+                           unsigned char* colors, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

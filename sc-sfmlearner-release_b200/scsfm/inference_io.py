@@ -125,6 +125,59 @@ def read_poses(path):
     return np.genfromtxt(path).astype(np.float64).reshape(-1, 3, 4)
 
 
+def odom_intrinsics(calib_path, cam, src_hw, dst_hw):
+    """K [3,3] float32 of camera `cam` (2 or 3: line P<cam> of a KITTI odometry calib.txt) for frames of size src_hw = (h, w)
+    resized to dst_hw: row 0 scaled by dst_w / w and row 1 by dst_h / h, in float32 (what the odometry training set's cam.txt
+    holds)."""
+    with open(calib_path) as f:
+        line = f.readlines()[int(cam)]
+    K = np.array(line.split()[1:]).reshape(3, 4).astype(np.float32)[0:3, 0:3]
+    K[0, :] *= dst_hw[1] / src_hw[1]
+    K[1, :] *= dst_hw[0] / src_hw[0]
+    return K
+
+
+# --- meshes ------------------------------------------------------------------------------------------------------------
+def write_ply(path, verts, faces, colors):
+    """Binary little-endian PLY: vertices float32 x y z with uint8 red green blue, faces as a uchar count and int32 indices."""
+    verts = np.ascontiguousarray(verts, dtype="<f4").reshape(-1, 3)
+    colors = np.ascontiguousarray(colors, dtype=np.uint8).reshape(-1, 3)
+    faces = np.asarray(faces).reshape(-1, 3)
+    if len(colors) != len(verts):
+        raise ValueError("%d colours for %d vertices" % (len(colors), len(verts)))
+    if len(faces) and (faces.min() < 0 or faces.max() >= len(verts) or len(verts) > 2 ** 31 - 1):
+        raise ValueError("face indices must lie in [0, %d) and fit int32" % len(verts))
+    vrec = np.empty(len(verts), dtype=[("p", "<f4", 3), ("c", "u1", 3)])
+    vrec["p"], vrec["c"] = verts, colors
+    frec = np.empty(len(faces), dtype=[("n", "u1"), ("i", "<i4", 3)])
+    frec["n"], frec["i"] = 3, faces
+    header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+              "property uchar red\nproperty uchar green\nproperty uchar blue\nelement face %d\n"
+              "property list uchar int vertex_indices\nend_header\n" % (len(verts), len(faces)))
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(vrec.tobytes())
+        f.write(frec.tobytes())
+
+
+def read_ply(path):
+    """(verts float32 [V,3], faces int64 [F,3], colors uint8 [V,3]) of a PLY written by write_ply."""
+    with open(path, "rb") as f:
+        data = f.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    counts = {}
+    for line in data[:end].decode("ascii").splitlines():
+        p = line.split()
+        if p[:1] == ["element"]:
+            counts[p[1]] = int(p[2])
+    nv, nf = counts["vertex"], counts["face"]
+    v = np.frombuffer(data, dtype=[("p", "<f4", 3), ("c", "u1", 3)], count=nv, offset=end)
+    fr = np.frombuffer(data, dtype=[("n", "u1"), ("i", "<i4", 3)], count=nf, offset=end + v.nbytes)
+    if nf and not np.all(fr["n"] == 3):
+        raise ValueError("%s: only triangle faces are read" % path)
+    return v["p"].copy(), fr["i"].astype(np.int64), v["c"].copy()
+
+
 def snippet_indices(n_imgs, seq_length=5):
     """[n_snippets, seq_length] frame indices: every target frame with (seq_length - 1) // 2 frames on each side."""
     demi = (seq_length - 1) // 2

@@ -24,6 +24,8 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 from PIL import Image
 
+from .inference_io import odom_intrinsics
+
 MIN_SPEED = 2
 
 
@@ -206,11 +208,7 @@ class KittiOdom:
             img_dir = os.path.join(drive, "image_" + c)
             ids = sorted(f.split(".")[0] for f in os.listdir(img_dir))
             h, w = _image_size(os.path.join(img_dir, ids[0] + ".png"))
-            with open(os.path.join(drive, "calib.txt")) as f:
-                line = f.readlines()[int(c)]
-            K = np.array(line.split()[1:]).reshape(3, 4).astype(np.float32)[0:3, 0:3]
-            K[0, :] *= self.w / w
-            K[1, :] *= self.h / h
+            K = odom_intrinsics(os.path.join(drive, "calib.txt"), c, (h, w), (self.h, self.w))
             scenes.append(Scene(name + "_" + c, K, [Frame(i, os.path.join(img_dir, i + ".png")) for i in ids]))
         return scenes
 
